@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py - synthesized audio samples/sec @ batch 64 + VQ-index bit-exact rate (BASELINE.json metric, config C4).
 
-    python bench.py --gpus N --steps K --warmup W [--impl b200|reference|torch_gpu] [--config c4|c2]
+    python bench.py --gpus N --steps K --warmup W [--impl b200|reference|torch_gpu] [--config c4|c2|c3]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the synthesis hot path over one batch of 64 synthetic utterances U
 (SURVEY.md §8: 64 phones, 8-s prompt -> 500 mel frames, durations forced to 8 -> 512 mel
@@ -24,8 +25,13 @@ Arms:  --impl b200       the product (this repo's CUDA path)                    
        --config c2       BASELINE config 2: STFT+mel kernel over 10k synthetic 16 kHz 3-s clips (HBM roofline)
        --config c3       BASELINE config 3: PLM autoregressive decode, 512 prosody tokens, batch 16 (reference-faithful)
 
-Output: ONE JSON line (contract in the task statement) with `roofline`, `cpu_baseline`, `e2e`, `clocks`,
-`gpu_launches` and the parity half of the metric: `vq_index_bit_exact_rate`, `duration_exact_rate`, `mel_l1`.
+Output: ONE JSON line with `roofline`, `cpu_baseline`, `e2e`, `clocks`, `gpu_launches` and the parity half of the
+metric: `vq_index_bit_exact_rate`, `duration_exact_rate`, `mel_l1`.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller as DIR/<name>.npy
+(float32, or float64 for integer ids), at most 64 MB in all: the waveforms of a fixed, seeded sample of the batch (C4),
+the mel spectrograms of a fixed sample of the clips (C2), the prosody ids (C3).  Inputs and weights are pure functions of
+fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -50,9 +56,10 @@ METRIC = "synthesized_audio_samples_per_sec_batch64"
 UNIT = "samples/s"
 SEED0 = 1234
 THREADS_PER_WORKER = 16                               # the CPU arm: concurrent batch-1 workers of this many torch threads
-MAX_WORKERS = 4                                       # (measured on the 128-cpu GPU box, profiles/r2b_cpu_arm_sweep.log: the batch-1
-#                                                       AR loops stream 0.7 GB of weights per step and are memory-bound - 4 x 16
-#                                                       threads is the fastest split; 16 x 8 is 4 % slower, 1 x 64 is 2x slower)
+MAX_WORKERS = 4                                       # (the batch-1 AR loops stream 0.7 GB of weights per step and are
+#                                                       memory-bound: a few wide workers beat many narrow ones)
+DUMP_SEED = 4321                                      # --dump-outputs: the seeded sample of the batch that is written
+DUMP_UTTS = 16
 
 
 def parse():
@@ -69,7 +76,29 @@ def parse():
     ap.add_argument("--cpu-workers", type=int, default=0, help="concurrent batch-1 CPU workers (0 = cpus / 16, at most 4)")
     ap.add_argument("--cpu-threads", type=int, default=0, help="torch threads per CPU worker (0 = 16)")
     ap.add_argument("--clips", type=int, default=10000, help="--config c2: number of 3-s clips")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     return ap.parse_args()
+
+
+def dump_outputs(d, arrays):
+    """arrays: name -> tensor; written as DIR/<name>.npy, integer tensors as float64 (exact), the rest as float32"""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        a = t.double().numpy() if not (t.is_floating_point() or t.is_complex()) else t.float().numpy()
+        total += a.nbytes
+        assert total <= 64 << 20, "--dump-outputs: more than 64 MB"
+        np.save(os.path.join(d, name + ".npy"), a)
+    log(f"dumped {', '.join(arrays)} to {d} ({total / 2**20:.1f} MiB)")
+
+
+def dump_sample(n, k, seed=DUMP_SEED):
+    """a fixed, seeded choice of min(n, k) of n rows, in increasing order"""
+    g = torch.Generator().manual_seed(seed)
+    return torch.randperm(n, generator=g)[:min(n, k)].sort().values
 
 
 def log(*a):
@@ -82,7 +111,8 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 - never reached, a ceiling
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -261,7 +291,7 @@ def run_b200(args):
     lo, hi = sharding.shard_bounds(world * B, world)[rank]            # this rank's slice of the global batch
     wav_h, phone_h, forced = make_inputs(range(lo, hi))
     wav_d, phone_d, forced_d = wav_h.to(dev), phone_h.to(dev), forced.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
     n_out = 256 * (TP * DUR + 10) + (256 * (TM_FRAMES + 10) if revocode else 0)
     out_h = torch.empty(B, 1, n_out, dtype=torch.float32).pin_memory()
     lib = L.lib()
@@ -273,7 +303,7 @@ def run_b200(args):
 
     # ---- set-up passes (untimed, not counted as warm-up): the first builds the packed-weight plans and grows the
     # workspace, the second captures the AR drivers' CUDA graphs, and the two after a capture still show one-off host-side
-    # costs of the first replays (measured: profiles/r2j2_stage_times_6_passes.log)
+    # costs of the first replays
     from megatts2_b200 import graphs
     for _ in range(4 if graphs.enabled() else 1):
         out = gpu_step(tts, wav_d, phone_d, forced_d, revocode)
@@ -316,6 +346,9 @@ def run_b200(args):
     barrier()
     ms_e2e = f0.elapsed_time(f1)
     log(f"e2e region: {ms_e2e / args.steps:.1f} ms/step")
+    if args.dump_outputs and rank == 0:         # the waveforms the last timed step returned (global utterance indices alongside)
+        pick = dump_sample(out.shape[0], DUMP_UTTS).to(out.device)
+        dump_outputs(args.dump_outputs, {"wav": out.index_select(0, pick), "wav_rows": pick + lo})
 
     if dist is not None:
         t = torch.tensor([ms, ms_e2e], device=dev)
@@ -371,17 +404,16 @@ def run_b200(args):
                     "achieved_tflops": round(fl_ / (ms_ / 1e3) / 1e12, 2) if ms_ > 0 else 0.0,
                     "share_of_step": round(ms_ / step_ms, 3)}
         classes = {"fp32_ffma_tapconv_kernel": cls(sp[0], sp[1], sp[2]),
-                   "tcgen05_tap_gemm_kernels (incl. their activation-split kernels)": cls(sp[3], sp[4], sp[5])}
+                   "wgmma_tap_gemm_kernels (incl. their activation-split kernels)": cls(sp[3], sp[4], sp[5])}
         dom_tc = sp[3] >= sp[0]
         d_ms, d_fl = (sp[3], sp[4]) if dom_tc else (sp[0], sp[1])
         achieved = d_fl / (d_ms / 1e3) / 1e12 if d_ms > 0 else 0.0
-        traffic, traffic_note = measured_traffic()
         roofline = {"bound": "tensor",
-                    "kernel": (f"conv_tc_kernel (tcgen05 tap-GEMM: every Linear / Conv1d / ConvTranspose1d; operands {scheme}; "
-                               "single-CTA and cta_group::2 pair variants)" if dom_tc else "tapconv_kernel (fp32 FFMA tap-GEMM)"),
+                    "kernel": (f"conv_tc_kernel (wgmma tap-GEMM: every Linear / Conv1d / ConvTranspose1d; operands {scheme})"
+                               if dom_tc else "tapconv_kernel (fp32 FFMA tap-GEMM)"),
                     "achieved": round(achieved, 3), "peak": peak, "unit": "TFLOP/s", "frac": round(achieved / peak, 5),
-                    "traffic": traffic, "traffic_note": traffic_note,
-                    "peak_source": f"{pk_src} dense bf16 (sustained). achieved = algorithmic fp32-grade FLOPs (2*M*N*K) / CUDA-event "
+                    "traffic": None, "traffic_note": "not measured",
+                    "peak_source": f"{pk_src} dense bf16. achieved = algorithmic fp32-grade FLOPs (2*M*N*K) / CUDA-event "
                                    f"time of the launches; the {scheme.split(' ')[0]} scheme issues {mma_per_product} 16-bit MMAs per such "
                                    f"FLOP pair, so its ceiling is peak/{mma_per_product}",
                     "frac_of_scheme_ceiling": round(achieved / (peak / mma_per_product), 4) if dom_tc and mma_per_product else None,
@@ -396,7 +428,7 @@ def run_b200(args):
                                    f"batch {B} synthetic utterances per GPU (64 phones, 500-frame prompt, "
                                    "512 mel frames, 64 prosody tokens, 131072 counted samples each)",
                        "global_batch": world * B, "parallelism": f"replicas x{world} (batch split, no data-path collective)",
-                       "l2": "256 MiB flush write between timed iterations; working set (1.57 GB weights) >> 126 MB L2",
+                       "l2": "256 MiB flush write between timed iterations; working set (1.57 GB weights) >> 50 MB L2",
                        "weights": "seeded random init of the reference architecture", "ar_semantics": "reference-faithful "
                        "non-causal full recompute per step (models/megatts2.py:165-181, 257-275)",
                        "tensor_core_operands": scheme,
@@ -406,6 +438,7 @@ def run_b200(args):
                     "h2d_bytes_per_step": world * (wav_h.numel() * 4 + phone_h.numel() * 8),
                     "d2h_bytes_per_step": world * out_h.numel() * 4},
             "gpu_launches": int(launches),
+            "gpu": torch.cuda.get_device_name(dev),
             "hbm_peak_bytes": int(torch.cuda.max_memory_allocated(dev)),
             "clocks": clocks,
             "roofline": roofline,
@@ -419,27 +452,6 @@ def run_b200(args):
         dist.barrier()
         dist.destroy_process_group()
     return result
-
-
-def measured_traffic():
-    """dram__bytes_read + dram__bytes_write per launch of the dominant kernel class, from the committed ncu capture of
-    this command (tools/summarize_ncu.py -> profiles/r2_traffic.json); null until a capture exists."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if not os.path.exists(p):
-        return None, "no ncu capture committed yet"
-    with open(p) as f:
-        d = json.load(f)
-    return d.get("dominant_kernel_dram_bytes_per_launch"), d.get("note", "profiles/r2_traffic.json")
-
-
-def mel_traffic(args):
-    """Measured DRAM bytes of one mel_kernel launch on config C2 (ncu capture committed under profiles/); only valid for the
-    default 10 000 clips."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if args.clips != 10000 or not os.path.exists(p):
-        return None
-    with open(p) as f:
-        return json.load(f).get("mel_kernel_dram_bytes_per_launch")
 
 
 def cpu_check(args, gpu, lo, revocode):
@@ -580,7 +592,7 @@ def run_torch_gpu(args):
 
 # ------------------------------------------------------------------------------------------ config C2 (mel front end)
 def run_c2(args):
-    """BASELINE config 2: the STFT + mel-filterbank kernel over `clips` synthetic 16 kHz 3-s clips on one B200, against
+    """BASELINE config 2: the STFT + mel-filterbank kernel over `clips` synthetic 16 kHz 3-s clips on one GPU, against
     the HBM roofline (algorithmic bytes = 48000*4 in + 188*80*4 out = 252,160 B per clip, SURVEY.md 8d)."""
     from megatts2_b200 import ops
     from megatts2_b200.modules.tokenizer import extract_mel_spec
@@ -605,6 +617,9 @@ def run_c2(args):
     clocks = sampler.stop()
     ms = e0.elapsed_time(e1) / args.steps
     launches = ops.launch_count() - n0
+    if args.dump_outputs:
+        pick = dump_sample(mel.shape[0], 256).to(mel.device)
+        dump_outputs(args.dump_outputs, {"mel": mel.index_select(0, pick), "mel_rows": pick})
     out_h = torch.empty(mel.shape, dtype=torch.float32).pin_memory()
     f0, f1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     f0.record()
@@ -632,19 +647,19 @@ def run_c2(args):
             "warmup": args.warmup, "ms_per_step": round(ms, 4), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": f"C2: STFT (1024/256, periodic Hann, reflect) + 80-bin slaney mel + log over {n} clips of 3 s @ 16 kHz",
-                       "l2": "input 1.92 GB + output 0.60 GB per step >> 126 MB L2"},
+                       "l2": "input 1.92 GB + output 0.60 GB per step >> 50 MB L2"},
             "e2e": {"value": round(n / (ms_e2e / 1e3), 1), "unit": "clips/s", "h2d_bytes_per_step": n * Ls * 4,
                     "d2h_bytes_per_step": int(mel.numel()) * 4},
             "gpu_launches": int(launches), "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "mel_kernel", "achieved": round(gbs, 1), "peak": pk["hbm_gbs"], "unit": "GB/s",
-                         "frac": round(gbs / pk["hbm_gbs"], 4), "traffic": mel_traffic(args), "peak_source": pk_src,
+                         "frac": round(gbs / pk["hbm_gbs"], 4), "traffic": None, "peak_source": pk_src,
                          "algorithmic_bytes_per_clip": bytes_per_clip},
             "cpu_baseline": cpu}
 
 # ------------------------------------------------------------------------------------------ config C3 (PLM decode, T = 512)
 def run_c3(args):
     """BASELINE config 3: MegaPLM.infer - the reference-faithful NON-causal full-recompute greedy decode
-    (models/megatts2.py:165-181) - of 512 prosody tokens at batch 16 on one B200.  A step = one whole decode.
+    (models/megatts2.py:165-181) - of 512 prosody tokens at batch 16 on one GPU.  A step = one whole decode.
     Parity: at sampled steps t the oracle's last-row logits for the GPU's own prefix must pick the GPU's id (a greedy decode
     is exactly the sequence for which that holds at every step)."""
     import ctypes as C
@@ -662,7 +677,7 @@ def run_c3(args):
     for _ in range(max(1, min(args.warmup, 2))):
         ids = tts.plm.infer(tc)
     torch.cuda.synchronize()
-    steps = max(1, min(args.steps, 5))
+    steps = max(1, args.steps)
     n0 = ops.launch_count()
     sampler = ClockSampler(0)
     sampler.start()
@@ -675,6 +690,8 @@ def run_c3(args):
     clocks = sampler.stop()
     ms = e0.elapsed_time(e1) / steps
     launches = ops.launch_count() - n0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"ids": ids})
     ids_h = torch.empty(B, T, dtype=torch.int64).pin_memory()
     f0, f1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     f0.record()
@@ -732,7 +749,7 @@ def run_c3(args):
             "config": {"workload": "C3: MegaPLM.infer, 512 prosody tokens, batch 16: non-causal full recompute per step as the "
                                    "reference does (the final layer's out-projection / FFN for the last row only, the only "
                                    "row consumed)",
-                       "l2": "weights 0.6 GB + activations per step >> 126 MB L2", "weights": "seeded random init",
+                       "l2": "weights 0.6 GB + activations per step >> 50 MB L2", "weights": "seeded random init",
                        "causal_kv_cache_decode_ms": round(c0.elapsed_time(c1), 2)},
             "e2e": {"value": round(B * T / (ms_e2e / 1e3), 1), "unit": "tokens/s", "h2d_bytes_per_step": int(tc_h.numel()) * 4,
                     "d2h_bytes_per_step": B * T * 8},

@@ -1,5 +1,5 @@
 /*
- * megatts2_b200.h - C ABI of libmegatts2_b200.so (sm_100a).
+ * megatts2_b200.h - C ABI of libmegatts2_b200.so (sm_90a).
  *
  * The reference (LSimon95/megatts2 @ 2ab81a1) has no FFI layer: its replaceable surface
  * is the Python nn.Module API (SURVEY.md §8b).  This library is what those modules bind
@@ -64,16 +64,16 @@ int mtts_tc_overflow_bind(int32_t* flag_dev);
  * size their grids from it, so work enqueued on two streams can share the device (the prompt re-vocode of Megatts.forward
  * runs beside the latency-bound AR loops). */
 int mtts_set_sm_limit(int32_t n_sms);
-/* Launch policy of the calling host thread while two streams share the device: SM budget (as above), whether the dense
- * layers may run as CTA pairs (cta_group::2 clusters need two free SMs of one TPC), and whether launches carry the
+/* Launch policy of the calling host thread while two streams share the device: SM budget (as above), allow_pairs (kept for
+ * ABI compatibility: the sm_90 tap-GEMM launches single CTAs only), and whether launches carry the
  * programmatic-dependent-launch attribute (a long kernel's successor would otherwise be scheduled early onto the SMs left
  * free for the other stream).  (0, 1, 1) restores the defaults.  Megatts.synthesize uses it to re-vocode the prompt
  * (models/megatts2.py:371-372 of the reference) beside the MRTE + ADM stages. */
 int mtts_set_launch_policy(int32_t sm_limit, int32_t allow_pairs, int32_t allow_pdl);
 /* Diagnostics (host only, no CUDA call): the launch plan the tap-GEMM dispatcher picks for a stride-1 layer of this shape
  * (B x T output rows, k taps) on n_sms SMs, with partial_bytes of split-K partial-sum space and, if ln_rides, a LayerNorm
- * that the split's reduction can carry.  out5 = {N-tile width, K splits, CTA pair, halo form (0 | 1 | 2 = as a pair),
- * K-slab bytes}. */
+ * that the split's reduction can carry.  out5 = {N-tile width, K splits, CTA pair (always 0),
+ * halo form (0 | 1), K-slab bytes}. */
 int mtts_tc_plan_query(int32_t n_sms, int32_t B, int32_t T, int32_t Cin, int32_t Cout, int32_t k, int32_t dil, int32_t fmt,
                        int64_t partial_bytes, int32_t ln_rides, int32_t* out5);
 
@@ -136,8 +136,8 @@ typedef struct {
 
 int mtts_conv1d_f32(const mtts_conv_params* p, void* stream);
 
-/* Tensor-core linear layer (tcgen05, sm_100a): Y[M,N] = post(pre(X)[M,K] . W[N,K]^T + bias) (+ R) with
- * fp32-grade accuracy from split operands (fp32 accumulation in TMEM).  w_planes: (3, N, K) bf16 [BF16X3] or
+/* Tensor-core linear layer (wgmma, sm_90a): Y[M,N] = post(pre(X)[M,K] . W[N,K]^T + bias) (+ R) with
+ * fp32-grade accuracy from split operands (fp32 accumulation in registers).  w_planes: (3, N, K) bf16 [BF16X3] or
  * (2, N, K) fp16 [F16X2] row-major; scratch receives the activation planes
  * (mtts_linear_tc_scratch_bytes(rows_cap, K), rows_cap >= M).  K %% 8 == 0. */
 int64_t mtts_linear_tc_scratch_bytes(int64_t rows_cap, int32_t K);
@@ -176,7 +176,7 @@ typedef struct {
 } mtts_attn_params;
 int mtts_attention_f32(const mtts_attn_params* p, void* stream);
 /* Opt-in: AR-step attention (Tq == Tk <= 64, even head count, dh 64 | 96) with at least `min_len` rows runs on the
- * two-heads-per-CTA tcgen05 kernel instead of the fp32 kernel; min_len <= 0 switches it off (the default: it is slower
+ * tensor-core kernel (one 64-row tile per head) instead of the fp32 kernel; min_len <= 0 switches it off (the default: it is slower
  * inside the synthesis step, see csrc/ops.cu).  Returns the previous setting. */
 int mtts_set_attention_pair_min(int32_t min_len);
 
@@ -337,7 +337,7 @@ typedef struct {
 
 typedef struct {
   int32_t n_layers, d_model, n_heads, ff_dim, conv_ff;
-  int32_t engine;                      /* 0: fp32 FFMA everywhere; tcgen05 for GEMMs with M >= 128: 1 = BF16X3, 2 = F16X2 operands */
+  int32_t engine;                      /* 0: fp32 FFMA everywhere; wgmma for GEMMs with M >= 128: 1 = BF16X3, 2 = F16X2 operands */
   const mtts_encoder_layer* layers;    /* HOST array of n_layers entries */
 } mtts_encoder;
 
@@ -399,7 +399,7 @@ typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv
 
 typedef struct {
   int32_t in_channels, out_channels, hidden, k, n_stacks, n_blocks;
-  int32_t engine;                      /* 0: fp32 FFMA; tcgen05 for the eligible convs: 1 = BF16X3, 2 = F16X2 */
+  int32_t engine;                      /* 0: fp32 FFMA; wgmma for the eligible convs: 1 = BF16X3, 2 = F16X2 */
   const float *w_first, *b_first;      /* packed (k, Cin, hidden) */
   const float *w_last, *b_last;        /* packed (k, hidden, Cout) */
   const mtts_conv_block* blocks;       /* HOST array [n_stacks*n_blocks] */

@@ -1,4 +1,4 @@
-"""megatts2_b200: B200-native (sm_100a) implementation of the Mega-TTS 2 synthesis hot path.
+"""megatts2_b200: H100-native (sm_90a) implementation of the Mega-TTS 2 synthesis hot path.
 
 Drop-in surface = the reference's nn.Module API (LSimon95/megatts2, SURVEY.md §8b):
 ``megatts2_b200.modules.{transformer,convnet,mrte,vqpe,embedding,tokenizer,quantization}``

@@ -4,7 +4,7 @@ these ``torch.autograd.Function``s, so ``MegaPLMTrainer`` / ``MegaADMTrainer.tra
 libmegatts2_b200.  torch supplies the tape, the loss and the optimiser; every contraction, normalisation, softmax and
 scatter of both passes is a hand-written kernel:
 
-* dense layers: forward ``x W^T`` and backward ``dX = dY W``, ``dW = dY^T X`` on the tcgen05 tap-GEMM (f16x2 operands: the
+* dense layers: forward ``x W^T`` and backward ``dX = dY W``, ``dW = dY^T X`` on the wgmma tap-GEMM (f16x2 operands: the
   gradients are fp32-grade, tighter than the bf16 autocast the reference trains under) - shapes the engine does not take
   (K = 1 embeddings of the ADM, fewer than 128 rows, ragged row counts) go to the strided fp32 batched matmul;
 * attention: unfused for training (the dropout inside ``F.scaled_dot_product_attention`` needs the probabilities):

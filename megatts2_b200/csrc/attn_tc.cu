@@ -1,20 +1,20 @@
-// Tensor-core attention (tcgen05): softmax(Q K^T * scale + mask) V with fp32-grade accuracy from f16x2 split operands
+// Tensor-core attention (wgmma): softmax(Q K^T * scale + mask) V with fp32-grade accuracy from f16x2 split operands
 // (kernels.h: x = x1 + x2' * 2^-11, three MMAs per product: x1*y1 | x1*y2' + x2'*y1, the correction accumulator scaled by
 // 2^-11 when it is read back).  Replaces F.scaled_dot_product_attention at modules/transformer.py:52-53 for the head dims
-// of the autoregressive stacks (PLM: 16 x 64, ADM: 8 x 96) whenever the sequence is long enough to feed a 128-row MMA.
+// of the autoregressive stacks (PLM: 16 x 64, ADM: 8 x 96).
 //
-// One CTA = one (batch item, head, 128-query tile), 128 threads, thread r owns query row r == TMEM lane r:
-//   stage   Q (128 x dh) once, then per 64-key tile K (64 x dh) and V^T (dh x 64): fp32 global -> f16x2 planes in shared
-//           memory, written directly in the UMMA K-major 64-byte-swizzle layout (what a TMA load with SWIZZLE_64B would
+// One CTA = one warpgroup (128 threads) = one (batch item, head, 64-query tile); the accumulators live in registers in the
+// wgmma fragment layout (tc_ptx.cuh), so the four lanes of a quad share a query row:
+//   stage   Q (64 x dh) once, then per 64-key tile K (64 x dh) and V^T (dh x 64): fp32 global -> f16x2 planes in shared
+//           memory, written directly in the K-major 64-byte-swizzle layout (what a TMA load with SWIZZLE_64B would
 //           produce: 16-byte chunk c of row r lands at chunk c ^ ((r >> 1) & 3)); fence.proxy.async hands them to the MMA
-//   S       one elected thread issues 3 * dh/16 MMAs (M 128, N 64) into two TMEM accumulators (main | correction)
-//   softmax each thread reads ITS row of S from TMEM (tcgen05.ld 32x32b), scales, masks, keeps the running max / sum of
-//           the online softmax in registers - no shuffles, no shared memory - and writes P (unnormalised, f16x2 planes)
-//           as the A operand of the second product
-//   O       3 * 4 MMAs (M 128, N dh, K 64 keys) into the SAME TMEM columns (S is dead by then); the tile's result is read
-//           back and folded into the row's fp32 accumulator with the usual exp(m_old - m_new) rescale
-//   out     acc / l  ->  fp32 rows and / or operand planes (bf16x3 | f16x2) for the out-projection GEMM
-// Shared memory: 96 KB (dh 64) / 128 KB (dh 96) / 160 KB (dh 128); TMEM: 128 / 256 / 256 columns.
+//   S       3 * dh/16 MMAs (M 64, N 64) into two register accumulators (main | correction)
+//   softmax scale, mask, running max / sum of the online softmax per row (quad shuffles), P (unnormalised, f16x2 planes)
+//           written to shared memory as the A operand of the second product
+//   O       3 * 4 MMAs (M 64, N dh, K 64 keys) accumulated into the output accumulators, which are rescaled by
+//           exp(m_old - m_new) first
+//   out     (main + correction) / l  ->  fp32 rows and / or operand planes (bf16x3 | f16x2) for the out-projection GEMM
+// Shared memory: 64 KB (dh 64) / 88 KB (dh 96) / 112 KB (dh 128).
 #include "kernels.h"
 #include "tc_ptx.cuh"
 
@@ -23,8 +23,7 @@ namespace mtts {
 namespace {
 
 constexpr int ATC_NK = 64;     // keys per tile
-
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+constexpr int ATC_NQ = 64;     // queries per CTA
 
 // 8 consecutive fp32 values -> one 16-byte chunk per f16x2 plane
 __device__ __forceinline__ void split8_f16x2(const float* v, uint4& p0, uint4& p1, bool& bad) {
@@ -54,14 +53,13 @@ __device__ __forceinline__ uint32_t sw64_off(int r, int c) { return (uint32_t)r 
 template <int DH>
 struct AtcCfg {
   static constexpr int NS = DH / 32;                      // 32-element (64-byte) K-slabs along dh
-  static constexpr int Q_SLAB = 128 * 64;                 // bytes: 128 rows x 64 B
+  static constexpr int Q_SLAB = ATC_NQ * 64;              // bytes: 64 rows x 64 B
   static constexpr int K_SLAB = ATC_NK * 64;
   static constexpr int V_SLAB = DH * 64;                  // V^T: dh rows, one slab per 32 keys
-  static constexpr int P_SLAB = 128 * 64;
+  static constexpr int P_SLAB = ATC_NQ * 64;
   static constexpr int Q_PLANE = NS * Q_SLAB, K_PLANE = NS * K_SLAB, V_PLANE = 2 * V_SLAB, P_PLANE = 2 * P_SLAB;
   static constexpr int OFF_Q = 0, OFF_K = OFF_Q + 2 * Q_PLANE, OFF_V = OFF_K + 2 * K_PLANE, OFF_P = OFF_V + 2 * V_PLANE;
-  static constexpr int SMEM = OFF_P + 2 * P_PLANE + 1024 + 64;      // + alignment slack + barrier / TMEM slot
-  static constexpr int TMEM_COLS = (2 * DH > 128) ? 256 : 128;      // max(2 * 64 for S, 2 * dh for O), power of two
+  static constexpr int SMEM = OFF_P + 2 * P_PLANE + 1024;      // + alignment slack
 };
 
 template <int DH>
@@ -72,65 +70,59 @@ attn_tc_kernel(const mtts_attn_params p, int32_t* ovf) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t bar = base + Cfg::OFF_P + 2 * Cfg::P_PLANE;
-  const uint32_t tmem_slot = bar + 16;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(sm + Cfg::OFF_P + 2 * Cfg::P_PLANE + 16);
 
   const int tid = threadIdx.x;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);        // warp-uniform for the compiler (uniform-register MMA operands)
-  const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
-  const int qrow = q0 + tid;
-  const bool qvalid = qrow < p.Tq;
-
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(Cfg::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  const int warp = tid >> 5, lane = tid & 31;
+  const int q0 = blockIdx.x * ATC_NQ, h = blockIdx.y, b = blockIdx.z;
+  // fragment rows of this thread: r0 = 16 warp + lane / 4 and r0 + 8; fragment columns 8 j + 2 (lane % 4) + {0, 1}
+  const int r0 = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
+  int qrow[2];
+  bool qvalid[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    qrow[i] = q0 + r0 + 8 * i;
+    qvalid[i] = qrow[i] < p.Tq;
   }
 
   pdl_wait();
   bool bad = false;
-  // ---- stage Q: thread r splits its own row (rows past Tq are zero)
+  // ---- stage Q (two threads per query row; rows past Tq are zero)
   {
-    const float* src = p.q + (int64_t)b * p.q_sb + (int64_t)(qvalid ? qrow : 0) * p.q_st + (int64_t)h * DH;
+    const int row = tid >> 1, half = tid & 1;
+    const bool valid = q0 + row < p.Tq;
+    const float* src = p.q + (int64_t)b * p.q_sb + (int64_t)(valid ? q0 + row : 0) * p.q_st + (int64_t)h * DH + half * (DH / 2);
 #pragma unroll
-    for (int c8 = 0; c8 < DH / 8; ++c8) {
+    for (int i = 0; i < DH / 16; ++i) {
       float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if (qvalid) {
-        const float4 a = *reinterpret_cast<const float4*>(src + c8 * 8);
-        const float4 c = *reinterpret_cast<const float4*>(src + c8 * 8 + 4);
+      if (valid) {
+        const float4 a = *reinterpret_cast<const float4*>(src + i * 8);
+        const float4 c = *reinterpret_cast<const float4*>(src + i * 8 + 4);
         v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = c.x; v[5] = c.y; v[6] = c.z; v[7] = c.w;
       }
       uint4 p0, p1;
       split8_f16x2(v, p0, p1, bad);
-      const uint32_t off = (uint32_t)(c8 >> 2) * Cfg::Q_SLAB + sw64_off(tid, c8 & 3);
+      const int c8 = half * (DH / 16) + i;
+      const uint32_t off = (uint32_t)(c8 >> 2) * Cfg::Q_SLAB + sw64_off(row, c8 & 3);
       *reinterpret_cast<uint4*>(sm + Cfg::OFF_Q + off) = p0;
       *reinterpret_cast<uint4*>(sm + Cfg::OFF_Q + Cfg::Q_PLANE + off) = p1;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot_ptr, 0);
-  const uint32_t leader = (warp == 0 && elect_one()) ? 1u : 0u;
-  const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);      // this warp's TMEM lane quarter
 
-  float m_run = -INFINITY, l_run = 0.f;
-  float acc[DH];
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};    // l_run: this thread's share of the row sum
+  float om[DH / 2], oc[DH / 2];                                       // O accumulators: main | correction
 #pragma unroll
-  for (int d = 0; d < DH; ++d) acc[d] = 0.f;
-  const float* mrow = p.mask ? p.mask + (int64_t)b * p.mask_sb + (int64_t)h * p.mask_sh + (int64_t)(qvalid ? qrow : 0) * p.mask_sq : nullptr;
+  for (int d = 0; d < DH / 2; ++d) { om[d] = 0.f; oc[d] = 0.f; }
+  const float* mrow[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+    mrow[i] = p.mask ? p.mask + (int64_t)b * p.mask_sb + (int64_t)h * p.mask_sh + (int64_t)(qvalid[i] ? qrow[i] : 0) * p.mask_sq
+                     : nullptr;
   const float* kb = p.k + (int64_t)b * p.k_sb + (int64_t)h * DH;
   const float* vb = p.v + (int64_t)b * p.v_sb + (int64_t)h * DH;
-  const uint64_t desc_hi = umma_desc_kmajor<64>(0u);
-  constexpr uint32_t IDESC_S = (1u << 4) | ((uint32_t)(ATC_NK >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // f16 x f16 -> f32
-  constexpr uint32_t IDESC_O = (1u << 4) | ((uint32_t)(DH >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  uint32_t phase = 0;
+  const uint64_t desc_hi = wgmma_desc<64>(0u);
 
   for (int k0 = 0; k0 < p.Tk; k0 += ATC_NK) {
+    __syncthreads();         // the previous tile's MMAs (which read K, V and P) have retired in every warp
     // ---- stage the K tile (two threads per key row) and the V^T tile (lanes = consecutive keys, so that a warp fills
     //      one 64-byte row of V^T with 2-byte stores); keys past Tk are zero
     {
@@ -177,123 +169,132 @@ attn_tc_kernel(const mtts_attn_params p, int32_t* ovf) {
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();       // every thread's TMEM reads of the previous tile (O) are complete before the MMAs overwrite it
     __syncthreads();
-    // ---- S = Q K^T   (warp 0 walks the issue loop uniformly; its elected lane executes the MMAs)
-    if (warp == 0) {
-      tc_fence_after();
+    // ---- S = Q K^T
+    float sm_[ATC_NK / 2], sc_[ATC_NK / 2];
+    wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < DH / 16; ++ks) {
-        const uint32_t qa = base + Cfg::OFF_Q + (ks >> 1) * Cfg::Q_SLAB + (ks & 1) * 32;
-        const uint32_t ka = base + Cfg::OFF_K + (ks >> 1) * Cfg::K_SLAB + (ks & 1) * 32;
-        const uint64_t a1 = desc_hi | (uint64_t)((qa >> 4) & 0x3FFF), a2 = desc_hi | (uint64_t)(((qa + Cfg::Q_PLANE) >> 4) & 0x3FFF);
-        const uint64_t b1 = desc_hi | (uint64_t)((ka >> 4) & 0x3FFF), b2 = desc_hi | (uint64_t)(((ka + Cfg::K_PLANE) >> 4) & 0x3FFF);
-        tc_mma_l(tmem + ATC_NK, a1, b2, IDESC_S, ks ? 1u : 0u, leader);      // correction: q1 k2' + q2' k1
-        tc_mma_l(tmem + ATC_NK, a2, b1, IDESC_S, 1u, leader);
-        tc_mma_l(tmem, a1, b1, IDESC_S, ks ? 1u : 0u, leader);               // main: q1 k1
+    for (int ks = 0; ks < DH / 16; ++ks) {
+      const uint32_t qa = base + Cfg::OFF_Q + (ks >> 1) * Cfg::Q_SLAB + (ks & 1) * 32;
+      const uint32_t ka = base + Cfg::OFF_K + (ks >> 1) * Cfg::K_SLAB + (ks & 1) * 32;
+      const uint64_t a1 = desc_hi | (uint64_t)((qa >> 4) & 0x3FFF), a2 = desc_hi | (uint64_t)(((qa + Cfg::Q_PLANE) >> 4) & 0x3FFF);
+      const uint64_t b1 = desc_hi | (uint64_t)((ka >> 4) & 0x3FFF), b2 = desc_hi | (uint64_t)(((ka + Cfg::K_PLANE) >> 4) & 0x3FFF);
+      Wgmma<ATC_NK>::template mma<false>(sc_, a1, b2, ks ? 1u : 0u);      // correction: q1 k2' + q2' k1
+      Wgmma<ATC_NK>::template mma<false>(sc_, a2, b1, 1u);
+      Wgmma<ATC_NK>::template mma<false>(sm_, a1, b1, ks ? 1u : 0u);      // main: q1 k1
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sm_);
+    wgmma_fence_regs(sc_);
+    // ---- online softmax on this thread's two rows (a row is spread over the four lanes of a quad)
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float tmax = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < ATC_NK / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = 4 * j + 2 * i + e, key = k0 + 8 * j + cq + e;
+          float x = fmaf(sc_[r], F16X2_INV_SCALE, sm_[r]) * p.scale;
+          if (mrow[i] && key < p.Tk) x += mrow[i][key];
+          x = key < p.Tk ? x : -INFINITY;
+          sm_[r] = x;
+          tmax = fmaxf(tmax, x);
+        }
       }
-      tc_commit_l(bar, leader);
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+      const float m_new = fmaxf(m_run[i], tmax);
+      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
+      alpha[i] = expf(m_run[i] - m_use);
+      float psum = 0.f;
+#pragma unroll
+      for (int j = 0; j < ATC_NK / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = 4 * j + 2 * i + e;
+          sm_[r] = expf(sm_[r] - m_use);
+          psum += sm_[r];
+        }
+      }
+      l_run[i] = l_run[i] * alpha[i] + psum;
+      m_run[i] = m_new;
     }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- online softmax on this thread's row
-    float s[ATC_NK];
+    // P (f16x2 planes, p in [0, 1]: never out of range): row r0 + 8 i, keys 8 j + cq + {0, 1} -> one 4-byte store per plane
 #pragma unroll
-    for (int u = 0; u < ATC_NK / 16; ++u) {
-      uint32_t r[16], rc[16];
-      tmem_ld16(lane_addr + u * 16, r);
-      tmem_ld16(lane_addr + ATC_NK + u * 16, rc);
-      tmem_ld_wait();
+    for (int j = 0; j < ATC_NK / 8; ++j) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int key = k0 + u * 16 + j;
-        float x = fmaf(__uint_as_float(rc[j]), F16X2_INV_SCALE, __uint_as_float(r[j])) * p.scale;
-        if (mrow && key < p.Tk) x += mrow[key];
-        s[u * 16 + j] = key < p.Tk ? x : -INFINITY;
+      for (int i = 0; i < 2; ++i) {
+        const float x0 = sm_[4 * j + 2 * i], x1 = sm_[4 * j + 2 * i + 1];
+        const __half2 hi = __floats2half2_rn(x0, x1);
+        const float2 hf = __half22float2(hi);
+        const __half2 lo = __floats2half2_rn((x0 - hf.x) * F16X2_SCALE, (x1 - hf.y) * F16X2_SCALE);
+        const int key = 8 * j + cq;
+        const uint32_t off = (uint32_t)(key >> 5) * Cfg::P_SLAB + sw64_off(r0 + 8 * i, (key >> 3) & 3) + (uint32_t)(key & 7) * 2u;
+        *reinterpret_cast<__half2*>(sm + Cfg::OFF_P + off) = hi;
+        *reinterpret_cast<__half2*>(sm + Cfg::OFF_P + Cfg::P_PLANE + off) = lo;
       }
     }
-    float tmax = s[0];
 #pragma unroll
-    for (int j = 1; j < ATC_NK; ++j) tmax = fmaxf(tmax, s[j]);
-    const float m_new = fmaxf(m_run, tmax);
-    const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-    const float alpha = expf(m_run - m_use);
-    float psum = 0.f;
+    for (int j = 0; j < DH / 8; ++j) {
 #pragma unroll
-    for (int j = 0; j < ATC_NK; ++j) {
-      s[j] = expf(s[j] - m_use);
-      psum += s[j];
-    }
-    l_run = l_run * alpha + psum;
-    m_run = m_new;
-    bool pbad = false;     // p is in [0, 1]: never out of range
-#pragma unroll
-    for (int c8 = 0; c8 < ATC_NK / 8; ++c8) {
-      uint4 p0, p1;
-      split8_f16x2(s + c8 * 8, p0, p1, pbad);
-      const uint32_t off = (uint32_t)(c8 >> 2) * Cfg::P_SLAB + sw64_off(tid, c8 & 3);
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_P + off) = p0;
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_P + Cfg::P_PLANE + off) = p1;
+      for (int e = 0; e < 4; ++e) {
+        om[4 * j + e] *= alpha[e >> 1];
+        oc[4 * j + e] *= alpha[e >> 1];
+      }
     }
     fence_proxy_async_smem();
-    tc_fence_before();       // this thread's reads of S are complete before O overwrites the columns
     __syncthreads();
-    // ---- O_tile = P V   (K = the tile's 64 keys: 4 k-steps)
-    if (warp == 0) {
-      tc_fence_after();
+    // ---- O += P V   (K = the tile's 64 keys: 4 k-steps)
+    wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < ATC_NK / 16; ++ks) {
-        const uint32_t pa = base + Cfg::OFF_P + (ks >> 1) * Cfg::P_SLAB + (ks & 1) * 32;
-        const uint32_t va = base + Cfg::OFF_V + (ks >> 1) * Cfg::V_SLAB + (ks & 1) * 32;
-        const uint64_t a1 = desc_hi | (uint64_t)((pa >> 4) & 0x3FFF), a2 = desc_hi | (uint64_t)(((pa + Cfg::P_PLANE) >> 4) & 0x3FFF);
-        const uint64_t b1 = desc_hi | (uint64_t)((va >> 4) & 0x3FFF), b2 = desc_hi | (uint64_t)(((va + Cfg::V_PLANE) >> 4) & 0x3FFF);
-        tc_mma_l(tmem + DH, a1, b2, IDESC_O, ks ? 1u : 0u, leader);
-        tc_mma_l(tmem + DH, a2, b1, IDESC_O, 1u, leader);
-        tc_mma_l(tmem, a1, b1, IDESC_O, ks ? 1u : 0u, leader);
-      }
-      tc_commit_l(bar, leader);
+    for (int ks = 0; ks < ATC_NK / 16; ++ks) {
+      const uint32_t pa = base + Cfg::OFF_P + (ks >> 1) * Cfg::P_SLAB + (ks & 1) * 32;
+      const uint32_t va = base + Cfg::OFF_V + (ks >> 1) * Cfg::V_SLAB + (ks & 1) * 32;
+      const uint64_t a1 = desc_hi | (uint64_t)((pa >> 4) & 0x3FFF), a2 = desc_hi | (uint64_t)(((pa + Cfg::P_PLANE) >> 4) & 0x3FFF);
+      const uint64_t b1 = desc_hi | (uint64_t)((va >> 4) & 0x3FFF), b2 = desc_hi | (uint64_t)(((va + Cfg::V_PLANE) >> 4) & 0x3FFF);
+      Wgmma<DH>::template mma<false>(oc, a1, b2, 1u);
+      Wgmma<DH>::template mma<false>(oc, a2, b1, 1u);
+      Wgmma<DH>::template mma<false>(om, a1, b1, 1u);
     }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-#pragma unroll
-    for (int u = 0; u < DH / 16; ++u) {
-      uint32_t r[16], rc[16];
-      tmem_ld16(lane_addr + u * 16, r);
-      tmem_ld16(lane_addr + DH + u * 16, rc);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        acc[u * 16 + j] = fmaf(acc[u * 16 + j], alpha, fmaf(__uint_as_float(rc[j]), F16X2_INV_SCALE, __uint_as_float(r[j])));
-    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(om);
+    wgmma_fence_regs(oc);
   }
   if (bad && ovf) *ovf = 1;
 
-  // ---- output: this thread's row
-  if (qvalid) {
-    const float inv = 1.0f / l_run;
-    if (p.o) {
-      float* o = p.o + (int64_t)b * p.o_sb + (int64_t)qrow * p.o_st + (int64_t)h * DH;
+  // ---- output.  Lane pairs (l, l ^ 1) swap halves so that each lane holds 4 consecutive columns of ONE row: the even
+  // lane columns 8 j + cq .. + 3 of row r0, the odd lane columns 8 j + cq - 2 .. + 1 of row r0 + 8.
+  float inv[2];
 #pragma unroll
-      for (int d = 0; d < DH; d += 4)
-        *reinterpret_cast<float4*>(o + d) = make_float4(acc[d] * inv, acc[d + 1] * inv, acc[d + 2] * inv, acc[d + 3] * inv);
-    }
-    if (p.o_planes) {
-      __nv_bfloat16* pl = reinterpret_cast<__nv_bfloat16*>(p.o_planes);
-      const int64_t off = ((int64_t)b * p.Tq + qrow) * p.o_planes_ld + (int64_t)h * DH;
-#pragma unroll
-      for (int d = 0; d < DH; d += 4) {
-        const float v[4] = {acc[d] * inv, acc[d + 1] * inv, acc[d + 2] * inv, acc[d + 3] * inv};
-        store_planes4(pl, p.o_plane_stride, off + d, v, p.o_planes_fmt, ovf);
-      }
-    }
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv[i] = 1.0f / l;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(Cfg::TMEM_COLS) : "memory");
+  const bool odd = lane & 1;
+  const int orow = odd ? qrow[1] : qrow[0];
+  const bool ovalid = odd ? qvalid[1] : qvalid[0];
+  float* o = p.o ? p.o + (int64_t)b * p.o_sb + (int64_t)(ovalid ? orow : 0) * p.o_st + (int64_t)h * DH : nullptr;
+  __nv_bfloat16* pl = reinterpret_cast<__nv_bfloat16*>(p.o_planes);
+  const int64_t poff = ((int64_t)b * p.Tq + (ovalid ? orow : 0)) * p.o_planes_ld + (int64_t)h * DH;
+#pragma unroll
+  for (int j = 0; j < DH / 8; ++j) {
+    float f[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) f[e] = fmaf(oc[4 * j + e], F16X2_INV_SCALE, om[4 * j + e]) * inv[e >> 1];
+    const float s0 = __shfl_xor_sync(0xffffffffu, odd ? f[0] : f[2], 1);
+    const float s1 = __shfl_xor_sync(0xffffffffu, odd ? f[1] : f[3], 1);
+    const float v[4] = {odd ? s0 : f[0], odd ? s1 : f[1], odd ? f[2] : s0, odd ? f[3] : s1};
+    const int col = 8 * j + cq - (odd ? 2 : 0);
+    if (ovalid) {
+      if (o) *reinterpret_cast<float4*>(o + col) = make_float4(v[0], v[1], v[2], v[3]);
+      if (pl) store_planes4(pl, p.o_plane_stride, poff + col, v, p.o_planes_fmt, ovf);
+    }
   }
 }
 
@@ -307,247 +308,8 @@ int attn_tc_launch(const mtts_attn_params& p, cudaStream_t st) {
     if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "attention_tc", (long long)e);
     configured.fetch_or(1ull << dev, std::memory_order_relaxed);
   }
-  dim3 grid((unsigned)cdiv64(p.Tq, 128), (unsigned)p.H, (unsigned)p.B);
+  dim3 grid((unsigned)cdiv64(p.Tq, ATC_NQ), (unsigned)p.H, (unsigned)p.B);
   launch_k(attn_tc_kernel<DH>, grid, 128, Cfg::SMEM, st, p, tc_ovf_ptr());
-  MTTS_CHECK_LAUNCH();
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Short sequences (the AR steps: Tq == Tk <= 64): TWO heads per CTA.  A head alone is a 64 x 64 x dh problem and fills half
-// of a 128-row MMA; here thread r owns query row (r & 63) of head 2 * blockIdx.x + (r >> 6).  The two heads are stacked:
-//   S = [Q_a; Q_b] [K_a; K_b]^T   one 128 x 128 x dh product whose off-diagonal 64 x 64 blocks (head a against head b) are
-//                                 simply never read,
-//   O = [P_a 0; 0 P_b] [V_a; V_b] one 128 x dh x 128 product with the block-diagonal P written by the softmax threads.
-// A single key tile, so no online-softmax rescale.  P reuses the Q | K staging area (both are dead once S has been
-// computed); with dh = 64 the CTA needs 97 KB and 256 TMEM columns, so two CTAs share an SM and one's staging / softmax
-// overlaps the other's MMAs.
-template <int DH>
-struct AtpCfg {
-  static constexpr int NS = DH / 32;                      // 64-byte K-slabs along dh
-  static constexpr int R_SLAB = 128 * 64;                 // 128 rows x 64 B (Q, K and P slabs)
-  static constexpr int V_SLAB = DH * 64;                  // V^T: dh rows, one slab per 32 keys, 4 slabs (128 stacked keys)
-  static constexpr int Q_PLANE = NS * R_SLAB, V_PLANE = 4 * V_SLAB, P_PLANE = 4 * R_SLAB;
-  static constexpr int OFF_Q = 0, OFF_K = 2 * Q_PLANE;
-  static constexpr int QK_BYTES = 4 * Q_PLANE, P_BYTES = 2 * P_PLANE;
-  static constexpr int OFF_P = 0;                         // aliases Q | K
-  static constexpr int OFF_V = QK_BYTES > P_BYTES ? QK_BYTES : P_BYTES;
-  static constexpr int OFF_BAR = OFF_V + 2 * V_PLANE;
-  static constexpr int SMEM = OFF_BAR + 1024 + 64;        // + alignment slack + barrier / TMEM slot
-  static constexpr int TMEM_COLS = 256;                   // S: 128 main + 128 correction; O (2 * dh <= 256) reuses them
-};
-
-template <int DH>
-__global__ void __launch_bounds__(128)
-attn_tc_pair_kernel(const mtts_attn_params p, int32_t* ovf) {
-  using Cfg = AtpCfg<DH>;
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t bar = base + Cfg::OFF_BAR;
-  const uint32_t tmem_slot = bar + 16;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(sm + Cfg::OFF_BAR + 16);
-
-  const int tid = threadIdx.x;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int hh = tid >> 6, row = tid & 63;
-  const int h = 2 * blockIdx.x + hh, b = blockIdx.y;
-  const int S = p.Tk;                                      // == Tq <= 64
-  const bool valid = row < S;
-
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(Cfg::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  pdl_wait();
-  bool bad = false;
-  // ---- stage Q and K: thread r splits row r of each stacked operand (rows past S are zero)
-  {
-    const float* qsrc = p.q + (int64_t)b * p.q_sb + (int64_t)(valid ? row : 0) * p.q_st + (int64_t)h * DH;
-    const float* ksrc = p.k + (int64_t)b * p.k_sb + (int64_t)(valid ? row : 0) * p.k_st + (int64_t)h * DH;
-#pragma unroll
-    for (int c8 = 0; c8 < DH / 8; ++c8) {
-      float vq[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, vk[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if (valid) {
-        const float4 a = *reinterpret_cast<const float4*>(qsrc + c8 * 8), c = *reinterpret_cast<const float4*>(qsrc + c8 * 8 + 4);
-        const float4 d = *reinterpret_cast<const float4*>(ksrc + c8 * 8), e = *reinterpret_cast<const float4*>(ksrc + c8 * 8 + 4);
-        vq[0] = a.x; vq[1] = a.y; vq[2] = a.z; vq[3] = a.w; vq[4] = c.x; vq[5] = c.y; vq[6] = c.z; vq[7] = c.w;
-        vk[0] = d.x; vk[1] = d.y; vk[2] = d.z; vk[3] = d.w; vk[4] = e.x; vk[5] = e.y; vk[6] = e.z; vk[7] = e.w;
-      }
-      uint4 p0, p1;
-      const uint32_t off = (uint32_t)(c8 >> 2) * Cfg::R_SLAB + sw64_off(tid, c8 & 3);
-      split8_f16x2(vq, p0, p1, bad);
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_Q + off) = p0;
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_Q + Cfg::Q_PLANE + off) = p1;
-      split8_f16x2(vk, p0, p1, bad);
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_K + off) = p0;
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_K + Cfg::Q_PLANE + off) = p1;
-    }
-  }
-  // ---- stage V^T: thread r transposes key (r & 63) of its head into column r of the (dh x 128) operand; a warp's 32
-  //      lanes fill one 64-byte row with 2-byte stores
-  {
-    const float* src = p.v + (int64_t)b * p.v_sb + (int64_t)(valid ? row : 0) * p.v_st + (int64_t)h * DH;
-    uint8_t* vt0 = sm + Cfg::OFF_V + (tid >> 5) * Cfg::V_SLAB;
-    const int kk = tid & 31;
-#pragma unroll
-    for (int i = 0; i < DH / 4; ++i) {
-      float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (valid) a = *reinterpret_cast<const float4*>(src + i * 4);
-      const float vv[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int d = i * 4 + e;
-        const __half x1 = __float2half_rn(vv[e]);
-        const __half x2 = __float2half_rn((vv[e] - __half2float(x1)) * F16X2_SCALE);
-        bad |= !(fabsf(vv[e]) <= 65504.0f);
-        const uint32_t off = sw64_off(d, kk >> 3) + (uint32_t)(kk & 7) * 2u;
-        *reinterpret_cast<uint16_t*>(vt0 + off) = __half_as_ushort(x1);
-        *reinterpret_cast<uint16_t*>(vt0 + Cfg::V_PLANE + off) = __half_as_ushort(x2);
-      }
-    }
-  }
-  fence_proxy_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot_ptr, 0);
-  const uint32_t leader = (warp == 0 && elect_one()) ? 1u : 0u;
-  const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-  const uint64_t desc_hi = umma_desc_kmajor<64>(0u);
-  constexpr uint32_t IDESC_S = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // f16 x f16 -> f32, N 128
-  constexpr uint32_t IDESC_O = (1u << 4) | ((uint32_t)(DH >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);    // N dh
-
-  // ---- S = [Q_a; Q_b] [K_a; K_b]^T
-  if (warp == 0) {
-#pragma unroll
-    for (int ks = 0; ks < DH / 16; ++ks) {
-      const uint32_t qa = base + Cfg::OFF_Q + (ks >> 1) * Cfg::R_SLAB + (ks & 1) * 32;
-      const uint32_t ka = base + Cfg::OFF_K + (ks >> 1) * Cfg::R_SLAB + (ks & 1) * 32;
-      const uint64_t a1 = desc_hi | (uint64_t)((qa >> 4) & 0x3FFF), a2 = desc_hi | (uint64_t)(((qa + Cfg::Q_PLANE) >> 4) & 0x3FFF);
-      const uint64_t b1 = desc_hi | (uint64_t)((ka >> 4) & 0x3FFF), b2 = desc_hi | (uint64_t)(((ka + Cfg::Q_PLANE) >> 4) & 0x3FFF);
-      tc_mma_l(tmem + 128, a1, b2, IDESC_S, ks ? 1u : 0u, leader);      // correction: q1 k2' + q2' k1
-      tc_mma_l(tmem + 128, a2, b1, IDESC_S, 1u, leader);
-      tc_mma_l(tmem, a1, b1, IDESC_S, ks ? 1u : 0u, leader);            // main: q1 k1
-    }
-    tc_commit_l(bar, leader);
-  }
-  mbar_wait(bar, 0);
-  tc_fence_after();
-  // ---- softmax over this thread's row: its own head's 64 columns
-  const float* mrow = p.mask ? p.mask + (int64_t)b * p.mask_sb + (int64_t)h * p.mask_sh + (int64_t)(valid ? row : 0) * p.mask_sq : nullptr;
-  float s[64];
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    uint32_t r[16], rc[16];
-    tmem_ld16(lane_addr + hh * 64 + u * 16, r);
-    tmem_ld16(lane_addr + 128 + hh * 64 + u * 16, rc);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int key = u * 16 + j;
-      float x = fmaf(__uint_as_float(rc[j]), F16X2_INV_SCALE, __uint_as_float(r[j])) * p.scale;
-      if (mrow && key < S) x += mrow[key];
-      s[key] = key < S ? x : -INFINITY;
-    }
-  }
-  float m = s[0];
-#pragma unroll
-  for (int j = 1; j < 64; ++j) m = fmaxf(m, s[j]);
-  const float m_use = (m == -INFINITY) ? 0.f : m;
-  float l = 0.f;
-#pragma unroll
-  for (int j = 0; j < 64; ++j) {
-    s[j] = expf(s[j] - m_use);
-    l += s[j];
-  }
-  // P row r: columns [64 hh, 64 hh + 64) hold this head's probabilities, the other head's 64 columns are zero
-  {
-    bool pbad = false;     // p is in [0, 1]: never out of range
-    const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-    for (int c8 = 0; c8 < 8; ++c8) {
-      uint4 p0, p1;
-      split8_f16x2(s + c8 * 8, p0, p1, pbad);
-      const int cm = hh * 8 + c8, cz = (1 - hh) * 8 + c8;       // 16-byte chunk index along the 128 stacked keys
-      const uint32_t off = (uint32_t)(cm >> 2) * Cfg::R_SLAB + sw64_off(tid, cm & 3);
-      const uint32_t offz = (uint32_t)(cz >> 2) * Cfg::R_SLAB + sw64_off(tid, cz & 3);
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_P + off) = p0;
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_P + Cfg::P_PLANE + off) = p1;
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_P + offz) = zero;
-      *reinterpret_cast<uint4*>(sm + Cfg::OFF_P + Cfg::P_PLANE + offz) = zero;
-    }
-  }
-  fence_proxy_async_smem();
-  tc_fence_before();       // this thread's reads of S are complete before O overwrites the columns
-  __syncthreads();
-  // ---- O = P [V_a; V_b]   (K = 128 stacked keys: 8 k-steps)
-  if (warp == 0) {
-    tc_fence_after();
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      const uint32_t pa = base + Cfg::OFF_P + (ks >> 1) * Cfg::R_SLAB + (ks & 1) * 32;
-      const uint32_t va = base + Cfg::OFF_V + (ks >> 1) * Cfg::V_SLAB + (ks & 1) * 32;
-      const uint64_t a1 = desc_hi | (uint64_t)((pa >> 4) & 0x3FFF), a2 = desc_hi | (uint64_t)(((pa + Cfg::P_PLANE) >> 4) & 0x3FFF);
-      const uint64_t b1 = desc_hi | (uint64_t)((va >> 4) & 0x3FFF), b2 = desc_hi | (uint64_t)(((va + Cfg::V_PLANE) >> 4) & 0x3FFF);
-      tc_mma_l(tmem + DH, a1, b2, IDESC_O, ks ? 1u : 0u, leader);
-      tc_mma_l(tmem + DH, a2, b1, IDESC_O, 1u, leader);
-      tc_mma_l(tmem, a1, b1, IDESC_O, ks ? 1u : 0u, leader);
-    }
-    tc_commit_l(bar, leader);
-  }
-  mbar_wait(bar, 1);
-  tc_fence_after();
-  if (bad && ovf) *ovf = 1;
-  // ---- output: this thread's row, 16 columns at a time
-  {
-    const float inv = 1.0f / l;
-    float* o = p.o ? p.o + (int64_t)b * p.o_sb + (int64_t)row * p.o_st + (int64_t)h * DH : nullptr;
-    __nv_bfloat16* pl = reinterpret_cast<__nv_bfloat16*>(p.o_planes);
-    const int64_t poff = ((int64_t)b * p.Tq + row) * p.o_planes_ld + (int64_t)h * DH;
-#pragma unroll
-    for (int u = 0; u < DH / 16; ++u) {
-      uint32_t r[16], rc[16];
-      tmem_ld16(lane_addr + u * 16, r);
-      tmem_ld16(lane_addr + DH + u * 16, rc);
-      tmem_ld_wait();
-      if (valid) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float v[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) v[e] = fmaf(__uint_as_float(rc[j + e]), F16X2_INV_SCALE, __uint_as_float(r[j + e])) * inv;
-          if (o) *reinterpret_cast<float4*>(o + u * 16 + j) = make_float4(v[0], v[1], v[2], v[3]);
-          if (pl) store_planes4(pl, p.o_plane_stride, poff + u * 16 + j, v, p.o_planes_fmt, ovf);
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(Cfg::TMEM_COLS) : "memory");
-  }
-}
-
-template <int DH>
-int attn_tc_pair_launch(const mtts_attn_params& p, cudaStream_t st) {
-  using Cfg = AtpCfg<DH>;
-  static std::atomic<uint64_t> configured{0};
-  const int dev = cur_device();
-  if (!(configured.load(std::memory_order_relaxed) & (1ull << dev))) {
-    cudaError_t e = cudaFuncSetAttribute(attn_tc_pair_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "attention_tc_pair", (long long)e);
-    configured.fetch_or(1ull << dev, std::memory_order_relaxed);
-  }
-  dim3 grid((unsigned)(p.H / 2), (unsigned)p.B);
-  launch_k(attn_tc_pair_kernel<DH>, grid, 128, Cfg::SMEM, st, p, tc_ovf_ptr());
   MTTS_CHECK_LAUNCH();
   return 0;
 }
@@ -566,14 +328,16 @@ bool attention_tc_eligible(const mtts_attn_params& p) {
   return p.B > 0 && p.H > 0 && p.Tq > 0 && p.Tk > 0 && p.H <= 65535 && p.B <= 65535;
 }
 
-// the two-heads-per-CTA form: an AR step (every query sees every key of an equally long sequence of at most 64 rows)
+// an AR step (every query sees every key of an equally long sequence of at most 64 rows): one 64-row tile per head, the
+// whole sequence in one key tile.  The same kernel as attention_tc; the entry point is kept for the opt-in routing of the
+// AR steps (mtts_set_attention_pair_min).
 bool attention_tc_pair_eligible(const mtts_attn_params& p) {
   return (p.dh == 64 || p.dh == 96) && p.Tq == p.Tk && p.Tk <= 64 && (p.H % 2) == 0 && attention_tc_eligible(p);
 }
 
 int attention_tc_pair(const mtts_attn_params& p, cudaStream_t st) {
-  MTTS_REQUIRE(attention_tc_pair_eligible(p), "shape / alignment not eligible for the two-head tensor-core attention");
-  return p.dh == 64 ? attn_tc_pair_launch<64>(p, st) : attn_tc_pair_launch<96>(p, st);
+  MTTS_REQUIRE(attention_tc_pair_eligible(p), "shape / alignment not eligible for the AR-step tensor-core attention");
+  return p.dh == 64 ? attn_tc_launch<64>(p, st) : attn_tc_launch<96>(p, st);
 }
 
 int attention_tc(const mtts_attn_params& p, cudaStream_t st) {

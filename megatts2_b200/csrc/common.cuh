@@ -1,4 +1,4 @@
-// Shared helpers for libmegatts2_b200 (sm_100a only).
+// Shared helpers for libmegatts2_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,7 +44,7 @@ extern bool g_trace_on;
   } while (0)
 
 // ---- programmatic dependent launch (PDL).  Every kernel of the library starts with pdl_entry() (or, for the kernels with
-// a real prologue - barrier init, TMEM allocation, descriptor prefetch - pdl_trigger() at entry and pdl_wait() before the
+// a real prologue - barrier init, descriptor prefetch - pdl_trigger() at entry and pdl_wait() before the
 // first access to global memory): launch_dependents lets the NEXT kernel of the stream be scheduled while this one still
 // runs, and the wait blocks it until this grid has completed and flushed, so only launch latency and prologues overlap -
 // never data.  Launches go through launch_k(), which sets the stream-serialisation attribute (MEGATTS2_PDL=0 disables it;

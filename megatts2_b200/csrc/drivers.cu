@@ -113,7 +113,7 @@ static bool last_row_tc() {
   return on;
 }
 
-// dense layer dispatch: one tap-GEMM call; conv1d() picks the tcgen05 engine when planes + scratch are attached
+// dense layer dispatch: one tap-GEMM call; conv1d() picks the wgmma engine when planes + scratch are attached
 // and the shape is eligible (M >= 128), else the exact FFMA engine
 static int lin(const mtts_encoder* e, const TcScratch* tc, const float* x, int ldx, int64_t M, int K, int N,
                const float* w32, const void* wtc, const float* bias, const float* res, int ldr, float* y, int ldy,

@@ -111,7 +111,7 @@ bool attention_tc_eligible(const mtts_attn_params& p);
 int attention_tc(const mtts_attn_params& p, cudaStream_t st);
 bool attention_tc_pair_eligible(const mtts_attn_params& p);
 int attention_tc_pair(const mtts_attn_params& p, cudaStream_t st);
-int set_attention_pair_min(int n);   // tcgen05 (attn_tc.cu)
+int set_attention_pair_min(int n);   // AR-step routing to attention_tc_pair (attn_tc.cu)
 int vq_argmin(const float* x, int ldx, const float* embed, int64_t N, int D, int K, int64_t* idx, cudaStream_t st);
 int vq_gather(const int64_t* idx, int idx_ld, const float* embed, int D, int K, int B, int T_out, int repeat, float* y,
               int64_t y_sb, int ldy, cudaStream_t st);

@@ -6,12 +6,12 @@
 // (modules/convnet.py:13-18, modules/transformer.py:26-31,76-85, modules/mrte.py:101-107,
 // HiFi-GAN generator).  This is the exact-fp32 engine: every product is an FFMA, so ids
 // derived from it (VQ codes, PLM argmax) are as close to the CPU fp32 reference as fp32
-// reassociation allows.  The tcgen05 3xTF32 engine (tapconv_tc.cu) shares this ABI.
+// reassociation allows.  The wgmma tap-GEMM (conv_tc.cu) shares this ABI.
 //
 // Tiling: BM x BN output tile per CTA, BK = 16 reduction slice, double-buffered shared
 // memory with register prefetch; each thread owns a TM x TN micro-tile split into 4-wide
 // groups so every shared-memory read is a conflict-free LDS.128.
-#include "common.cuh"
+#include "kernels.h"
 
 namespace mtts {
 
@@ -416,10 +416,12 @@ int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st) {
   {
     const int64_t tiles64 = cdiv64(M, 64) * cdiv64(p.Cout, 64);
     const int nk = (p.Cin + 15) / 16;
-    if (p.k == 1 && p.stride == 1 && p.pad == 0 && p.out_shift == 0 && !p.in_lens && M <= 256 && tiles64 <= 148 &&
+    const int sms = cur_device_sms();
+    if (p.k == 1 && p.stride == 1 && p.pad == 0 && p.out_shift == 0 && !p.in_lens && M <= 256 && tiles64 <= sms &&
         nk >= 16 && p.tc_scratch) {
       // two CTAs per SM: a lone 8-warp CTA cannot hide the L2 latency of its one-chunk-ahead prefetch
-      static const int target = []() { const char* e = getenv("MEGATTS2_SPLITK_CTAS"); return e ? atoi(e) : 296; }();
+      static const int target_env = []() { const char* e = getenv("MEGATTS2_SPLITK_CTAS"); return e ? atoi(e) : 0; }();
+      const int target = target_env > 0 ? target_env : 2 * sms;
       int splits = (int)(target / tiles64);
       if (splits > 16) splits = 16;
       if (splits > nk / 4) splits = nk / 4;

@@ -1,6 +1,6 @@
 // Backward / training-mode kernels (SURVEY.md 8f-4): what autograd needs around the tensor-core GEMMs so that
 // MegaPLMTrainer / MegaADMTrainer.training_step (models/trainer.py:243-268, 334-355) run forward AND backward through the
-// drop-in modules.  The dense contractions of the backward pass (dX = dY W, dW = dY^T X) go through the same tcgen05
+// drop-in modules.  The dense contractions of the backward pass (dX = dY W, dW = dY^T X) go through the same wgmma
 // tap-GEMM as the forward (megatts2_b200/autograd.py); this file holds the rest:
 //   bmm_kernel            strided batched matmul (fp32 FFMA) for the attention products and for shapes the tensor-core
 //                         engine does not take (K = 1 embeddings of the ADM, ragged row counts)

@@ -563,8 +563,8 @@ class Megatts(nn.Module):
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
-        # the three rules that make two streams share the device (csrc/conv_tc.cu, set_launch_policy): complementary budgets,
-        # no programmatic dependent launch on the vocoder's stream, no CTA pairs on the AR stream.  The calling stream joins
+        # the rules that make two streams share the device (csrc/conv_tc.cu, set_launch_policy): complementary budgets and
+        # no programmatic dependent launch on the vocoder's stream.  The calling stream joins
         # the side stream before the first full-width stage (length regulator -> PLM), so nothing sized for the whole device is
         # ever enqueued while the vocoder's persistent CTAs hold SMs.
         pw_side, side, n_side = None, None, 0

@@ -51,7 +51,7 @@ def conv1d(x, w_packed, bias=None, *, k, stride=1, dil=1, pad=0, pad_mode=L.PAD_
            pre_slope=0.0, post_act=L.ACT_NONE, post_slope=0.0, res=None, out=None, out_scale=1.0, accumulate=False,
            t_out=None, in_lens=None, w_tc=None):
     """x (B,T,Cin) channels-last, w_packed (k,Cin,Cout) -> (B,T_out,Cout).
-    w_tc: optional operand planes, (3,k,Cout,Cin) bf16 [bf16x3] or (2,k,Cout,Cin) fp16 [f16x2] -> the tcgen05 engine
+    w_tc: optional operand planes, (3,k,Cout,Cin) bf16 [bf16x3] or (2,k,Cout,Cin) fp16 [f16x2] -> the wgmma engine
     is used when the shape is eligible."""
     x = _dev(x, name="x")
     x, x_sb, ldx = _rows(x)
@@ -104,7 +104,7 @@ def _plane_fmt(w_planes):
 
 
 def linear_tc(x, w_planes, bias=None, *, res=None, pre_act=L.ACT_NONE, pre_slope=0.0, post_act=L.ACT_NONE):
-    """Tensor-core (tcgen05) dense layer: x (..., K) fp32, w_planes (3, N, K) bf16 [bf16x3] or (2, N, K) fp16 [f16x2]
+    """Tensor-core (wgmma) dense layer: x (..., K) fp32, w_planes (3, N, K) bf16 [bf16x3] or (2, N, K) fp16 [f16x2]
     -> (..., N) fp32."""
     x = _dev(x, name="x")
     shp = x.shape
@@ -384,7 +384,8 @@ def launch_policy_now():
 
 class launch_policy:
     """``with ops.launch_policy(sm_limit, pairs=..., pdl=...)``: the enclosed enqueues of this thread size their persistent
-    grids for ``sm_limit`` SMs, optionally without CTA pairs / programmatic dependent launch (include/megatts2_b200.h,
+    grids for ``sm_limit`` SMs, optionally without programmatic dependent launch (``pairs`` is accepted and ignored:
+    no CTA-pair kernels on sm_90) (include/megatts2_b200.h,
     mtts_set_launch_policy).  Restored on exit, also when the body raises."""
 
     def __init__(self, sm_limit, pairs=True, pdl=True):

@@ -195,8 +195,8 @@ class engine_scope:
 
 def default_engine() -> int:
     """Engine for the dense contractions with M >= 128 (MEGATTS2_ENGINE = f16x2 | bf16x3 | ffma):
-    2 = tcgen05 with f16x2 operands (default: 3 MMAs per fp32-grade product, |activation| <= 65504 guarded by the
-    overflow flag, see ops.tc_overflow), 1 = tcgen05 with bf16x3 operands (6 MMAs, full fp32 range), 0 = fp32 FFMA
+    2 = wgmma with f16x2 operands (default: 3 MMAs per fp32-grade product, |activation| <= 65504 guarded by the
+    overflow flag, see ops.tc_overflow), 1 = wgmma with bf16x3 operands (6 MMAs, full fp32 range), 0 = fp32 FFMA
     everywhere.  All three are fp32-grade; ids are bit-identical between them in the tests."""
     import os
     if _engine_override is not None:

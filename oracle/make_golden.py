@@ -2,12 +2,11 @@
 
     python -m oracle.make_golden
 
-Imports /root/reference under oracle/stubs.py, loads the seeded weights of
+Imports the reference checkout named by $MEGATTS2_REFERENCE under oracle/stubs.py, loads the seeded weights of
 oracle/weights.py into the reference's own modules (load_state_dict strict=True,
 which also pins the state_dict key set), runs the reference functions on seeded
 inputs, asserts that the restatement in oracle/ref_megatts2.py agrees, and writes
-inputs + reference outputs as small fixtures.  The GPU box has no /root/reference:
-tests there read only the fixtures.
+inputs + reference outputs as small fixtures.  The tests read only the fixtures.
 """
 import json
 import os

@@ -1,6 +1,6 @@
-"""sys.modules shims so the REAL reference (/root/reference) imports here.
+"""sys.modules shims so the REAL reference (a checkout named by $MEGATTS2_REFERENCE) imports here.
 
-Container-only test infrastructure (the GPU box has no /root/reference).
+Fixture-generation infrastructure only (oracle/make_golden.py); the tests never need the reference.
 The reference imports matplotlib, pypinyin, phonemizer, lhotse, speechbrain,
 librosa, lightning and tqdm at module import time (utils/utils.py:5,
 modules/tokenizer.py:1-17, models/megatts2.py:18-25, modules/datamodule.py:1-21);
@@ -11,11 +11,11 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("MEGATTS2_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("MEGATTS2_REFERENCE", "")
 
 
 def reference_available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "modules"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "modules"))
 
 
 def _mod(name, **attrs):

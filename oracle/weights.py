@@ -3,9 +3,9 @@
 TEST INFRASTRUCTURE (see oracle/__init__.py).  No checkpoint of the reference
 exists anywhere (infer.py:5-10 points at the author's local files), so parity is
 checked on seeded random weights.  Every tensor is a pure function of
-(base_seed, state_dict key, shape): the same values are produced in the build
-container (where the real reference loads them via load_state_dict) and on the
-GPU box (where /root/reference does not exist).
+(base_seed, state_dict key, shape): the same values are produced wherever they
+are built (oracle/make_golden.py loads them into the real reference via
+load_state_dict; the tests only need this module).
 
 Key sets follow the reference's state_dict layout (SURVEY.md §8b); a golden test
 pins them against the real reference's ``state_dict().keys()``.

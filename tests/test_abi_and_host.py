@@ -62,7 +62,7 @@ def test_launch_policy_is_scoped_and_restored():
     assert src.count("ops.launch_policy_now()") >= 2          # MegaPLM.infer and MegaADM.infer graph keys
 
 
-def _plan(M, K, N, ln=0, k=1, B=1, dil=1, partial=64 << 20, sms=148):
+def _plan(M, K, N, ln=0, k=1, B=1, dil=1, partial=64 << 20, sms=132):
     from megatts2_b200 import _lib as L
     out = (ctypes.c_int32 * 5)()
     L.check(L.lib().mtts_tc_plan_query(sms, B, M, K, N, k, dil, L.TC_F16X2, partial, ln, out))
@@ -72,9 +72,9 @@ def _plan(M, K, N, ln=0, k=1, B=1, dil=1, partial=64 << 20, sms=148):
 def test_tap_gemm_launch_plan_policy():
     """The dispatcher's plan is a pure host function (csrc/conv_tc.cu tc_plan): dense-layer tile widths minimise
     ceil(tiles / SMs) x per-MMA cost (65 cycles at N = 128, 55 below; ties to the narrower tile), splits need partial-sum
-    space, the small-channel vocoder convs take the halo form (C = 64 as a CTA pair), and a no-pairs launch policy is obeyed."""
+    space, the small-channel vocoder convs take the halo form, and no plan uses CTA pairs (none exist on sm_90)."""
     from megatts2_b200 import ops
-    sms = 148
+    sms = 132
     cd = lambda a, b: (a + b - 1) // b
     for D, FF in ((1024, 4096), (768, 1024)):                       # PLM / ADM stacks, rows = 64 x step
         for S in range(1, 65):
@@ -85,22 +85,19 @@ def test_tap_gemm_launch_plan_policy():
                 if pl["splits"] > 1:
                     assert pl["BN"] == 128 and not pl["pair"] and pl["splits"] * M * N * 4 <= 64 << 20 and pl["splits"] <= (K // 64) // 2
                     continue
-                if pl["pair"]:
-                    assert pl["BN"] == 128
-                    continue
+                assert pl["pair"] == 0
                 cost = {bn: cd(cd(M, 128) * cd(N, bn), sms) * (65 if bn == 128 else 55) for bn in (128, 64, 32)}
                 assert cost[pl["BN"]] == min(cost.values()), (M, K, N, pl, cost)
                 assert _plan(M, K, N, ln, partial=0)["splits"] == 1
     # the case the fill rule got wrong: PLM FF2 at step 20 = 80 tiles of N = 128 in one wave, not 160 of N = 64 in two
     assert _plan(64 * 20, 4096, 1024, 1)["BN"] == 128
-    # full-width dense layers run as CTA pairs; not under a no-pairs policy (two streams sharing the device)
-    assert _plan(4096, 1024, 3072)["pair"] == 1
-    with ops.launch_policy(74, pairs=False):
-        assert _plan(4096, 1024, 3072, sms=74)["pair"] == 0
-    assert _plan(4096, 1024, 3072)["pair"] == 1
-    # vocoder ResBlock convs: halo form at C = 32 (64-byte K-slabs) and C = 64 (as a pair), plain form at C = 128
+    # full-width dense layers: single CTAs of N = 128, also under a launch policy (two streams sharing the device)
+    assert _plan(4096, 1024, 3072) == dict(BN=128, splits=1, pair=0, halo=0, swb=128)
+    with ops.launch_policy(66, pairs=False):
+        assert _plan(4096, 1024, 3072, sms=66) == dict(BN=128, splits=1, pair=0, halo=0, swb=128)
+    # vocoder ResBlock convs: halo form at C = 32 (64-byte K-slabs) and C = 64, plain form at C = 128
     assert _plan(66816, 32, 32, k=7, B=64, dil=3, partial=0) == dict(BN=32, splits=1, pair=0, halo=1, swb=64)
-    assert _plan(33408, 64, 64, k=7, B=64, dil=3, partial=0) == dict(BN=64, splits=1, pair=0, halo=2, swb=128)
+    assert _plan(33408, 64, 64, k=7, B=64, dil=3, partial=0) == dict(BN=64, splits=1, pair=0, halo=1, swb=128)
     assert _plan(33408, 128, 128, k=11, B=64, dil=5, partial=0)["halo"] == 0
 
 

@@ -259,7 +259,7 @@ def test_vq_search_golden(golden, weights_cpu):
     helpers.record("vq_adversarial_fixture", dict(rows=int(idx.numel()), mismatches=int(mism.sum()), bit_exact_rate=rate,
                                                   max_gap64_of_a_mismatch=float(g["gap64"][mism].max()) if mism.any() else 0.0))
     # the fixture's second block is BUILT from near-ties (fp64 gap of the two best codes below fp32 rounding of
-    # |x|^2 + |e|^2 ~ 500); measured on B200: 0 mismatches of 1088 rows (profiles/r2_parity_rates.jsonl), so the bar is 1.0
+    # |x|^2 + |e|^2 ~ 500); measured on H100: 0 mismatches of 1088 rows, so the bar is 1.0
     assert rate == 1.0
     assert torch.equal(idx[:512], ref[:512])                 # the random (non-adversarial) block
     assert torch.equal(idx[-64:], torch.arange(64))          # exact codes map to themselves

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 engine (both operand formats: bf16x3 = engine 1, f16x2 = engine 2) against fp64 and against the
+"""GPU: the wgmma engine (both operand formats: bf16x3 = engine 1, f16x2 = engine 2) against fp64 and against the
 exact FFMA engine / golden ids."""
 import math
 
@@ -58,7 +58,7 @@ def test_linear_tc_vs_fp64(c, engine):
                       res=r.to(DEV) if r is not None else None, post_act=1 if c.get("relu") else 0)
     torch.cuda.synchronize()
     err = (y.cpu().double() - ref).abs().max().item()
-    # fp32-grade: the split drops O(2^-24) terms; accumulation is fp32 in TMEM
+    # fp32-grade: the split drops O(2^-24) terms; accumulation is fp32 in the wgmma register accumulators
     assert err < 3e-5 * max(1.0, ref.abs().max().item()), err
     # and it must be much closer to fp64 than a single-pass bf16 product could be (~4e-3 relative)
     y_ffma = ops.linear(x.to(DEV), pack.pack_linear(w).to(DEV), b.to(DEV) if b is not None else None,
@@ -162,7 +162,7 @@ CONV_TC_CASES = [
     dict(B=2, T=64, Cin=512, Cout=1024, k=5, post=1),                                  # conv-FF first conv
     dict(B=2, T=64, Cin=1024, Cout=512, k=5, res=True),                                # conv-FF second conv
     dict(B=1, T=130, Cin=96, Cout=160, k=3, pad_mode=2),                               # odd sizes: K and N tails
-    # full-machine grids (>= 148 tiles), long sequences
+    # full-machine grids (>= 132 tiles), long sequences
     dict(B=4, T=5000, Cin=64, Cout=64, k=7, dil=3, pad_mode=1, pre=2, res=True),
     dict(B=4, T=5000, Cin=64, Cout=64, k=11, dil=5, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3),
     dict(B=4, T=5000, Cin=64, Cout=64, k=3, dil=1, pad_mode=1, pre=2),

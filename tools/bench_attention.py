@@ -1,4 +1,4 @@
-"""A/B of the two attention kernels (diagnostics, GPU only): fp32 FFMA kernel (ops.cu) vs tcgen05 kernel (attn_tc.cu)
+"""A/B of the two attention kernels (diagnostics, GPU only): fp32 FFMA kernel (ops.cu) vs wgmma kernel (attn_tc.cu)
 at the PLM / ADM head shapes, sequence lengths 32 .. 512.  One process per kernel (the switch is read once)."""
 import os
 import sys

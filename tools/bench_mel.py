@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Config C2: STFT + mel-filterbank kernel on 10k synthetic 16 kHz 3-s clips, one B200.
+"""Config C2: STFT + mel-filterbank kernel on 10k synthetic 16 kHz 3-s clips, one GPU.
 Prints one JSON line: clips/s, achieved algorithmic GB/s (252,160 B per clip: 192,000 in + 60,160 out)
 and the fraction of the measured HBM peak."""
 import json
@@ -32,7 +32,7 @@ def main():
     bytes_alg = n * (48000 * 4 + 80 * 188 * 4)
     gbs = bytes_alg / (ms / 1e3) / 1e9
     pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(
-        os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+        os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0      # H100 SXM data sheet
     frames = n * 188
     print(json.dumps({"config": "C2 mel front end", "clips": n, "ms": round(ms, 4), "clips_per_s": round(n / (ms / 1e3)),
                       "frames_per_s": round(frames / (ms / 1e3)), "achieved_gbs": round(gbs, 1), "peak_gbs": pk,
