@@ -47,18 +47,28 @@ struct ConvTcArgs {
   int32_t bo_mode;             // halo form, diagnostics: 1 = put (addr >> 7) & 7 into the descriptors' base-offset field
 };
 
-// One CTA = 2 consumer warpgroups (rows 0-63 | 64-127 of a 128-row tile, accumulators in registers, each runs its own
-// epilogue) + 1 TMA producer warp; persistent over the work items, a STAGES-deep ring of operand stages between them.
+// One CTA = 2 consumer warpgroups + 1 TMA producer warpgroup, persistent over the work items, a STAGES-deep ring of
+// operand stages between them.  Ping-pong schedule: the consumer warpgroups take the CTA's work items alternately, each
+// item whole (mainloop, then its own epilogue, accumulators in registers throughout), and take turns on the tensor pipe
+// through a pair of named barriers: warpgroup A issues the MMAs of its item while warpgroup B runs the epilogue of its
+// previous one, so every epilogue hides under the other warpgroup's MMAs.  An item is ROWS x BN with at most 128
+// accumulator registers per thread: 64 x 128 (one m64 MMA per product) at BN = 128, 128 x BN (two m64 halves) below.
+// The producer warpgroup hands its registers to the consumers (setmaxnreg); one elected lane issues the loads, in the
+// order the consumers take the items.
 // HALO = 1 (convolutions whose input channels fit ONE K-slab, Cin <= SWB / 2): the activation tile of an output tile -
 // its 128 rows plus the dil * (k - 1) halo rows - is loaded ONCE into a multi-buffered region and every tap reads it
 // through a row-shifted wgmma descriptor; only the (tiny) per-tap weight tiles stream through the stage ring.  The plain
 // form re-reads the tile once per tap (k-fold L2 -> SM traffic), which is what bounds the C = 32 / 64 HiFi-GAN stages.
 constexpr int CTC_HALO_ROWS = 192;     // rows of a halo tile buffer: 128 + dil * (k - 1) <= 192, a multiple of 8
-constexpr int CTC_THREADS = 288;       // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int CTC_THREADS = 384;       // warps 0-7: two consumer warpgroups, warps 8-11: TMA producer warpgroup
+constexpr int CTC_PRODUCER_REGS = 40, CTC_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
 template <int BN, int SWB, int NP = 3, int HALO = 0>
 struct ConvTcCfg {
+  static constexpr int ROWS = BN == 128 ? 64 : 128;       // output rows of a work item
+  static constexpr int HALVES = ROWS / 64;                 // m64 MMAs per product
+  static_assert(!HALO || ROWS == 128, "the halo form keeps 128-row tiles");
   static constexpr int BK = SWB / 2;                       // bf16 elements per swizzled row
-  static constexpr int A_PLANE = (HALO ? CTC_HALO_ROWS : 128) * SWB;
+  static constexpr int A_PLANE = (HALO ? CTC_HALO_ROWS : ROWS) * SWB;
   static constexpr int B_PLANE = BN * SWB;
   static constexpr int STAGE = HALO ? NP * B_PLANE : NP * (A_PLANE + B_PLANE);
   // halo-tile buffers: a tile's rows are requested when the buffer of the tile A_BUFS back is released, i.e. A_BUFS - 1 tiles
@@ -88,7 +98,8 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform as far as the compiler can tell
   const int lane = threadIdx.x & 31;
-  const int num_t = (g.T + 127) / 128, num_n = (g.Cout + BN - 1) / BN;
+  constexpr int ROWS = Cfg::ROWS, HALVES = Cfg::HALVES;
+  const int num_t = (g.T + ROWS - 1) / ROWS, num_n = (g.Cout + BN - 1) / BN;
   const int num_tiles = g.B * num_t * num_n * g.splits;      // work items: (tile, K split)
   const int ncb = (g.Cin + Cfg::BK - 1) / Cfg::BK;
   const int num_k = g.k * ncb;
@@ -101,12 +112,12 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 8);          // one arrive per consumer warp
+      mbar_init(empty_bar + 8 * s, 4);          // one arrive per warp of the consumer warpgroup that owns the item
     }
     if constexpr (HALO) {
       for (int s = 0; s < Cfg::A_BUFS; ++s) {
         mbar_init(afull_bar + 8 * s, 1);
-        mbar_init(aempty_bar + 8 * s, 8);
+        mbar_init(aempty_bar + 8 * s, 4);
       }
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -114,8 +125,10 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   __syncthreads();
   pdl_wait();        // everything above (barriers, descriptor prefetch) overlapped the previous kernel's tail
 
-  if (warp == 8) {
-    // ================= TMA producer (the whole warp walks the loops, one elected lane issues) =================
+  if (warp >= 8) {
+    // ================= TMA producer (warp 8 walks the loops, one elected lane issues) =================
+    setmaxnreg_dec<CTC_PRODUCER_REGS>();
+    if (warp != 8) return;
     const bool leader = elect_one();
     int stage = 0, phase = 0;
     [[maybe_unused]] int ait = 0;
@@ -124,7 +137,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       const int kb0 = (int)((int64_t)sp * num_k / g.splits), kb1 = (int)((int64_t)(sp + 1) * num_k / g.splits);
       const int nb = tile % num_n, r = tile / num_n;
       const int tb = r % num_t, b = r / num_t;
-      const int trow = tb * 128 + g.row0;      // the tile's first (padded) input row
+      const int trow = tb * ROWS + g.row0;     // the item's first (padded) input row
       if constexpr (HALO) {
         // the tile's activation rows [trow, trow + 128 + dil * (k - 1)) once, then one weight tile per tap
         const int ab = ait % Cfg::A_BUFS, aph = (ait / Cfg::A_BUFS) & 1;
@@ -168,7 +181,8 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
     return;
   }
 
-  // ================= consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile =================
+  // ================= consumers: warpgroup wg owns the CTA's work items wg, wg + 2, wg + 4, ... =================
+  setmaxnreg_inc<CTC_CONSUMER_REGS>();
   constexpr float CS = NP == 2 ? F16X2_INV_SCALE : 1.0f;   // weight of the correction accumulator (exact: a power of two)
   constexpr bool BF16 = NP == 3;
   const int wg = warp >> 2, w4 = warp & 3;
@@ -183,23 +197,34 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   const int64_t ystep = 8 * (int64_t)g.ldy, rstep = 8 * (int64_t)g.ldr, ostep = 8 * (int64_t)g.op_ld;
   const int64_t pstep = 8 * (int64_t)g.Cout;
   const uint64_t desc_base = wgmma_desc<SWB>(0u);      // everything except the start address
-  const uint32_t a_rows = (uint32_t)(wg * 64 * SWB);   // this warpgroup's rows inside an activation tile
   // Each unit = this warp's 16 rows x 16 columns.  The fragment holds two rows x two columns per lane; writing them out
   // like that would make every global instruction touch 16 different lines, so the unit is transposed through a padded
   // shared buffer and ALL global traffic of the epilogue (y, residual, accumulate, operand planes) is issued as 8 rows x
   // 64 contiguous bytes per instruction.
   float* stg = epi_stage + warp * (16 * 20);
-  float acc[BN / 2], cor[BN / 2];
-  int stage = 0, phase = 0, it = 0;
-  for (int item = blockIdx.x; item < num_tiles; item += gridDim.x, ++it) {
+  float acc[HALVES][BN / 2], cor[HALVES][BN / 2];
+  // Turns on the tensor pipe: warpgroup wg waits on barrier 1 + wg before it issues the MMAs of its item li (li > 0); the
+  // other warpgroup arrives there once it has issued all MMAs of item li - 1.  Arrivals are made only for an item that
+  // exists, so no barrier is left half-arrived when the CTA exits.
+  const int n_items = num_tiles > (int)blockIdx.x ? (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+  int stage = 0, phase = 0;
+  for (int li = 0; li < n_items; ++li) {
+    const int item = blockIdx.x + li * gridDim.x;
     const int sp = item % splits, tile = item / splits;
     const int kb0 = (int)((int64_t)sp * num_k / splits), kb1 = (int)((int64_t)(sp + 1) * num_k / splits);
+    if ((li & 1) != wg) {                       // the other warpgroup's item: step over its stages of the ring
+      const int s = stage + (kb1 - kb0);
+      phase ^= (s / STAGES) & 1;
+      stage = s % STAGES;
+      continue;
+    }
     const int nb = tile % num_n, r = tile / num_n;
     const int tb = r % num_t, b = r / num_t;
     [[maybe_unused]] int ab = 0;
+    if (li > 0) named_bar_sync(1 + wg, 256);
     if constexpr (HALO) {
-      ab = it % Cfg::A_BUFS;
-      mbar_wait(afull_bar + 8 * ab, (it / Cfg::A_BUFS) & 1);
+      ab = li % Cfg::A_BUFS;
+      mbar_wait(afull_bar + 8 * ab, (li / Cfg::A_BUFS) & 1);
     }
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
@@ -207,31 +232,35 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       // HALO: A is the halo tile shifted by kb * dil rows (kb == tap: one K-slab per tap).  The swizzle is a function of the
       // shared-memory ADDRESS bits (the TMA wrote with them, the MMA reads with them), so a start address that is a whole
       // number of rows into the tile needs nothing else; bo_mode = 1 puts the row phase into the base-offset field instead.
-      const uint32_t a_addr = HALO ? smem_a + ab * NP * Cfg::A_PLANE + (uint32_t)(kb * g.dil) * SWB + a_rows
-                                   : smem_base + stage * Cfg::STAGE + a_rows;
+      const uint32_t a_addr = HALO ? smem_a + ab * NP * Cfg::A_PLANE + (uint32_t)(kb * g.dil) * SWB
+                                   : smem_base + stage * Cfg::STAGE;
       const uint32_t b_addr = smem_base + stage * Cfg::STAGE + (HALO ? 0 : NP * Cfg::A_PLANE);
       const uint32_t first = (kb == kb0) ? 0u : 1u;
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < Cfg::BK / 16; ++ks) {
-        const uint32_t aa = a_addr + ks * 32, bb = b_addr + ks * 32;
-        const uint64_t a1 = wgmma_desc_shifted(desc_base, aa, HALO ? g.bo_mode : 0);
-        const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::A_PLANE, HALO ? g.bo_mode : 0);
+        const uint32_t bb = b_addr + ks * 32;
         const uint64_t b1 = desc_base | (uint64_t)((bb >> 4) & 0x3FFF), b2 = desc_base | (uint64_t)(((bb + Cfg::B_PLANE) >> 4) & 0x3FFF);
         const uint32_t f = (ks == 0) ? first : 1u;
-        if constexpr (NP == 2) {
-          Wgmma<BN>::template mma<BF16>(cor, a1, b2, f);       // x1 w2'
-          Wgmma<BN>::template mma<BF16>(cor, a2, b1, 1u);      // x2' w1
-          Wgmma<BN>::template mma<BF16>(acc, a1, b1, f);       // x1 w1
-        } else {
-          const uint64_t a3 = wgmma_desc_shifted(desc_base, aa + 2 * Cfg::A_PLANE, HALO ? g.bo_mode : 0);
-          const uint64_t b3 = desc_base | (uint64_t)(((bb + 2 * Cfg::B_PLANE) >> 4) & 0x3FFF);
-          Wgmma<BN>::template mma<BF16>(cor, a2, b2, f);       // x2 w2   (smallest terms first)
-          Wgmma<BN>::template mma<BF16>(cor, a1, b3, 1u);      // x1 w3
-          Wgmma<BN>::template mma<BF16>(cor, a3, b1, 1u);      // x3 w1
-          Wgmma<BN>::template mma<BF16>(cor, a1, b2, 1u);      // x1 w2
-          Wgmma<BN>::template mma<BF16>(cor, a2, b1, 1u);      // x2 w1
-          Wgmma<BN>::template mma<BF16>(acc, a1, b1, f);       // x1 w1
+#pragma unroll
+        for (int hv = 0; hv < HALVES; ++hv) {                  // rows [64 hv, 64 hv + 64) of the item
+          const uint32_t aa = a_addr + hv * 64 * SWB + ks * 32;
+          const uint64_t a1 = wgmma_desc_shifted(desc_base, aa, HALO ? g.bo_mode : 0);
+          const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::A_PLANE, HALO ? g.bo_mode : 0);
+          if constexpr (NP == 2) {
+            Wgmma<BN>::template mma<BF16>(cor[hv], a1, b2, f);       // x1 w2'
+            Wgmma<BN>::template mma<BF16>(cor[hv], a2, b1, 1u);      // x2' w1
+            Wgmma<BN>::template mma<BF16>(acc[hv], a1, b1, f);       // x1 w1
+          } else {
+            const uint64_t a3 = wgmma_desc_shifted(desc_base, aa + 2 * Cfg::A_PLANE, HALO ? g.bo_mode : 0);
+            const uint64_t b3 = desc_base | (uint64_t)(((bb + 2 * Cfg::B_PLANE) >> 4) & 0x3FFF);
+            Wgmma<BN>::template mma<BF16>(cor[hv], a2, b2, f);       // x2 w2   (smallest terms first)
+            Wgmma<BN>::template mma<BF16>(cor[hv], a1, b3, 1u);      // x1 w3
+            Wgmma<BN>::template mma<BF16>(cor[hv], a3, b1, 1u);      // x3 w1
+            Wgmma<BN>::template mma<BF16>(cor[hv], a1, b2, 1u);      // x1 w2
+            Wgmma<BN>::template mma<BF16>(cor[hv], a2, b1, 1u);      // x2 w1
+            Wgmma<BN>::template mma<BF16>(acc[hv], a1, b1, f);       // x1 w1
+          }
         }
       }
       wgmma_commit();
@@ -240,71 +269,78 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
+    if (li + 1 < n_items) named_bar_arrive(2 - wg, 256);      // all MMAs of this item issued: the other warpgroup's turn
     wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-    wgmma_fence_regs(cor);
+#pragma unroll
+    for (int hv = 0; hv < HALVES; ++hv) {
+      wgmma_fence_regs(acc[hv]);
+      wgmma_fence_regs(cor[hv]);
+    }
     if (lane == 0) {
       if (prev >= 0) mbar_arrive(empty_bar + 8 * prev);
       if constexpr (HALO) mbar_arrive(aempty_bar + 8 * ab);     // the halo tile is free once this tile's MMAs have retired
     }
 
-    // ---- epilogue of this warp's 16 rows
-    const int t0 = tb * 128 + wg * 64 + w4 * 16 + rsub;          // this lane's rows: t0 + 8 i
-    const int nbase = nb * BN + chunk * 4;
-    const int64_t yo = (int64_t)t0 * g.ldy + nbase;                // within batch item b
-    const int64_t yb = (int64_t)b * g.y_sb;
-    const int64_t ro = (int64_t)b * g.res_sb + (int64_t)t0 * g.ldr + nbase;
-    const int64_t oo = ((int64_t)b * g.op_tp + g.op_hl + t0) * g.op_ld + nbase;
-    const int64_t po = (((int64_t)sp * g.B + b) * g.T + t0) * g.Cout + nbase;
+    // ---- epilogue of this warp's 16 rows of each 64-row half
 #pragma unroll
-    for (int u = 0; u < BN / 16; ++u) {
-      const int n = nbase + u * 16;
-      const bool ncol = n < g.Cout;                 // Cout % 4 == 0: a 4-wide chunk is all-in or all-out
+    for (int hv = 0; hv < HALVES; ++hv) {
+      const int t0 = tb * ROWS + hv * 64 + w4 * 16 + rsub;         // this lane's rows: t0 + 8 i
+      const int nbase = nb * BN + chunk * 4;
+      const int64_t yo = (int64_t)t0 * g.ldy + nbase;                // within batch item b
+      const int64_t yb = (int64_t)b * g.y_sb;
+      const int64_t ro = (int64_t)b * g.res_sb + (int64_t)t0 * g.ldr + nbase;
+      const int64_t oo = ((int64_t)b * g.op_tp + g.op_hl + t0) * g.op_ld + nbase;
+      const int64_t po = (((int64_t)sp * g.B + b) * g.T + t0) * g.Cout + nbase;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {                 // fragment columns 8 (2u + h) + 2 (lane % 4) + {0, 1}, rows lane / 4 + {0, 8}
-        const int j = 2 * u + h, c = 8 * h + 2 * chunk;
-        *reinterpret_cast<float2*>(stg + rsub * 20 + c) =
-            make_float2(fmaf(cor[4 * j + 0], CS, acc[4 * j + 0]), fmaf(cor[4 * j + 1], CS, acc[4 * j + 1]));
-        *reinterpret_cast<float2*>(stg + (rsub + 8) * 20 + c) =
-            make_float2(fmaf(cor[4 * j + 2], CS, acc[4 * j + 2]), fmaf(cor[4 * j + 3], CS, acc[4 * j + 3]));
-      }
-      __syncwarp();
-      float4 bvec = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (has_bias && ncol) bvec = __ldg(reinterpret_cast<const float4*>(g.bias + n));
+      for (int u = 0; u < BN / 16; ++u) {
+        const int n = nbase + u * 16;
+        const bool ncol = n < g.Cout;                 // Cout % 4 == 0: a 4-wide chunk is all-in or all-out
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        if (!(ncol && (t0 + 8 * i) < g.T)) continue;
-        const float4 a4 = *reinterpret_cast<const float4*>(stg + (i * 8 + rsub) * 20 + chunk * 4);
-        if (partial_out) {
-          *reinterpret_cast<float4*>(g.partial + po + i * pstep + u * 16) = a4;
-          continue;
+        for (int h = 0; h < 2; ++h) {                 // fragment columns 8 (2u + h) + 2 (lane % 4) + {0, 1}, rows lane / 4 + {0, 8}
+          const int j = 2 * u + h, c = 8 * h + 2 * chunk;
+          *reinterpret_cast<float2*>(stg + rsub * 20 + c) =
+              make_float2(fmaf(cor[hv][4 * j + 0], CS, acc[hv][4 * j + 0]), fmaf(cor[hv][4 * j + 1], CS, acc[hv][4 * j + 1]));
+          *reinterpret_cast<float2*>(stg + (rsub + 8) * 20 + c) =
+              make_float2(fmaf(cor[hv][4 * j + 2], CS, acc[hv][4 * j + 2]), fmaf(cor[hv][4 * j + 3], CS, acc[hv][4 * j + 3]));
         }
-        float4 rv = make_float4(0.f, 0.f, 0.f, 0.f), ov = rv;
-        if (has_res) rv = *reinterpret_cast<const float4*>(g.res + ro + i * rstep + u * 16);
-        if (has_acc) ov = *reinterpret_cast<const float4*>(g.y + yb + yo + i * ystep + u * 16);
-        float v[4] = {a4.x + bvec.x, a4.y + bvec.y, a4.z + bvec.z, a4.w + bvec.w};
-        if (g.post_act != MTTS_ACT_NONE) {
+        __syncwarp();
+        float4 bvec = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (has_bias && ncol) bvec = __ldg(reinterpret_cast<const float4*>(g.bias + n));
 #pragma unroll
-          for (int e = 0; e < 4; ++e) v[e] = act_apply(v[e], g.post_act, g.post_slope);
-        }
-        v[0] = (v[0] + rv.x) * g.out_scale + ov.x;
-        v[1] = (v[1] + rv.y) * g.out_scale + ov.y;
-        v[2] = (v[2] + rv.z) * g.out_scale + ov.z;
-        v[3] = (v[3] + rv.w) * g.out_scale + ov.w;
-        if (has_y) {
-          const int64_t flat = yo + i * ystep + u * 16 + out_shift;      // out_shift % 4 == 0: all-in or all-out
-          if (HALO || (flat >= 0 && flat + 4 <= g.ybe))
-            *reinterpret_cast<float4*>(g.y + yb + flat) = make_float4(v[0], v[1], v[2], v[3]);
-        }
-        if (has_op) {
-          if (g.op_act != MTTS_ACT_NONE) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] = act_apply(v[e], g.op_act, g.op_slope);
+        for (int i = 0; i < 2; ++i) {
+          if (!(ncol && (t0 + 8 * i) < g.T)) continue;
+          const float4 a4 = *reinterpret_cast<const float4*>(stg + (i * 8 + rsub) * 20 + chunk * 4);
+          if (partial_out) {
+            *reinterpret_cast<float4*>(g.partial + po + i * pstep + u * 16) = a4;
+            continue;
           }
-          store_planes4(g.op, g.op_stride, oo + i * ostep + u * 16, v, NP == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3, g.ovf);
+          float4 rv = make_float4(0.f, 0.f, 0.f, 0.f), ov = rv;
+          if (has_res) rv = *reinterpret_cast<const float4*>(g.res + ro + i * rstep + u * 16);
+          if (has_acc) ov = *reinterpret_cast<const float4*>(g.y + yb + yo + i * ystep + u * 16);
+          float v[4] = {a4.x + bvec.x, a4.y + bvec.y, a4.z + bvec.z, a4.w + bvec.w};
+          if (g.post_act != MTTS_ACT_NONE) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) v[e] = act_apply(v[e], g.post_act, g.post_slope);
+          }
+          v[0] = (v[0] + rv.x) * g.out_scale + ov.x;
+          v[1] = (v[1] + rv.y) * g.out_scale + ov.y;
+          v[2] = (v[2] + rv.z) * g.out_scale + ov.z;
+          v[3] = (v[3] + rv.w) * g.out_scale + ov.w;
+          if (has_y) {
+            const int64_t flat = yo + i * ystep + u * 16 + out_shift;      // out_shift % 4 == 0: all-in or all-out
+            if (HALO || (flat >= 0 && flat + 4 <= g.ybe))
+              *reinterpret_cast<float4*>(g.y + yb + flat) = make_float4(v[0], v[1], v[2], v[3]);
+          }
+          if (has_op) {
+            if (g.op_act != MTTS_ACT_NONE) {
+#pragma unroll
+              for (int e = 0; e < 4; ++e) v[e] = act_apply(v[e], g.op_act, g.op_slope);
+            }
+            store_planes4(g.op, g.op_stride, oo + i * ostep + u * 16, v, NP == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3, g.ovf);
+          }
         }
+        __syncwarp();   // the staging buffer is reused by the next unit
       }
-      __syncwarp();   // the staging buffer is reused by the next unit
     }
   }
 }
@@ -659,8 +695,8 @@ static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, cudaStrea
     if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "conv_tc", (long long)e);
     g_dev[dev].attr_done |= (1u << slot);
   }
-  const int64_t tiles = (int64_t)a.B * cdiv64(a.T, 128) * cdiv64(a.Cout, BN) * a.splits;
-  const int grid = (int)(tiles < sms ? tiles : sms);
+  const int64_t items = (int64_t)a.B * cdiv64(a.T, Cfg::ROWS) * cdiv64(a.Cout, BN) * a.splits;
+  const int grid = (int)(items < sms ? items : sms);
   launch_k(conv_tc_kernel<BN, SWB, NP, HALO>, grid, CTC_THREADS, Cfg::SMEM, st, maps, a);
   MTTS_CHECK_LAUNCH();
   return 0;
@@ -824,10 +860,12 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   const TcPlan pl = tc_plan(env, sms, p, np, ln_rides);
   const int SWB = pl.SWB, BN = pl.BN, splits = pl.splits;
   const bool halo_form = pl.halo_form;
+  // activation box: the work item's rows (ConvTcCfg::ROWS: 64 at BN = 128, else 128), the halo form adds the halo rows
+  const int a_rows = halo_form ? 128 + halo : (BN == 128 ? 64 : 128);
   ConvTcMaps maps;
   for (int q = 0; q < np; ++q) {
     MTTS_TRY(cmap_get(planes + q * plane_stride, (uint64_t)p.Cin, (uint64_t)Tp_map, (uint64_t)p.B, SWB / 2,
-                      halo_form ? 128 + halo : 128, SWB, fmt, &maps.a[q]));
+                      a_rows, SWB, fmt, &maps.a[q]));
     MTTS_TRY(cmap_get((const __nv_bfloat16*)p.w_tc + (int64_t)q * p.k * p.Cout * p.Cin, (uint64_t)p.Cin,
                       (uint64_t)p.k * p.Cout, 0, SWB / 2, BN, SWB, fmt, &maps.b[q]));
   }

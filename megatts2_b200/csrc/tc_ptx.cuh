@@ -55,6 +55,20 @@ __device__ __forceinline__ bool elect_one() {
 // generic-proxy shared-memory writes (operands staged by threads) become visible to the MMA's async proxy
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// per-thread register budget of the executing warpgroup (every warp of the warpgroup executes the same instruction):
+// a producer warpgroup gives registers back, the consumer warpgroups take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// named barriers (id 0 is __syncthreads): `threads` counts the waiting and the arriving side together
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // ---- wgmma (warpgroup MMA): D (fp32, in the registers of the 128 threads of a warpgroup) += A (64 x 16) B^T (N x 16), both
 // operands K-major in shared memory.  Fragment of m64nN: thread t (warp w = t / 32 of the warpgroup, lane l) holds d[4 j + 2 i + e]
 // = D[16 w + l / 4 + 8 i][8 j + 2 (l % 4) + e].
