@@ -51,14 +51,17 @@ int mtts_profile_split(double* out6);
 int mtts_trace_begin(void* stream);
 int mtts_trace_end(char* buf, int32_t buf_len);
 
-/* Tensor-core operand formats.  Both give fp32-grade results (the tests hold them to the same bars):
+/* Tensor-core operand formats.  BF16X3 and F16X2 give fp32-grade results (the tests hold them to the same bars):
  *   BF16X3: x = x1 + x2 + x3 (bf16), products x1w1 + x1w2 + x2w1 + x2w2 + x1w3 + x3w1  -> 6 MMAs, fp32 range
  *   F16X2 : x = x1 + x2' * 2^-11 (fp16, residual stored scaled so it stays in the normal range), products
  *           x1w1 + (x1w2' + x2'w1) * 2^-11 -> 3 MMAs, 22 significant bits per operand; |x| must be <= 65504.
- * An activation outside the fp16 range poisons its result (inf/NaN) and sets the int32 flag registered here for
- * the current device (the caller owns the 4 bytes; NULL unbinds).  The Python layer checks it once per synthesis
- * and reruns the batch on BF16X3. */
-enum { MTTS_TC_BF16X3 = 0, MTTS_TC_F16X2 = 1 };
+ * F16 is the opt-in half-precision inference format, NOT fp32-grade:
+ *   F16   : x ~ x1 = fp16(x) (round-to-nearest, one plane), product x1w1 -> 1 MMA into an fp32 accumulator,
+ *           11 significant bits per operand; |x| must be <= 65504.
+ * A format has 3 - fmt planes.  An activation outside the fp16 range (F16X2, F16) poisons its result (inf/NaN) and sets
+ * the int32 flag registered here for the current device (the caller owns the 4 bytes; NULL unbinds).  The Python layer
+ * checks it once per synthesis and reruns the batch on BF16X3. */
+enum { MTTS_TC_BF16X3 = 0, MTTS_TC_F16X2 = 1, MTTS_TC_F16 = 2 };
 int mtts_tc_overflow_bind(int32_t* flag_dev);
 /* SM budget of the calling host thread's subsequent launches (0 = the whole device): the persistent tensor-core kernels
  * size their grids from it, so work enqueued on two streams can share the device (the prompt re-vocode of Megatts.forward
@@ -125,8 +128,9 @@ typedef struct {
    * fill the GPU, K is split across CTAs into fp32 partials here and a second kernel reduces them in a fixed order and
    * applies the epilogue.  >= splits * B*Tout * Cout * 4 bytes; NULL -> never split. */
   void* tc_partial; int64_t tc_partial_bytes;
-  /* operand format of w_tc / the activation planes: MTTS_TC_BF16X3 (three bf16 planes, 6 MMAs per product) or
-   * MTTS_TC_F16X2 (two fp16 planes, residual scaled by 2^11, 3 MMAs per product; see mtts_tc_overflow_bind) */
+  /* operand format of w_tc / the activation planes: MTTS_TC_BF16X3 (three bf16 planes, 6 MMAs per product),
+   * MTTS_TC_F16X2 (two fp16 planes, residual scaled by 2^11, 3 MMAs per product; see mtts_tc_overflow_bind) or
+   * MTTS_TC_F16 (one fp16 plane, 1 MMA per product, not fp32-grade) */
   int32_t tc_fmt;
   /* tc_presplit only: the planes in tc_scratch may be a SHARED buffer with a larger halo than this conv needs -
    * tc_in_tp rows per batch item (0 -> Tout + dil*(k-1)) and this conv's first padded row at tc_in_row0 (HiFi-GAN: the
@@ -137,15 +141,15 @@ typedef struct {
 int mtts_conv1d_f32(const mtts_conv_params* p, void* stream);
 
 /* Tensor-core linear layer (wgmma, sm_90a): Y[M,N] = post(pre(X)[M,K] . W[N,K]^T + bias) (+ R) with
- * fp32-grade accuracy from split operands (fp32 accumulation in registers).  w_planes: (3, N, K) bf16 [BF16X3] or
- * (2, N, K) fp16 [F16X2] row-major; scratch receives the activation planes
+ * fp32-grade accuracy from split operands (fp32 accumulation in registers).  w_planes: (3, N, K) bf16 [BF16X3],
+ * (2, N, K) fp16 [F16X2] or (1, N, K) fp16 [F16, half precision] row-major; scratch receives the activation planes
  * (mtts_linear_tc_scratch_bytes(rows_cap, K), rows_cap >= M).  K %% 8 == 0. */
 int64_t mtts_linear_tc_scratch_bytes(int64_t rows_cap, int32_t K);
 int mtts_linear_tc_f32(const float* x, int32_t ldx, int64_t M, int32_t K, const void* w_planes, int32_t N,
                        const float* bias, const float* res, int32_t ldr, float* y, int32_t ldy,
                        int32_t pre_act, float pre_slope, int32_t post_act,
                        void* scratch, int64_t scratch_bytes, int64_t rows_cap, int32_t fmt, void* stream);
-/* fp32 (rows, C) with row stride ldx -> operand planes (3 | 2, rows, C) of `fmt` (the split the kernels apply to
+/* fp32 (rows, C) with row stride ldx -> operand planes (3 | 2 | 1, rows, C) of `fmt` (the split the kernels apply to
  * activations; the host side uses it to pack weights once).  C %% 4 == 0, x 16-byte aligned. */
 int mtts_split_planes_f32(const float* x, int32_t ldx, int64_t rows, int32_t C, void* planes, int32_t fmt, void* stream);
 
@@ -172,7 +176,7 @@ typedef struct {
   /* optional: write the output as three bf16 planes (row b*Tq + t, stride o_planes_ld) for a following
    * tensor-core GEMM; o may then be NULL */
   void* o_planes; int64_t o_plane_stride; int32_t o_planes_ld;
-  int32_t o_planes_fmt;                    /* MTTS_TC_BF16X3 | MTTS_TC_F16X2 */
+  int32_t o_planes_fmt;                    /* MTTS_TC_BF16X3 | MTTS_TC_F16X2 | MTTS_TC_F16 */
 } mtts_attn_params;
 int mtts_attention_f32(const mtts_attn_params* p, void* stream);
 /* Opt-in: AR-step attention (Tq == Tk <= 64, even head count, dh 64 | 96) with at least `min_len` rows runs on the
@@ -337,7 +341,7 @@ typedef struct {
 
 typedef struct {
   int32_t n_layers, d_model, n_heads, ff_dim, conv_ff;
-  int32_t engine;                      /* 0: fp32 FFMA everywhere; wgmma for GEMMs with M >= 128: 1 = BF16X3, 2 = F16X2 operands */
+  int32_t engine;                      /* 0: fp32 FFMA everywhere; wgmma for GEMMs with M >= 128: 1 = BF16X3, 2 = F16X2, 3 = F16 operands */
   const mtts_encoder_layer* layers;    /* HOST array of n_layers entries */
 } mtts_encoder;
 
@@ -399,7 +403,7 @@ typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv
 
 typedef struct {
   int32_t in_channels, out_channels, hidden, k, n_stacks, n_blocks;
-  int32_t engine;                      /* 0: fp32 FFMA; wgmma for the eligible convs: 1 = BF16X3, 2 = F16X2 */
+  int32_t engine;                      /* 0: fp32 FFMA; wgmma for the eligible convs: 1 = BF16X3, 2 = F16X2, 3 = F16 */
   const float *w_first, *b_first;      /* packed (k, Cin, hidden) */
   const float *w_last, *b_last;        /* packed (k, hidden, Cout) */
   const mtts_conv_block* blocks;       /* HOST array [n_stacks*n_blocks] */

@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libmegatts2_b200.so")
 
 ABI_VERSION = 3
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_TANH = 0, 1, 2, 3
-TC_BF16X3, TC_F16X2 = 0, 1
+TC_BF16X3, TC_F16X2, TC_F16 = 0, 1, 2
 PAD_ZERO, PAD_REFLECT, PAD_REPLICATE = 0, 1, 2
 
 vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float

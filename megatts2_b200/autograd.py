@@ -50,6 +50,13 @@ def _tc_ok(M, K, N):
             (N in (32, 64) or (N >= 128 and N % 32 == 0)) and not (K < 64 and N != 32))
 
 
+def _train_fmt():
+    """operand format of the training products: fp32-grade always - the half-precision f16 inference engine trains on
+    f16x2 operands (single-pass fp16 gradients underflow)"""
+    e = pack.default_engine()
+    return pack.FMT_F16X2 if e == pack.ENGINE_F16 else pack.engine_fmt(e)
+
+
 def matmul_nt(a, b):
     """a (M, K) @ b (N, K)^T -> (M, N), fp32-grade: tensor cores when the shape is eligible, else the fp32 batched matmul."""
     M, K = a.shape
@@ -57,7 +64,7 @@ def matmul_nt(a, b):
     if M == 0 or N == 0:
         return torch.zeros(M, N, dtype=_F32, device=a.device)
     if _tc_ok(M, K, N):
-        fmt = pack.engine_fmt(pack.default_engine())
+        fmt = _train_fmt()
         return ops.linear_tc(_c(a), pack.pack_tc_planes(_c(b), fmt))
     return bmm(a, b, 1, 1, M, N, K, (0, 0, a.stride(0), a.stride(1)), (0, 0, b.stride(1), b.stride(0)))[0, 0]
 
@@ -92,7 +99,7 @@ class LinearFn(torch.autograd.Function):
         act = L.ACT_RELU if relu else L.ACT_NONE
         M, K = x2.shape
         if _tc_ok(M, K, w.shape[0]):      # bias + activation ride in the tap-GEMM's epilogue on both engines
-            y = ops.linear_tc(x2, pack.pack_tc_planes(_c(w), pack.engine_fmt(pack.default_engine())), b, post_act=act)
+            y = ops.linear_tc(x2, pack.pack_tc_planes(_c(w), _train_fmt()), b, post_act=act)
         else:
             y = ops.linear(x2, pack.pack_linear(w), b, post_act=act)
         ctx.save_for_backward(x2, w, y if relu else None)

@@ -5,6 +5,8 @@
 //                    whenever x is); three products x1*w1 | x1*w2' + x2'*w1, the correction accumulator is scaled by 2^-11
 //                    in the epilogue.  22 significant bits per operand: the dropped x2*w2 term is 2^-22 relative, below
 //                    the rounding noise of an fp32 dot product; half the MMAs and two thirds of the operand bytes.
+//   NP = 1 (f16):    x ~ fp16(x), ONE product x1*w1 into one accumulator - the opt-in half-precision inference engine, not
+//                    fp32-grade (11 significant bits per operand, fp32 accumulation); a sixth of bf16x3's MMAs.
 // Eligible wherever Cin % 8 == 0, Cin >= 32, Cout in {32, 64, >= 128 and % 32 == 0} and B*T >= 128; everything else
 // stays on the exact FFMA engine (tapconv.cu).  Reference layers: modules/convnet.py:13-18, modules/transformer.py:16-102,
 // the speechbrain HiFi-GAN generator (ResBlock1 convs, ConvTranspose1d upsamplers).
@@ -64,7 +66,9 @@ constexpr int CTC_THREADS = 384;       // warps 0-7: two consumer warpgroups, wa
 constexpr int CTC_PRODUCER_REGS = 40, CTC_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
 template <int BN, int SWB, int NP = 3, int HALO = 0>
 struct ConvTcCfg {
-  static constexpr int ROWS = BN == 128 ? 64 : 128;       // output rows of a work item
+  // output rows of a work item.  NP = 1 keeps 64 rows at BN = 128 although its single accumulator would fit a 128-row item:
+  // the 64-row item measured faster over the PLM / ADM / vocoder shapes (DESIGN.md section 4)
+  static constexpr int ROWS = BN == 128 ? 64 : 128;
   static constexpr int HALVES = ROWS / 64;                 // m64 MMAs per product
   static_assert(!HALO || ROWS == 128, "the halo form keeps 128-row tiles");
   static constexpr int BK = SWB / 2;                       // bf16 elements per swizzled row
@@ -73,7 +77,7 @@ struct ConvTcCfg {
   static constexpr int STAGE = HALO ? NP * B_PLANE : NP * (A_PLANE + B_PLANE);
   // halo-tile buffers: a tile's rows are requested when the buffer of the tile A_BUFS back is released, i.e. A_BUFS - 1 tiles
   // ahead, so the next tiles' rows are in flight while this one's MMAs and epilogue run
-  static constexpr int A_BUFS = HALO ? (SWB == 64 ? 4 : (NP == 2 ? 3 : 2)) : 0;
+  static constexpr int A_BUFS = HALO ? ((SWB == 64 || NP == 1) ? 4 : (NP == 2 ? 3 : 2)) : 0;
   static constexpr int A_REGION = A_BUFS * NP * A_PLANE;
   static constexpr int EPI_STAGE = 8 * 16 * 20 * 4;          // epilogue transpose buffers: 8 warps x [16 rows][20 floats]
   static constexpr int STAGES_RAW = (227 * 1024 - 1024 - 256 - EPI_STAGE - A_REGION) / STAGE;
@@ -185,6 +189,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   setmaxnreg_inc<CTC_CONSUMER_REGS>();
   constexpr float CS = NP == 2 ? F16X2_INV_SCALE : 1.0f;   // weight of the correction accumulator (exact: a power of two)
   constexpr bool BF16 = NP == 3;
+  constexpr int NCOR = NP == 1 ? 1 : BN / 2;               // NP = 1: no correction accumulator
   const int wg = warp >> 2, w4 = warp & 3;
   const int chunk = lane & 3, rsub = lane >> 2;
   const int splits = HALO ? 1 : g.splits;
@@ -202,7 +207,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   // shared buffer and ALL global traffic of the epilogue (y, residual, accumulate, operand planes) is issued as 8 rows x
   // 64 contiguous bytes per instruction.
   float* stg = epi_stage + warp * (16 * 20);
-  float acc[HALVES][BN / 2], cor[HALVES][BN / 2];
+  float acc[HALVES][BN / 2], cor[HALVES][NCOR];
   // Turns on the tensor pipe: warpgroup wg waits on barrier 1 + wg before it issues the MMAs of its item li (li > 0); the
   // other warpgroup arrives there once it has issued all MMAs of item li - 1.  Arrivals are made only for an item that
   // exists, so no barrier is left half-arrived when the CTA exits.
@@ -247,7 +252,9 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
           const uint32_t aa = a_addr + hv * 64 * SWB + ks * 32;
           const uint64_t a1 = wgmma_desc_shifted(desc_base, aa, HALO ? g.bo_mode : 0);
           const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::A_PLANE, HALO ? g.bo_mode : 0);
-          if constexpr (NP == 2) {
+          if constexpr (NP == 1) {
+            Wgmma<BN>::template mma<BF16>(acc[hv], a1, b1, f);       // x1 w1: the only product
+          } else if constexpr (NP == 2) {
             Wgmma<BN>::template mma<BF16>(cor[hv], a1, b2, f);       // x1 w2'
             Wgmma<BN>::template mma<BF16>(cor[hv], a2, b1, 1u);      // x2' w1
             Wgmma<BN>::template mma<BF16>(acc[hv], a1, b1, f);       // x1 w1
@@ -274,7 +281,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
 #pragma unroll
     for (int hv = 0; hv < HALVES; ++hv) {
       wgmma_fence_regs(acc[hv]);
-      wgmma_fence_regs(cor[hv]);
+      if constexpr (NP > 1) wgmma_fence_regs(cor[hv]);
     }
     if (lane == 0) {
       if (prev >= 0) mbar_arrive(empty_bar + 8 * prev);
@@ -298,10 +305,15 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {                 // fragment columns 8 (2u + h) + 2 (lane % 4) + {0, 1}, rows lane / 4 + {0, 8}
           const int j = 2 * u + h, c = 8 * h + 2 * chunk;
-          *reinterpret_cast<float2*>(stg + rsub * 20 + c) =
-              make_float2(fmaf(cor[hv][4 * j + 0], CS, acc[hv][4 * j + 0]), fmaf(cor[hv][4 * j + 1], CS, acc[hv][4 * j + 1]));
-          *reinterpret_cast<float2*>(stg + (rsub + 8) * 20 + c) =
-              make_float2(fmaf(cor[hv][4 * j + 2], CS, acc[hv][4 * j + 2]), fmaf(cor[hv][4 * j + 3], CS, acc[hv][4 * j + 3]));
+          if constexpr (NP == 1) {
+            *reinterpret_cast<float2*>(stg + rsub * 20 + c) = make_float2(acc[hv][4 * j + 0], acc[hv][4 * j + 1]);
+            *reinterpret_cast<float2*>(stg + (rsub + 8) * 20 + c) = make_float2(acc[hv][4 * j + 2], acc[hv][4 * j + 3]);
+          } else {
+            *reinterpret_cast<float2*>(stg + rsub * 20 + c) =
+                make_float2(fmaf(cor[hv][4 * j + 0], CS, acc[hv][4 * j + 0]), fmaf(cor[hv][4 * j + 1], CS, acc[hv][4 * j + 1]));
+            *reinterpret_cast<float2*>(stg + (rsub + 8) * 20 + c) =
+                make_float2(fmaf(cor[hv][4 * j + 2], CS, acc[hv][4 * j + 2]), fmaf(cor[hv][4 * j + 3], CS, acc[hv][4 * j + 3]));
+          }
         }
         __syncwarp();
         float4 bvec = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -336,7 +348,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
 #pragma unroll
               for (int e = 0; e < 4; ++e) v[e] = act_apply(v[e], g.op_act, g.op_slope);
             }
-            store_planes4(g.op, g.op_stride, oo + i * ostep + u * 16, v, NP == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3, g.ovf);
+            store_planes4(g.op, g.op_stride, oo + i * ostep + u * 16, v, 3 - NP, g.ovf);   // the format of this kernel's NP
           }
         }
         __syncwarp();   // the staging buffer is reused by the next unit
@@ -498,7 +510,8 @@ split_pad_kernel(const float* __restrict__ x, int64_t x_sb, int ldx, int T, int 
 }
 
 // Materialise the padding rows of plane buffers whose interior rows were written by a producer epilogue:
-// planes (3, B, Tp, C) bf16 with hl leading halo rows; reflect / replicate / zero about the T interior rows.
+// planes (3 | 2 | 1, B, Tp, C) of `fmt` (one plane per gridDim.z) with hl leading halo rows; reflect / replicate / zero
+// about the T interior rows.
 __global__ void __launch_bounds__(256)
 halo_fill_kernel(__nv_bfloat16* __restrict__ planes, int64_t plane_stride, int T, int C, int hl, int Tp, int pad_mode) {
   pdl_entry();
@@ -522,14 +535,15 @@ halo_fill_kernel(__nv_bfloat16* __restrict__ planes, int64_t plane_stride, int T
   }
 }
 
-int halo_fill(void* planes_base, int B, int T, int C, int hl, int hr, int pad_mode, cudaStream_t st) {
+int halo_fill(void* planes_base, int B, int T, int C, int hl, int hr, int pad_mode, int fmt, cudaStream_t st) {
   MTTS_REQUIRE(planes_base && C % 8 == 0 && hl >= 0 && hr >= 0, "bad arguments");
+  MTTS_REQUIRE(fmt == MTTS_TC_BF16X3 || fmt == MTTS_TC_F16X2 || fmt == MTTS_TC_F16, "unknown operand format");
   if (hl + hr == 0 || B <= 0) return 0;
   __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>((((uintptr_t)planes_base) + 1023) & ~(uintptr_t)1023);
   const int Tp = T + hl + hr;
   const int64_t plane_stride = (int64_t)B * Tp * C;
   const int work = (hl + hr) * (C / 8);
-  dim3 grid((unsigned)cdiv64(work, 256), (unsigned)B, 3);
+  dim3 grid((unsigned)cdiv64(work, 256), (unsigned)B, (unsigned)(3 - fmt));
   launch_k(halo_fill_kernel, grid, 256, 0, st, planes, plane_stride, T, C, hl, Tp, pad_mode);
   MTTS_CHECK_LAUNCH();
   return 0;
@@ -665,7 +679,7 @@ static int cmap_get(const void* p, uint64_t d0, uint64_t d1, uint64_t d2, uint32
   cuuint32_t box[3] = {b0, b1, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   CUtensorMap m;
-  CUresult r = g_enc(&m, fmt == MTTS_TC_F16X2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank,
+  CUresult r = g_enc(&m, fmt != MTTS_TC_BF16X3 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank,
                      const_cast<void*>(p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      swb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -683,8 +697,8 @@ template <int BN, int SWB, int NP, int HALO = 0>
 static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, cudaStream_t st) {
   using Cfg = ConvTcCfg<BN, SWB, NP, HALO>;
   // one bit per instantiation in the per-device table (the max-dynamic-shared-memory attribute is per device)
-  constexpr int slot = HALO ? 12 + (BN == 64 ? 0 : 1) + 2 * (NP == 3 ? 0 : 1)
-                            : (BN == 128 ? 0 : BN == 64 ? 1 : 2) + 3 * (SWB == 128 ? 0 : 1) + 6 * (NP == 3 ? 0 : 1);
+  constexpr int slot = HALO ? 18 + (BN == 64 ? 0 : 1) + 2 * (3 - NP)
+                            : (BN == 128 ? 0 : BN == 64 ? 1 : 2) + 3 * (SWB == 128 ? 0 : 1) + 6 * (3 - NP);
   static_assert(slot < 32, "attribute slots");
   const int dev = cur_device();
   const int sms = cur_device_sms();
@@ -714,7 +728,7 @@ static int conv_tc_dispatch(const ConvTcMaps& maps, const ConvTcArgs& a, int BN,
 
 bool conv_tc_eligible(const mtts_conv_params& p) {
   if (!p.w_tc || !p.tc_scratch) return false;
-  if (p.tc_fmt != MTTS_TC_BF16X3 && p.tc_fmt != MTTS_TC_F16X2) return false;
+  if (p.tc_fmt != MTTS_TC_BF16X3 && p.tc_fmt != MTTS_TC_F16X2 && p.tc_fmt != MTTS_TC_F16) return false;
   if (p.stride != 1 || p.in_lens) return false;
   if (p.out_shift != 0 && (p.out_shift % 4 != 0 || p.y_batch_elems % 4 != 0 || p.res || p.accumulate || p.tc_out_planes || !p.y))
     return false;
@@ -760,7 +774,7 @@ static TcPlan tc_plan(const CtcEnv& env, int sms, const mtts_conv_params& p, int
     const int64_t rows = (int64_t)p.B * p.Tout;
     const int64_t mt = (int64_t)p.B * cdiv64(p.Tout, 128);
     const int nk = (p.Cin + 63) / 64;
-    const double mm = 4.0 * (np == 2 ? 3 : 6);                       // MMAs per 64-wide K-slab
+    const double mm = 4.0 * (np == 1 ? 1 : np == 2 ? 3 : 6);        // MMAs per 64-wide K-slab
     double best = 1e30;
     const int cands[3] = {128, 64, 32};
     for (int i = 0; i < 3; ++i) {
@@ -818,7 +832,7 @@ static TcPlan tc_plan(const CtcEnv& env, int sms, const mtts_conv_params& p, int
         if (sk >= 2 && (int64_t)sk * rows * p.Cout * 4 <= p.tc_partial_bytes) {
           const int64_t tiles_bn = (int64_t)p.B * cdiv64(p.Tout, 128) * cdiv64(p.Cout, BN);
           const double waves = (double)cdiv64(tiles_bn, sms);
-          const double mmas = 4.0 * (2 * np);                                                 // MMAs per 64-wide K-slab
+          const double mmas = 4.0 * (np == 1 ? 1 : 2 * np);                                   // MMAs per 64-wide K-slab (modelled)
           const double cost_now = waves * nk * mmas * (BN == 128 ? 65.0 : 55.0);                // cycles per CTA
           const double cost_split = (double)cdiv64(nk, sk) * mmas * 65.0 + (ln_rides ? env.ln_red : 9000.0);   // + reduction kernel
           if (cost_split < env.margin * cost_now) { splits = sk; BN = 128; }
@@ -841,7 +855,7 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   const CtcEnv& env = ctc_env();
   const int sms = cur_device_sms();
   const int fmt = p.tc_fmt;
-  const int np = fmt == MTTS_TC_F16X2 ? 2 : 3;
+  const int np = 3 - fmt;                                     // operand planes
   int32_t* ovf = tc_ovf_ptr();
   const int halo = p.dil * (p.k - 1);
   const int hl = p.pad, Tp = p.Tout + halo;
@@ -869,7 +883,7 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
     MTTS_TRY(cmap_get((const __nv_bfloat16*)p.w_tc + (int64_t)q * p.k * p.Cout * p.Cin, (uint64_t)p.Cin,
                       (uint64_t)p.k * p.Cout, 0, SWB / 2, BN, SWB, fmt, &maps.b[q]));
   }
-  if (np == 2) { maps.a[2] = maps.a[1]; maps.b[2] = maps.b[1]; }
+  for (int q = np; q < 3; ++q) { maps.a[q] = maps.a[np - 1]; maps.b[q] = maps.b[np - 1]; }   // unused
   ConvTcArgs a;
   a.B = p.B; a.T = p.Tout; a.Cin = p.Cin; a.Cout = p.Cout; a.k = p.k; a.dil = p.dil;
   a.bias = p.bias; a.res = p.res; a.res_sb = p.res_batch_stride; a.ldr = p.ldr;
@@ -881,11 +895,15 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   a.splits = splits; a.partial = reinterpret_cast<float*>(p.tc_partial);
   a.fmt = fmt; a.ovf = ovf; a.bo_mode = env.halo_bo; a.row0 = p.tc_in_row0;
   if (halo_form) {
-    if (SWB == 64) return np == 2 ? conv_tc_launch<32, 64, 2, 1>(maps, a, st) : conv_tc_launch<32, 64, 3, 1>(maps, a, st);
-    return np == 2 ? conv_tc_launch<64, 128, 2, 1>(maps, a, st) : conv_tc_launch<64, 128, 3, 1>(maps, a, st);
+    if (SWB == 64)
+      return np == 1 ? conv_tc_launch<32, 64, 1, 1>(maps, a, st)
+           : np == 2 ? conv_tc_launch<32, 64, 2, 1>(maps, a, st) : conv_tc_launch<32, 64, 3, 1>(maps, a, st);
+    return np == 1 ? conv_tc_launch<64, 128, 1, 1>(maps, a, st)
+         : np == 2 ? conv_tc_launch<64, 128, 2, 1>(maps, a, st) : conv_tc_launch<64, 128, 3, 1>(maps, a, st);
   }
   if (splits > 1) {
-    MTTS_TRY(np == 2 ? (conv_tc_launch<128, 128, 2>(maps, a, st)) : (conv_tc_launch<128, 128, 3>(maps, a, st)));
+    MTTS_TRY(np == 1 ? (conv_tc_launch<128, 128, 1>(maps, a, st))
+           : np == 2 ? (conv_tc_launch<128, 128, 2>(maps, a, st)) : (conv_tc_launch<128, 128, 3>(maps, a, st)));
     // the rows' LayerNorm rides on the reduction when the caller asked for it and a row is 3 / 4 / 6 / 8 x 128 wide
     if (ln && ln->po.p && a.y && !a.op && a.out_shift == 0 && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384) &&
         p.ldy % 4 == 0 && ln->po.ld % 4 == 0 && ln->po.stride % 4 == 0) {
@@ -903,21 +921,22 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
     MTTS_CHECK_LAUNCH();
     return 0;
   }
-  return np == 2 ? conv_tc_dispatch<2>(maps, a, BN, SWB, st) : conv_tc_dispatch<3>(maps, a, BN, SWB, st);
+  return np == 1 ? conv_tc_dispatch<1>(maps, a, BN, SWB, st)
+       : np == 2 ? conv_tc_dispatch<2>(maps, a, BN, SWB, st) : conv_tc_dispatch<3>(maps, a, BN, SWB, st);
 }
 
 // diagnostics: the plan conv_tc() would pick for a stride-1 tap-GEMM of this shape on `sms` SMs; out = {BN, splits, CTA pair
 // (always 0: no pair kernels on sm_90), halo form (0 | 1), K-slab bytes}
 int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides, int32_t* out5) {
   MTTS_REQUIRE(out5 && sms > 0 && B > 0 && T > 0 && Cin > 0 && Cout > 0 && k > 0 && dil > 0, "bad arguments");
-  MTTS_REQUIRE(fmt == MTTS_TC_BF16X3 || fmt == MTTS_TC_F16X2, "unknown operand format");
+  MTTS_REQUIRE(fmt == MTTS_TC_BF16X3 || fmt == MTTS_TC_F16X2 || fmt == MTTS_TC_F16, "unknown operand format");
   mtts_conv_params p;
   memset(&p, 0, sizeof(p));
   p.B = B; p.Tin = T + dil * (k - 1); p.Tout = T; p.Cin = Cin; p.Cout = Cout; p.k = k; p.stride = 1; p.dil = dil;
   static float dummy;
   p.y = &dummy;
   if (partial_bytes > 0) { p.tc_partial = &dummy; p.tc_partial_bytes = partial_bytes; }
-  const TcPlan pl = tc_plan(ctc_env(), sms, p, fmt == MTTS_TC_F16X2 ? 2 : 3, ln_rides != 0);
+  const TcPlan pl = tc_plan(ctc_env(), sms, p, 3 - fmt, ln_rides != 0);
   out5[0] = pl.BN; out5[1] = pl.splits; out5[2] = 0; out5[3] = pl.halo_form ? 1 : 0; out5[4] = pl.SWB;
   return 0;
 }
@@ -936,10 +955,10 @@ int split_pad(const float* x, int64_t x_sb, int ldx, int B, int T, int C, int hl
   return 0;
 }
 
-// fp32 (rows, C) -> operand planes (3 | 2, rows, C): the activation split, exposed for packing weights on the device
+// fp32 (rows, C) -> operand planes (3 | 2 | 1, rows, C): the activation split, exposed for packing weights on the device
 int split_planes(const float* x, int ldx, int64_t rows, int C, void* planes, int fmt, cudaStream_t st) {
   MTTS_REQUIRE(x && planes && C > 0 && C % 4 == 0 && ldx % 4 == 0 && ((((uintptr_t)x) | ((uintptr_t)planes)) & 15) == 0, "bad arguments");
-  MTTS_REQUIRE(fmt == MTTS_TC_BF16X3 || fmt == MTTS_TC_F16X2, "unknown operand format");
+  MTTS_REQUIRE(fmt == MTTS_TC_BF16X3 || fmt == MTTS_TC_F16X2 || fmt == MTTS_TC_F16, "unknown operand format");
   if (rows <= 0) return 0;
   MTTS_REQUIRE(rows < (int64_t)1 << 31, "too many rows");
   const int64_t total4 = rows * C / 4;

@@ -745,7 +745,7 @@ static int hifigan_forward(const mtts_hifigan* h, const float* mel, int64_t mel_
           c1.tc_out_act = MTTS_ACT_LEAKY; c1.tc_out_slope = 0.1f;
           if (!conv_tc_eligible(c1)) return fail(MTTS_ERR_UNSUPPORTED, "%s: fused ResBlock conv not eligible (C=%lld L=%lld)", "hifigan", Co, Lo);
           MTTS_TRY(conv1d(c1, st));
-          MTTS_TRY(halo_fill(planes2, B, Lo, Co, h2, h2, MTTS_PAD_REFLECT, st));
+          MTTS_TRY(halo_fill(planes2, B, Lo, Co, h2, h2, MTTS_PAD_REFLECT, hfmt, st));
           const bool lastm = (m == 2);
           mtts_conv_params c2 = conv_same_params(nullptr, rb.w2[m], rb.b2[m], lastm ? z : xr, B, Lo, Co, Co, rb.k, 1, MTTS_PAD_REFLECT);
           c2.w_tc = rb.w2_tc[m]; c2.tc_scratch = planes2; c2.tc_scratch_bytes = tc.bytes; c2.tc_presplit = 1; c2.tc_fmt = hfmt;
@@ -762,7 +762,7 @@ static int hifigan_forward(const mtts_hifigan* h, const float* mel, int64_t mel_
           }
           if (!conv_tc_eligible(c2)) return fail(MTTS_ERR_UNSUPPORTED, "%s: fused ResBlock conv not eligible (C=%lld L=%lld)", "hifigan", Co, Lo);
           MTTS_TRY(conv1d(c2, st));
-          if (!lastm) MTTS_TRY(halo_fill(tc.scratch, B, Lo, Co, rb.dil[m + 1] * (rb.k - 1) / 2, rb.dil[m + 1] * (rb.k - 1) / 2, MTTS_PAD_REFLECT, st));
+          if (!lastm) MTTS_TRY(halo_fill(tc.scratch, B, Lo, Co, rb.dil[m + 1] * (rb.k - 1) / 2, rb.dil[m + 1] * (rb.k - 1) / 2, MTTS_PAD_REFLECT, hfmt, st));
           (void)h1;
           xcur = xr;
         }

@@ -13,7 +13,10 @@ namespace mtts {
 //                  (x0w0 | x0w1' + x1'w0, the second accumulator scaled by 2^-11 in the epilogue).  fp16 range:
 //                  |x| > 65504 cannot be represented - the split then poisons the value (inf/NaN propagate to the
 //                  output) and raises the caller-registered overflow flag (mtts_tc_overflow_bind).
-enum { MTTS_TC_BF16X3 = 0, MTTS_TC_F16X2 = 1 };
+//   fmt 2  f16   : x ~ p0 = fp16(x) (one fp16 plane, round-to-nearest; 11 significant bits); ONE MMA per product.
+//                  Not fp32-grade: the opt-in half-precision inference engine.  Same fp16 range and flag as f16x2.
+// The number of planes of fmt is 3 - fmt.
+enum { MTTS_TC_BF16X3 = 0, MTTS_TC_F16X2 = 1, MTTS_TC_F16 = 2 };
 constexpr float F16X2_SCALE = 2048.0f;           // 2^11
 constexpr float F16X2_INV_SCALE = 1.0f / 2048.0f;
 
@@ -24,26 +27,28 @@ struct PlanesOut {
   int ld;                // row stride (elements)
   int act;               // activation applied to the planes copy (the consumer's pre-activation)
   float slope;
-  int fmt;               // MTTS_TC_BF16X3 | MTTS_TC_F16X2
-  int32_t* ovf;          // f16x2 range flag (device, may be null)
+  int fmt;               // MTTS_TC_BF16X3 | MTTS_TC_F16X2 | MTTS_TC_F16
+  int32_t* ovf;          // fp16 range flag (device, may be null)
 };
 
 // 4 consecutive elements -> one 8-byte store per plane
 __device__ __forceinline__ void store_planes4(__nv_bfloat16* planes, int64_t plane_stride, int64_t off, const float* v,
                                               int fmt = MTTS_TC_BF16X3, int32_t* ovf = nullptr) {
-  if (fmt == MTTS_TC_F16X2) {
+  if (fmt == MTTS_TC_F16X2 || fmt == MTTS_TC_F16) {
     // two elements per conversion instruction (cvt.rn.f16x2.f32); the range check is one NaN-propagating max per element
     const __half2 h01 = __floats2half2_rn(v[0], v[1]), h23 = __floats2half2_rn(v[2], v[3]);   // +-inf beyond the fp16 range
-    const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-    const __half2 l01 = __floats2half2_rn((v[0] - f01.x) * F16X2_SCALE, (v[1] - f01.y) * F16X2_SCALE);   // exact difference,
-    const __half2 l23 = __floats2half2_rn((v[2] - f23.x) * F16X2_SCALE, (v[3] - f23.y) * F16X2_SCALE);   // exact scaling
     uint2 o;
     o.x = *reinterpret_cast<const uint32_t*>(&h01);
     o.y = *reinterpret_cast<const uint32_t*>(&h23);
     *reinterpret_cast<uint2*>(planes + off) = o;
-    o.x = *reinterpret_cast<const uint32_t*>(&l01);
-    o.y = *reinterpret_cast<const uint32_t*>(&l23);
-    *reinterpret_cast<uint2*>(planes + plane_stride + off) = o;
+    if (fmt == MTTS_TC_F16X2) {
+      const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
+      const __half2 l01 = __floats2half2_rn((v[0] - f01.x) * F16X2_SCALE, (v[1] - f01.y) * F16X2_SCALE);   // exact difference,
+      const __half2 l23 = __floats2half2_rn((v[2] - f23.x) * F16X2_SCALE, (v[3] - f23.y) * F16X2_SCALE);   // exact scaling
+      o.x = *reinterpret_cast<const uint32_t*>(&l01);
+      o.y = *reinterpret_cast<const uint32_t*>(&l23);
+      *reinterpret_cast<uint2*>(planes + plane_stride + off) = o;
+    }
     if (ovf) {
       float m;
       asm("{\n\t.reg .f32 t0, t1, t2, t3;\n\tabs.f32 t0, %1;\n\tabs.f32 t1, %2;\n\tabs.f32 t2, %3;\n\tabs.f32 t3, %4;\n\t"
@@ -79,7 +84,10 @@ int cur_device_sms();
 int set_sm_limit(int n);
 int set_launch_policy(int sm_limit, int allow_pairs, int allow_pdl);
 int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides, int32_t* out5);
-static inline int tc_fmt_of_engine(int engine) { return engine == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3; }
+// engine 1 | 2 | 3 (bf16x3 | f16x2 | f16) -> operand format; the one place that maps engines to formats
+static inline int tc_fmt_of_engine(int engine) {
+  return engine == 3 ? MTTS_TC_F16 : engine == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3;
+}
 int layernorm_ex(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr, float* y,
                  int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, PlanesOut po, cudaStream_t st);
 int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st);
@@ -94,7 +102,7 @@ struct LnFuse {
   int done;
 };
 int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln = nullptr);
-int halo_fill(void* planes_base, int B, int T, int C, int hl, int hr, int pad_mode, cudaStream_t st);
+int halo_fill(void* planes_base, int B, int T, int C, int hl, int hr, int pad_mode, int fmt, cudaStream_t st);
 int64_t linear_tc_scratch_bytes(int64_t rows_cap, int K);
 int linear_tc(const float* x, int ldx, int64_t M, int K, const void* w_planes, int N, const float* bias,
               const float* res, int ldr, float* y, int ldy, int pre_act, float pre_slope, int post_act,

@@ -364,7 +364,7 @@ class HifiganGenerator(pack.PlanMixin, nn.Module):
                 s.up_factor[i], s.up_kernel[i] = u, k
                 wp, bp = pack.pack_conv_transpose(self.ups[i].weight, self.ups[i].bias, u)
                 s.w_up[i], s.b_up[i] = pl.p(wp), pl.p(bp)
-                if engine >= 1:     # (2, Cin, s*Cout) fp32 -> (3 | 2, 2, s*Cout, Cin) operand planes
+                if engine >= 1:     # (2, Cin, s*Cout) fp32 -> (3 | 2 | 1, 2, s*Cout, Cin) operand planes
                     tup = pack.pack_conv_transpose_tc_planes(wp, fmt)
                     pl.keep.append(tup)
                     s.w_up_tc[i] = tup.data_ptr()
@@ -535,13 +535,16 @@ class Megatts(nn.Module):
         overlapped one even when the budget's default is 0.  Waveforms are identical either way (the vocoder has no
         batch- or grid-dependent reduction order); the ADM / MRTE dense layers pick their K split from the SM budget, so
         their fp32 results move within rounding noise.
-        ``check_range``: with the f16x2 operand engine, read the range flag after the batch (one 4-byte readback) and,
-        if any activation left the fp16 range, redo the batch on the bf16x3 engine."""
+        ``check_range``: with an fp16 operand engine (f16x2, or the half-precision f16) as the default engine, read the
+        range flag after the batch (one 4-byte readback) and, if any activation left the fp16 range, redo the batch on the
+        bf16x3 engine.  The check keys off the default engine (``MEGATTS2_ENGINE`` / ``pack.engine_scope``): a module
+        whose ``.engine`` is set by hand - e.g. only the vocoder on f16 (``hifi_gan.generator.engine =
+        pack.ENGINE_F16``) - is not guarded by it."""
         dev = phone_tokens.device
         out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt)
-        if check_range and pack.default_engine() == pack.ENGINE_F16X2 and ops.tc_overflow(dev):
+        if check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16) and ops.tc_overflow(dev):
             import warnings
-            warnings.warn("megatts2_b200: an activation left the fp16 range of the f16x2 operand split; "
+            warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
                           "re-running this batch on the bf16x3 engine")
             with pack.engine_scope(pack.ENGINE_BF16X3):
                 out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt)

@@ -51,8 +51,8 @@ def conv1d(x, w_packed, bias=None, *, k, stride=1, dil=1, pad=0, pad_mode=L.PAD_
            pre_slope=0.0, post_act=L.ACT_NONE, post_slope=0.0, res=None, out=None, out_scale=1.0, accumulate=False,
            t_out=None, in_lens=None, w_tc=None):
     """x (B,T,Cin) channels-last, w_packed (k,Cin,Cout) -> (B,T_out,Cout).
-    w_tc: optional operand planes, (3,k,Cout,Cin) bf16 [bf16x3] or (2,k,Cout,Cin) fp16 [f16x2] -> the wgmma engine
-    is used when the shape is eligible."""
+    w_tc: optional operand planes, (3,k,Cout,Cin) bf16 [bf16x3], (2,k,Cout,Cin) fp16 [f16x2] or (1,k,Cout,Cin) fp16
+    [f16] -> the wgmma engine is used when the shape is eligible."""
     x = _dev(x, name="x")
     x, x_sb, ldx = _rows(x)
     B, Tin, Cin = x.shape
@@ -96,16 +96,17 @@ def linear(x, w_packed, bias=None, **kw):
 
 
 def _plane_fmt(w_planes):
+    """operand format of weight planes: bf16 -> bf16x3; fp16 -> f16x2 (two planes) or f16 (one plane)"""
     if w_planes.dtype == torch.float16:
-        return L.TC_F16X2
+        return L.TC_F16 if w_planes.shape[0] == 1 else L.TC_F16X2
     if w_planes.dtype == torch.bfloat16:
         return L.TC_BF16X3
-    raise L.MttsError(f"operand planes must be bf16 (bf16x3) or fp16 (f16x2), got {w_planes.dtype}")
+    raise L.MttsError(f"operand planes must be bf16 (bf16x3) or fp16 (f16x2, f16), got {w_planes.dtype}")
 
 
 def linear_tc(x, w_planes, bias=None, *, res=None, pre_act=L.ACT_NONE, pre_slope=0.0, post_act=L.ACT_NONE):
-    """Tensor-core (wgmma) dense layer: x (..., K) fp32, w_planes (3, N, K) bf16 [bf16x3] or (2, N, K) fp16 [f16x2]
-    -> (..., N) fp32."""
+    """Tensor-core (wgmma) dense layer: x (..., K) fp32, w_planes (3, N, K) bf16 [bf16x3], (2, N, K) fp16 [f16x2] or
+    (1, N, K) fp16 [f16] -> (..., N) fp32."""
     x = _dev(x, name="x")
     shp = x.shape
     x2 = x.reshape(-1, shp[-1])
@@ -316,7 +317,7 @@ def mel_spectrogram(wav, window, fb_w, fb_off, fb_start, n_mels=80, clamp=1e-5, 
     return out
 
 
-# ------------------------------------------------------------------------------ f16x2 range guard
+# ------------------------------------------------------------------------------ fp16 range guard (f16x2, f16)
 _ovf_flags = {}
 
 
@@ -331,7 +332,7 @@ def set_attention_pair_min(min_len):
 
 
 def tc_overflow_bind(device):
-    """Registers (once per device) the int32 flag the f16x2 operand split raises when an activation leaves the
+    """Registers (once per device) the int32 flag the fp16 operand splits raise when an activation leaves the
     fp16 range (|x| > 65504); returns the flag tensor."""
     idx = _dev_index(device)
     flag = _ovf_flags.get(idx)
@@ -344,7 +345,7 @@ def tc_overflow_bind(device):
 
 
 def tc_overflow(device, reset=True):
-    """True if any f16x2 split on `device` saw an out-of-range activation since the last reset (one host sync)."""
+    """True if any fp16 (f16x2 / f16) split on `device` saw an out-of-range activation since the last reset (one host sync)."""
     flag = tc_overflow_bind(device)
     hit = bool(flag.item())
     if hit and reset:

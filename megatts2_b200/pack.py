@@ -11,7 +11,7 @@ import torch
 from . import _lib as L
 
 
-FMT_BF16X3, FMT_F16X2 = 0, 1
+FMT_BF16X3, FMT_F16X2, FMT_F16 = 0, 1, 2
 F16X2_SCALE = 2048.0
 
 
@@ -118,21 +118,25 @@ def cat_rows(*ws):
 
 
 def plane_dtype(fmt):
-    return torch.float16 if fmt == FMT_F16X2 else torch.bfloat16
+    return torch.bfloat16 if fmt == FMT_BF16X3 else torch.float16
 
 
 def pack_tc_planes(w, fmt=FMT_BF16X3):
-    """(N, K) fp32 weight -> tensor-core operand planes, the same split the kernels apply to activations:
+    """(N, K) fp32 weight -> tensor-core operand planes, the same split the kernels apply to activations
+    (a format has 3 - fmt planes):
     bf16x3: (3, N, K) bf16 with w = w1 + w2 + w3 to ~2^-24 (round-to-nearest at every step);
-    f16x2:  (2, N, K) fp16 with w = w1 + w2 * 2^-11 (the residual is stored scaled by 2^11)."""
+    f16x2:  (2, N, K) fp16 with w = w1 + w2 * 2^-11 (the residual is stored scaled by 2^11);
+    f16:    (1, N, K) fp16 with w ~ fp16(w) (round-to-nearest; half precision, not fp32-grade)."""
     w = _f32(w)
     if w.is_cuda:
         if not w.is_contiguous():
             w = w.contiguous()
         N, K = w.shape
-        out = torch.empty(2 if fmt == FMT_F16X2 else 3, N, K, dtype=plane_dtype(fmt), device=w.device)
+        out = torch.empty(3 - fmt, N, K, dtype=plane_dtype(fmt), device=w.device)
         L.check(L.lib().mtts_split_planes_f32(C.c_void_p(w.data_ptr()), K, N, K, C.c_void_p(out.data_ptr()), fmt, _stream()))
         return out
+    if fmt == FMT_F16:
+        return w.to(torch.float16)[None]
     if fmt == FMT_F16X2:
         p1 = w.to(torch.float16)
         p2 = ((w - p1.float()) * F16X2_SCALE).to(torch.float16)
@@ -145,7 +149,7 @@ def pack_tc_planes(w, fmt=FMT_BF16X3):
 
 
 def pack_conv_tc_planes(w, fmt=FMT_BF16X3):
-    """nn.Conv1d weight (Cout, Cin, k) fp32 -> (3 | 2, k, Cout, Cin) operand planes (per-tap K-major B operands)."""
+    """nn.Conv1d weight (Cout, Cin, k) fp32 -> (3 | 2 | 1, k, Cout, Cin) operand planes (per-tap K-major B operands)."""
     w = _f32(w)
     co, ci, k = w.shape
     if w.is_cuda:
@@ -158,7 +162,7 @@ def pack_conv_tc_planes(w, fmt=FMT_BF16X3):
 
 
 def pack_conv_transpose_tc_planes(wp, fmt=FMT_BF16X3):
-    """packed transposed-conv weight (2, Cin, s*Cout) fp32 -> (3 | 2, 2, s*Cout, Cin) operand planes."""
+    """packed transposed-conv weight (2, Cin, s*Cout) fp32 -> (3 | 2 | 1, 2, s*Cout, Cin) operand planes."""
     two, cin, n = wp.shape
     if wp.is_cuda:
         tmp = torch.empty(two, n, cin, dtype=torch.float32, device=wp.device)
@@ -169,7 +173,7 @@ def pack_conv_transpose_tc_planes(wp, fmt=FMT_BF16X3):
     return pack_tc_planes(flat, fmt).reshape(-1, two, n, cin)
 
 
-ENGINE_FFMA, ENGINE_BF16X3, ENGINE_F16X2 = 0, 1, 2
+ENGINE_FFMA, ENGINE_BF16X3, ENGINE_F16X2, ENGINE_F16 = 0, 1, 2, 3
 
 
 _engine_override = None
@@ -194,10 +198,13 @@ class engine_scope:
 
 
 def default_engine() -> int:
-    """Engine for the dense contractions with M >= 128 (MEGATTS2_ENGINE = f16x2 | bf16x3 | ffma):
+    """Engine for the dense contractions with M >= 128 (MEGATTS2_ENGINE = f16x2 | bf16x3 | ffma | f16):
     2 = wgmma with f16x2 operands (default: 3 MMAs per fp32-grade product, |activation| <= 65504 guarded by the
     overflow flag, see ops.tc_overflow), 1 = wgmma with bf16x3 operands (6 MMAs, full fp32 range), 0 = fp32 FFMA
-    everywhere.  All three are fp32-grade; ids are bit-identical between them in the tests."""
+    everywhere.  These three are fp32-grade; ids are bit-identical between them in the tests.
+    3 = wgmma with f16 operands is NOT: the opt-in half-precision inference engine (one fp16 plane per operand, one MMA
+    per product into an fp32 accumulator, the same fp16 range guard).  Its results differ from the others by fp16
+    rounding, and ids may differ too; it is reported separately."""
     import os
     if _engine_override is not None:
         return _engine_override
@@ -206,11 +213,13 @@ def default_engine() -> int:
         return ENGINE_FFMA
     if v in ("bf16x3", "tc", "1"):
         return ENGINE_BF16X3
+    if v in ("f16", "3"):
+        return ENGINE_F16
     return ENGINE_F16X2
 
 
 def engine_fmt(engine: int) -> int:
-    return FMT_F16X2 if engine == ENGINE_F16X2 else FMT_BF16X3
+    return {ENGINE_F16X2: FMT_F16X2, ENGINE_F16: FMT_F16}.get(engine, FMT_BF16X3)
 
 
 _epoch = 0

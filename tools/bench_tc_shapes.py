@@ -2,7 +2,8 @@
 
 For each (shape, variant) runs the op `reps` times inside the library's event trace and reports the main kernel's
 time per launch (the activation split is traced separately) and its rate in fp32-equivalent TFLOP/s
-(2*M*N*K*k; the tensor pipe executes 6 bf16 MMAs per fp32 product, so dense-bf16-equivalent = 6x).
+(2*M*N*K*k; the tensor pipe executes 6 | 3 | 1 16-bit MMAs per product under bf16x3 | f16x2 | f16, so the dense
+16-bit rate is that multiple of it).
 """
 import ctypes as C
 import math
@@ -63,7 +64,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--shapes", type=str, default="", help="comma-separated shape indices (default: all)")
-    ap.add_argument("--fmt", type=str, default="f16x2", choices=["f16x2", "bf16x3"])
+    ap.add_argument("--fmt", type=str, default="f16x2", choices=["f16x2", "bf16x3", "f16"])
     ap.add_argument("--variants", type=str, default="", help="comma-separated variant indices (default: all)")
     args = ap.parse_args()
     reps = args.reps
@@ -75,8 +76,8 @@ def main():
         x = torch.randn(s["B"], s["T"], s["Cin"], generator=g).to(DEV)
         w = torch.randn(s["Cout"], s["Cin"], k, generator=g) / math.sqrt(s["Cin"] * k)
         b = torch.randn(s["Cout"], generator=g).to(DEV)
-        fmt = pack.FMT_F16X2 if args.fmt == "f16x2" else pack.FMT_BF16X3
-        nm = 3 if fmt == pack.FMT_F16X2 else 6
+        fmt = {"f16x2": pack.FMT_F16X2, "bf16x3": pack.FMT_BF16X3, "f16": pack.FMT_F16}[args.fmt]
+        nm = {pack.FMT_F16X2: 3, pack.FMT_BF16X3: 6, pack.FMT_F16: 1}[fmt]
         wp, wt = pack.pack_conv(w.to(DEV)), pack.pack_conv_tc_planes(w.to(DEV), fmt)
         out = torch.empty(s["B"], s["T"], s["Cout"], device=DEV)
         flops = 2.0 * s["B"] * s["T"] * s["Cin"] * s["Cout"] * k
@@ -84,7 +85,7 @@ def main():
         for vname, env in variants:
             os.environ.update(env)
             ms = trace_ms(lambda: ops.conv1d(x, wp, b, out=out, w_tc=wt, k=k, dil=dil, pad=pad, pad_mode=1 if k > 1 else 0), reps)
-            print(f"{s['name']:30s} {vname:30s} {ms:8.3f} ms  {flops / ms / 1e9:7.1f} TFLOP/s fp32-equiv "
+            print(f"{s['name']:30s} {vname:30s} {ms:8.3f} ms  {flops / ms / 1e9:7.1f} TFLOP/s per product "
                   f"({nm * flops / ms / 1e9:7.0f} dense 16-bit, {args.fmt})", flush=True)
         del x, out
         torch.cuda.empty_cache()
