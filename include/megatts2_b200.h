@@ -55,6 +55,9 @@ int mtts_trace_end(char* buf, int32_t buf_len);
  *   BF16X3: x = x1 + x2 + x3 (bf16), products x1w1 + x1w2 + x2w1 + x2w2 + x1w3 + x3w1  -> 6 MMAs, fp32 range
  *   F16X2 : x = x1 + x2' * 2^-11 (fp16, residual stored scaled so it stays in the normal range), products
  *           x1w1 + (x1w2' + x2'w1) * 2^-11 -> 3 MMAs, 22 significant bits per operand; |x| must be <= 65504.
+ *           At the low end x1 is an fp16 subnormal below 2^-14 and both planes are zero below about 2^-35, so
+ *           the representation error is |x - x^| <= 2^-22 |x| + 2^-36, not 2^-22 |x|: tiny operands (training
+ *           gradients) lose their precision, and below 2^-36 they vanish.  BF16X3 has neither edge.
  * F16 is the opt-in half-precision inference format, NOT fp32-grade:
  *   F16   : x ~ x1 = fp16(x) (round-to-nearest, one plane), product x1w1 -> 1 MMA into an fp32 accumulator,
  *           11 significant bits per operand; |x| must be <= 65504.
@@ -178,9 +181,15 @@ typedef struct {
   void* o_planes; int64_t o_plane_stride; int32_t o_planes_ld;
   int32_t o_planes_fmt;                    /* MTTS_TC_BF16X3 | MTTS_TC_F16X2 | MTTS_TC_F16 */
 } mtts_attn_params;
+/* fp32 kernel for every shape: q, k and v may use the full fp32 range (the BF16X3 and FFMA engines). */
 int mtts_attention_f32(const mtts_attn_params* p, void* stream);
-/* Opt-in: AR-step attention (Tq == Tk <= 64, even head count, dh 64 | 96) with at least `min_len` rows runs on the
- * tensor-core kernel (one 64-row tile per head) instead of the fp32 kernel; min_len <= 0 switches it off (the default: it is slower
+/* The same operation for callers whose engine accepts fp16-range operands (F16X2, F16): sequences of at least 65 queries
+ * with dh in {64, 96, 128}, and the opt-in AR steps below, run on the tensor-core kernel, which splits q, k and v into
+ * F16X2 planes - |x| must be <= 65504 (an element beyond it poisons the result and sets the flag of
+ * mtts_tc_overflow_bind); every other shape runs as mtts_attention_f32. */
+int mtts_attention_tc_f32(const mtts_attn_params* p, void* stream);
+/* Opt-in, mtts_attention_tc_f32 only: AR-step attention (Tq == Tk <= 64, even head count, dh 64 | 96) with at least
+ * `min_len` rows runs on the tensor-core kernel (one 64-row tile per head) instead of the fp32 kernel; min_len <= 0 switches it off (the default: it is slower
  * inside the synthesis step, see csrc/ops.cu).  Returns the previous setting. */
 int mtts_set_attention_pair_min(int32_t min_len);
 

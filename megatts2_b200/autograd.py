@@ -4,8 +4,9 @@ these ``torch.autograd.Function``s, so ``MegaPLMTrainer`` / ``MegaADMTrainer.tra
 libmegatts2_b200.  torch supplies the tape, the loss and the optimiser; every contraction, normalisation, softmax and
 scatter of both passes is a hand-written kernel:
 
-* dense layers: forward ``x W^T`` and backward ``dX = dY W``, ``dW = dY^T X`` on the wgmma tap-GEMM (f16x2 operands: the
-  gradients are fp32-grade, tighter than the bf16 autocast the reference trains under) - shapes the engine does not take
+* dense layers: forward ``x W^T`` and backward ``dX = dY W``, ``dW = dY^T X`` on the wgmma tap-GEMM (bf16x3 operands
+  under every tensor-core engine: the gradients are fp32-grade at any magnitude, tighter than the bf16 autocast the
+  reference trains under; the fp16 planes of f16x2 would flush tiny gradients to zero) - shapes the engine does not take
   (K = 1 embeddings of the ADM, fewer than 128 rows, ragged row counts) go to the strided fp32 batched matmul;
 * attention: unfused for training (the dropout inside ``F.scaled_dot_product_attention`` needs the probabilities):
   ``S = Q K^T`` -> softmax(+mask, +dropout) -> ``P V`` and the four products of its backward, all ``mtts_bmm_f32`` on head
@@ -51,10 +52,11 @@ def _tc_ok(M, K, N):
 
 
 def _train_fmt():
-    """operand format of the training products: fp32-grade always - the half-precision f16 inference engine trains on
-    f16x2 operands (single-pass fp16 gradients underflow)"""
-    e = pack.default_engine()
-    return pack.FMT_F16X2 if e == pack.ENGINE_F16 else pack.engine_fmt(e)
+    """operand format of the training products: bf16x3 under every tensor-core engine.  Gradients span far more than the
+    fp16 exponent range: an f16x2 operand below 2^-14 loses precision (|x - x^| <= 2^-22 |x| + 2^-36) and one below
+    about 2^-35 becomes zero, which silently drops e.g. the weight gradient of a vocabulary row the model has learnt to
+    rule out.  bf16x3 has the fp32 range, so every product is fp32-grade at any magnitude."""
+    return pack.FMT_BF16X3
 
 
 def matmul_nt(a, b):

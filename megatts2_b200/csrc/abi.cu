@@ -100,7 +100,12 @@ int mtts_layernorm_f32(const float* x, int32_t ldx, const float* gamma, const fl
 
 int mtts_attention_f32(const mtts_attn_params* p, void* stream) {
   MTTS_REQUIRE(p, "null params");
-  return attention(*p, (cudaStream_t)stream);
+  return attention(*p, false, (cudaStream_t)stream);
+}
+
+int mtts_attention_tc_f32(const mtts_attn_params* p, void* stream) {
+  MTTS_REQUIRE(p, "null params");
+  return attention(*p, true, (cudaStream_t)stream);
 }
 
 int mtts_vq_argmin_f32(const float* x, int32_t ldx, const float* embed, int64_t N, int32_t D, int32_t K, int64_t* idx,

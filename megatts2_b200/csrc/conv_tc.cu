@@ -850,6 +850,16 @@ static TcPlan tc_plan(const CtcEnv& env, int sms, const mtts_conv_params& p, int
   return pl;
 }
 
+// MEGATTS2_LN_FUSE=0: the LayerNorm a split-K reduction could carry runs as its own launch instead (read once).  The launch
+// plan does not change with it, so the two forms sum the same partials in the same order and agree bit for bit.
+static bool ln_fuse() {
+  static const bool on = [] {
+    const char* e = getenv("MEGATTS2_LN_FUSE");
+    return !(e && e[0] == '0');
+  }();
+  return on;
+}
+
 int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   if (ln) ln->done = 0;
   const CtcEnv& env = ctc_env();
@@ -905,7 +915,7 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
     MTTS_TRY(np == 1 ? (conv_tc_launch<128, 128, 1>(maps, a, st))
            : np == 2 ? (conv_tc_launch<128, 128, 2>(maps, a, st)) : (conv_tc_launch<128, 128, 3>(maps, a, st)));
     // the rows' LayerNorm rides on the reduction when the caller asked for it and a row is 3 / 4 / 6 / 8 x 128 wide
-    if (ln && ln->po.p && a.y && !a.op && a.out_shift == 0 && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384) &&
+    if (ln_fuse() && ln && ln->po.p && a.y && !a.op && a.out_shift == 0 && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384) &&
         p.ldy % 4 == 0 && ln->po.ld % 4 == 0 && ln->po.stride % 4 == 0) {
       const unsigned grid = (unsigned)cdiv64((int64_t)p.B * p.Tout, 4);      // 4 rows (warps) per CTA
       if (p.Cout == 1024) launch_k(tc_splitk_reduce_ln_kernel<8>, grid, 128, 0, st, a, ln->gamma, ln->beta, ln->eps, ln->po);

@@ -95,15 +95,6 @@ static int lin_planes(const TcScratch* tc, __nv_bfloat16* planes, int64_t M, int
   return rc;
 }
 
-// MEGATTS2_LN_FUSE=0: LayerNorm always as its own launch (read once)
-static bool ln_fuse() {
-  static const bool on = [] {
-    const char* e = getenv("MEGATTS2_LN_FUSE");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
 // MEGATTS2_LAST_ROW_TC=0: the final layer's last-row work stays on the exact FFMA engine (read once)
 static bool last_row_tc() {
   static const bool on = [] {
@@ -191,10 +182,10 @@ static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int 
       ap.q = qkv; ap.q_sb = (int64_t)T * 3 * D; ap.q_st = 3 * D; ap.Tq = T;
       if (fused) {
         ap.o = nullptr; ap.o_planes = Pa; ap.o_plane_stride = tc->rows_cap * (int64_t)D; ap.o_planes_ld = D; ap.o_planes_fmt = tc->fmt;
-        MTTS_TRY(attention(ap, st));
+        MTTS_TRY(attention(ap, engine_allows_f16_operands(e->engine), st));
         // out-projection (+ residual); a split-K launch's reduction kernel applies LN2 to the finished rows as well
         LnFuse ln2{L.ln2_g, L.ln2_b, 1e-5f, pa_out, 0};
-        MTTS_TRY(lin_planes(tc, Pa, M, D, D, L.w_o_tc, L.b_o, xin, D, xw, D, 0, nullptr, 0, st, part, part_bytes, ln_fuse() ? &ln2 : nullptr));
+        MTTS_TRY(lin_planes(tc, Pa, M, D, D, L.w_o_tc, L.b_o, xin, D, xw, D, 0, nullptr, 0, st, part, part_bytes, &ln2));
         if (!ln2.done) MTTS_TRY(layernorm_ex(xw, D, L.ln2_g, L.ln2_b, nullptr, 0, nullptr, 0, M, D, 1e-5f, 0, 0, pa_out, st));
         // FF1: relu(h W1 + b1) goes straight to planes P_b; FF2 reads them
         MTTS_TRY(lin_planes(tc, Pa, M, D, F, L.w_ff1_tc, L.b_ff1, nullptr, 0, nullptr, 0, MTTS_ACT_RELU, Pb, F, st, part, part_bytes));
@@ -203,13 +194,13 @@ static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int 
         const bool next_ln = l + 1 < e->n_layers;
         LnFuse ln1{next_ln ? e->layers[l + 1].ln1_g : nullptr, next_ln ? e->layers[l + 1].ln1_b : nullptr, 1e-5f, pa_out, 0};
         MTTS_TRY(lin_planes(tc, Pb, M, F, D, L.w_ff2_tc, L.b_ff2, xw, D, xw, D, 0, nullptr, 0, st, part, part_bytes,
-                            (next_ln && ln_fuse()) ? &ln1 : nullptr));
+                            next_ln ? &ln1 : nullptr));
         ln1_done = ln1.done != 0;
         xin = xw;
         continue;
       }
       ap.o = a; ap.o_sb = (int64_t)T * D; ap.o_st = D;
-      MTTS_TRY(attention(ap, st));
+      MTTS_TRY(attention(ap, engine_allows_f16_operands(e->engine), st));
       // x = x + a Wo + bo
       MTTS_TRY(lin(e, tc, a, D, M, D, D, L.w_o, L.w_o_tc, L.b_o, xin, D, xw, D, 0, st));
       if (e->conv_ff) {
@@ -240,7 +231,7 @@ static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int 
         // LN2 and FF1 write operand planes like the full-sequence layers.  The exact-FFMA form below took 21 + 5 us per
         // dense layer at B = 64 (weight streaming through the FP32 pipe), 4 layers per AR step.
         ap.o = nullptr; ap.o_planes = Pa; ap.o_plane_stride = tc->rows_cap * (int64_t)D; ap.o_planes_ld = D; ap.o_planes_fmt = tc->fmt;
-        MTTS_TRY(attention(ap, st));
+        MTTS_TRY(attention(ap, engine_allows_f16_operands(e->engine), st));
         MTTS_TRY(lin_planes(tc, Pa, B, D, D, L.w_o_tc, L.b_o, xin + (int64_t)(T - 1) * D, T * D, y, D, 0, nullptr, 0, st, part, part_bytes));
         MTTS_TRY(layernorm_ex(y, D, L.ln2_g, L.ln2_b, nullptr, 0, nullptr, 0, B, D, 1e-5f, 0, 0, pa_out, st));
         MTTS_TRY(lin_planes(tc, Pa, B, D, F, L.w_ff1_tc, L.b_ff1, nullptr, 0, nullptr, 0, MTTS_ACT_RELU, Pb, F, st, part, part_bytes));
@@ -248,7 +239,7 @@ static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int 
         continue;
       }
       ap.o = a; ap.o_sb = D; ap.o_st = D;
-      MTTS_TRY(attention(ap, st));
+      MTTS_TRY(attention(ap, engine_allows_f16_operands(e->engine), st));
       mtts_conv_params p;
       memset(&p, 0, sizeof(p));
       p.x = a; p.ldx = D; p.x_batch_stride = D;
@@ -425,7 +416,7 @@ static int causal_step(const mtts_encoder* e, int B, int T, int t, const CausalB
     ap.k = kv; ap.k_sb = (int64_t)T * 2 * D; ap.k_st = 2 * D;
     ap.v = kv + D; ap.v_sb = (int64_t)T * 2 * D; ap.v_st = 2 * D;
     ap.o = cb.a; ap.o_sb = D; ap.o_st = D;
-    MTTS_TRY(attention(ap, st));
+    MTTS_TRY(attention(ap, engine_allows_f16_operands(e->engine), st));
     mtts_conv_params po = linear_params(cb.a, D, L.w_o, L.b_o, cb.x, D, B, D, D);
     po.res = cb.x; po.ldr = D;
     skinny(po);

@@ -12,7 +12,10 @@ namespace mtts {
 //                  magnitude - and the normal range - of x; 22 significant bits); three MMAs per product
 //                  (x0w0 | x0w1' + x1'w0, the second accumulator scaled by 2^-11 in the epilogue).  fp16 range:
 //                  |x| > 65504 cannot be represented - the split then poisons the value (inf/NaN propagate to the
-//                  output) and raises the caller-registered overflow flag (mtts_tc_overflow_bind).
+//                  output) and raises the caller-registered overflow flag (mtts_tc_overflow_bind).  At the low
+//                  end p0 is subnormal below 2^-14 and both terms are zero below about 2^-35: the representation
+//                  error is |x - x^| <= 2^-22 |x| + 2^-36, so tiny operands lose precision (training gradients run
+//                  on bf16x3 for that reason).
 //   fmt 2  f16   : x ~ p0 = fp16(x) (one fp16 plane, round-to-nearest; 11 significant bits); ONE MMA per product.
 //                  Not fp32-grade: the opt-in half-precision inference engine.  Same fp16 range and flag as f16x2.
 // The number of planes of fmt is 3 - fmt.
@@ -88,6 +91,8 @@ int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int 
 static inline int tc_fmt_of_engine(int engine) {
   return engine == 3 ? MTTS_TC_F16 : engine == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3;
 }
+// engines whose operands are limited to the fp16 range (f16x2, f16): the only ones whose attention may use attn_tc.cu
+static inline int engine_allows_f16_operands(int engine) { return engine == 2 || engine == 3; }
 int layernorm_ex(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr, float* y,
                  int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, PlanesOut po, cudaStream_t st);
 int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st);
@@ -114,7 +119,8 @@ int tc_overflow_bind(int32_t* flag);
 int mask_tail(float* x, int B, int rows, int L, const int32_t* keep, cudaStream_t st);
 int layernorm(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr, float* y,
               int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, cudaStream_t st);
-int attention(const mtts_attn_params& p, cudaStream_t st);
+// allow_f16_operands: the caller's engine accepts fp16-range operands, so long sequences may use attn_tc.cu (f16x2 planes)
+int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t st);
 bool attention_tc_eligible(const mtts_attn_params& p);
 int attention_tc(const mtts_attn_params& p, cudaStream_t st);
 bool attention_tc_pair_eligible(const mtts_attn_params& p);

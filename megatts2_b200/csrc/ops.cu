@@ -393,7 +393,7 @@ static std::atomic<int> g_attn_pair_min{[] {
 }()};
 int set_attention_pair_min(int n) { return g_attn_pair_min.exchange(n > 0 ? n : (1 << 30), std::memory_order_relaxed); }
 
-int attention(const mtts_attn_params& p, cudaStream_t st) {
+int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t st) {
   MTTS_REQUIRE(p.q && p.k && p.v && (p.o || p.o_planes), "null pointer");
   MTTS_REQUIRE(!p.o_planes || (p.o_planes_ld % 4 == 0 && p.o_plane_stride % 4 == 0), "plane output alignment");
   MTTS_REQUIRE(p.B >= 0 && p.H > 0 && p.Tq >= 0 && p.Tk > 0, "bad dims");
@@ -403,7 +403,9 @@ int attention(const mtts_attn_params& p, cudaStream_t st) {
   // shapes (Tq = Tk <= 64) a head is a 64 x 64 x 64 problem, all latency, so the AR steps of the benchmark stay on this fp32
   // kernel; longer sequences (teacher-forced forwards, config C3) go to the tensor cores.
   // (MEGATTS2_ATTN_TC = 0 disables it, MEGATTS2_ATTN_TC_MIN sets the minimum Tq; read once per process)
-  {
+  // That kernel splits Q, K and V into f16x2 planes, so only callers on an fp16-range engine take it; the bf16x3 and
+  // FFMA engines keep the full fp32 range here.
+  if (allow_f16_operands) {
     static const int tc_min = [] {
       const char* e = getenv("MEGATTS2_ATTN_TC");
       if (e && e[0] == '0') return 1 << 30;

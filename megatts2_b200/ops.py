@@ -12,6 +12,7 @@ import threading
 import torch
 
 from . import _lib as L
+from . import pack
 
 _F32 = torch.float32
 
@@ -146,7 +147,9 @@ def layernorm(x, gamma, beta, *, res=None, out=None, eps=1e-5, post_act=L.ACT_NO
 
 def attention(q, k, v, n_heads, mask=None):
     """q (B,Tq,D), k/v (B,Tk,D) (any row strides, unit channel stride) -> (B,Tq,D).
-    mask: additive fp32 broadcastable to (B,H,Tq,Tk)."""
+    mask: additive fp32 broadcastable to (B,H,Tq,Tk).  Under an fp16-range default engine (f16x2, f16) long sequences
+    may run on the tensor-core kernel, whose f16x2 operands are range-guarded like the GEMMs'; under bf16x3 and FFMA
+    every call keeps the full fp32 range."""
     q, k, v = _dev(q, name="q"), _dev(k, name="k"), _dev(v, name="v")
     B, Tq, D = q.shape
     Tk = k.shape[1]
@@ -170,7 +173,11 @@ def attention(q, k, v, n_heads, mask=None):
         keep = m
     p.B, p.H, p.Tq, p.Tk, p.dh = B, n_heads, Tq, Tk, dh
     p.scale = 1.0 / math.sqrt(dh)
-    L.check(L.lib().mtts_attention_f32(C.byref(p), _stream()))
+    if pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16):
+        tc_overflow_bind(q.device)
+        L.check(L.lib().mtts_attention_tc_f32(C.byref(p), _stream()))
+    else:
+        L.check(L.lib().mtts_attention_f32(C.byref(p), _stream()))
     return o
 
 

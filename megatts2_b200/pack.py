@@ -200,8 +200,11 @@ class engine_scope:
 def default_engine() -> int:
     """Engine for the dense contractions with M >= 128 (MEGATTS2_ENGINE = f16x2 | bf16x3 | ffma | f16):
     2 = wgmma with f16x2 operands (default: 3 MMAs per fp32-grade product, |activation| <= 65504 guarded by the
-    overflow flag, see ops.tc_overflow), 1 = wgmma with bf16x3 operands (6 MMAs, full fp32 range), 0 = fp32 FFMA
-    everywhere.  These three are fp32-grade; ids are bit-identical between them in the tests.
+    overflow flag, see ops.tc_overflow; at the low end an operand keeps |x - x^| <= 2^-22 |x| + 2^-36, so values
+    below 2^-14 lose precision and values below about 2^-35 vanish - training therefore runs on bf16x3), 1 = wgmma
+    with bf16x3 operands (6 MMAs, full fp32 range), 0 = fp32 FFMA everywhere.  These three are fp32-grade at
+    activation magnitudes; ids are bit-identical between them in the tests.  Attention runs on the f16x2 tensor-core
+    kernel only under engines 2 and 3; under 1 and 0 it stays on the fp32 kernel.
     3 = wgmma with f16 operands is NOT: the opt-in half-precision inference engine (one fp16 plane per operand, one MMA
     per product into an fp32 accumulator, the same fp16 range guard).  Its results differ from the others by fp16
     rounding, and ids may differ too; it is reported separately."""

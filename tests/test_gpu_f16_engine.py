@@ -501,9 +501,9 @@ def test_f16_graph_replay_matches_eager(weights_cpu):
 @gpu
 @TIMEOUT
 def test_training_gradients_identical_under_f16_and_f16x2(weights_cpu):
-    """The training Functions keep fp32-grade operands: under the f16 engine they run on f16x2, bit for bit.  The embedding
-    tables' gradients are scatter-added with atomics (train.cu embedding_bwd), whose order - and so last bit - is not
-    fixed under any engine; they are held to rounding instead."""
+    """The training Functions keep fp32-grade operands: under the f16 and f16x2 engines alike they run on bf16x3, bit for
+    bit.  The embedding tables' gradients are scatter-added with atomics (train.cu embedding_bwd), whose order - and so
+    last bit - is not fixed under any engine; they are held to rounding instead."""
     B, T = 4, 40
     tc = F.relu(torch.randn(B, T, 512, generator=gen(5)))
     codes = torch.cat([torch.full((B, 1), 1024), torch.randint(0, 1024, (B, T), generator=gen(6))], 1)
