@@ -407,6 +407,44 @@ int mtts_adm_decode_causal_f32(const mtts_adm* m, const float* tc_latent, int64_
                                int32_t B, int32_t T, int32_t* dur_out, float* raw_out,
                                void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Opt-in sampled PLM decode: temperature, top-k and top-p, with a device-side Gumbel-max draw (the greedy entry points
+ * above are unchanged and stay the reference-faithful path).  For one logits row z[0..V) (fp32) at AR step t of a row
+ * whose key is kappa:
+ *   1. temperature == 0 or top_k == 1: exactly the greedy argmax (lowest index on ties).
+ *   2. y_i = z_i / temperature (fp32 division); NaN and -inf are never candidates.
+ *   3. top_k > 0 and < V: keep the top_k largest y, ordered by (value descending, index ascending).
+ *   4. top_p < 1: over the kept tokens in that order, keep the shortest prefix whose softmax mass is >= top_p (>= 1 token).
+ *   5. pick = argmax over kept i of y_i - log(-log u_i), lowest index on ties, with u_i = ((w_i >> 8) + 0.5) * 2^-24 and
+ *      w_i = word (i & 3) of Philox4x32-10 with key (seed_lo, seed_hi) and counter (i >> 2, t, kappa_lo, kappa_hi).
+ *   6. a row with a +inf y returns its lowest +inf index; a row without a candidate returns 0.
+ * A draw depends only on (row, parameters, seed, kappa, t): not on the batch size, the row's position or the launch, and
+ * a replayed CUDA graph picks up new seed / key values from device memory.  V <= 4096 (MTTS_ERR_UNSUPPORTED above). */
+typedef struct {
+  float temperature;         /* finite, >= 0 */
+  int32_t top_k;             /* >= 0; 0 = off (as is top_k >= V) */
+  float top_p;               /* in (0, 1]; 1 = off */
+  int32_t reserved;          /* must be 0 */
+  const uint64_t* seed;      /* device, 1 element */
+  const uint64_t* keys;      /* device, one element per row */
+} mtts_sampling;
+/* out[r * ld_out] = the pick of row r of logits (rows, V), row stride ld (0: every row reads the same logits) */
+int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t rows, int32_t step, const mtts_sampling* s,
+                         int64_t* out, int64_t ld_out, void* stream);
+/* The sampler's generator on its own: out[4 i .. 4 i + 3] = Philox4x32-10(counter ctr[4 i .. 4 i + 3], key key[2 i, 2 i + 1])
+ * (uint32 words), for callers that reproduce or audit its noise. */
+int mtts_philox4x32_10_u32(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, void* stream);
+/* mtts_plm_infer_f32 / mtts_plm_decode_causal_f32 with step t's codes drawn by the sampler above (row b keyed by
+ * s->keys[b]) instead of the argmax; the drawn codes are what the next step consumes.  logits_out keeps the raw,
+ * untempered logits.  Same arguments plus `s` (non-NULL), and the same workspace sizes: mtts_plm_infer_workspace_bytes and
+ * mtts_plm_decode_causal_workspace_bytes. */
+int mtts_plm_infer_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                              int32_t B, int32_t T, int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                              void* workspace, int64_t workspace_bytes, void* stream);
+int mtts_plm_decode_causal_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                      int32_t B, int32_t T, int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                                      void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ConvNet family (modules/convnet.py).  One ConvBlock = ReLU -> Conv1d(C,C,k,same) -> LN(C). */
 typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv_block;   /* w packed (k,C,C); w_tc (3,k,C,C) bf16 or NULL */
 

@@ -73,6 +73,10 @@ class ADM(C.Structure):
                 ("emb_dim", i32), ("tc_dim", i32), ("tc_emb_dim", i32)]
 
 
+class Sampling(C.Structure):
+    _fields_ = [("temperature", f32), ("top_k", i32), ("top_p", f32), ("reserved", i32), ("seed", vp), ("keys", vp)]
+
+
 class ConvBlock(C.Structure):
     _fields_ = [("w", vp), ("b", vp), ("ln_g", vp), ("ln_b", vp), ("w_tc", vp)]
 
@@ -164,6 +168,12 @@ SIGNATURES = {
     "mtts_plm_decode_causal_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
     "mtts_adm_decode_causal_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32]),
     "mtts_adm_decode_causal_f32": (C.c_int, [C.POINTER(ADM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
+    "mtts_sample_rows_f32": (C.c_int, [vp, i64, i32, i32, i32, C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_philox4x32_10_u32": (C.c_int, [vp, vp, vp, i64, vp]),
+    "mtts_plm_infer_sample_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, C.POINTER(Sampling), vp, i64,
+                                            vp]),
+    "mtts_plm_decode_causal_sample_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, C.POINTER(Sampling), vp,
+                                                    i64, vp]),
     "mtts_convnet_workspace_bytes": (i64, [C.POINTER(ConvNet), i32, i32]),
     "mtts_convnet_forward_f32": (C.c_int, [C.POINTER(ConvNet), vp, i64, i32, vp, i64, i32, i32, i32, vp, i64, vp]),
     "mtts_convnet_double_out_len": (i32, [C.POINTER(ConvNetDouble), i32]),

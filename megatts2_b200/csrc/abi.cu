@@ -108,6 +108,16 @@ int mtts_attention_tc_f32(const mtts_attn_params* p, void* stream) {
   return attention(*p, true, (cudaStream_t)stream);
 }
 
+int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t rows, int32_t step, const mtts_sampling* s,
+                         int64_t* out, int64_t ld_out, void* stream) {
+  MTTS_REQUIRE(s, "null sampling parameters");
+  return sample_rows(logits, ld, V, rows, step, *s, out, ld_out, nullptr, 0, (cudaStream_t)stream);
+}
+
+int mtts_philox4x32_10_u32(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, void* stream) {
+  return philox4x32_10_words(ctr, key, out, n, (cudaStream_t)stream);
+}
+
 int mtts_vq_argmin_f32(const float* x, int32_t ldx, const float* embed, int64_t N, int32_t D, int32_t K, int64_t* idx,
                        void* stream) {
   return vq_argmin(x, ldx, embed, N, D, K, idx, (cudaStream_t)stream);

@@ -276,8 +276,9 @@ static int64_t plm_ws_floats(const mtts_plm* m, int B, int T) {
          2 * ((int64_t)B * (T + 1) + 64) + 6 * 64;
 }
 
+// smp == nullptr: greedy (argmax_rows); otherwise each step's codes are drawn by the opt-in sampler (sample.cu)
 static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
-                     float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st) {
+                     float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st, const mtts_sampling* smp = nullptr) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
@@ -310,7 +311,8 @@ static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_l
     p.B = B; p.Tin = 1; p.Tout = 1; p.Cin = D; p.Cout = V; p.k = 1; p.stride = 1; p.dil = 1; p.out_scale = 1.0f;
     if (tcs.p) { p.tc_scratch = tcs.p; p.tc_scratch_bytes = tcs.bytes; }
     MTTS_TRY(conv1d(p, st));
-    MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
+    if (smp) MTTS_TRY(sample_rows(lg, lg_sb, V, B, t, *smp, codes + (t + 1), T + 1, codes_out + t, T, st));
+    else MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
   }
   return 0;
 }
@@ -439,7 +441,8 @@ static int64_t plm_causal_ws_floats(const mtts_plm* m, int B, int T) {
 }
 
 static int plm_decode_causal(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
-                             float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st) {
+                             float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
+                             const mtts_sampling* smp = nullptr) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
@@ -463,7 +466,8 @@ static int plm_decode_causal(const mtts_plm* m, const float* tc, int64_t tc_sb, 
     p.B = B; p.Tin = 1; p.Tout = 1; p.x_batch_stride = D;
     p.tc_scratch = cb.scratch; p.tc_scratch_bytes = cb.scratch_bytes;
     MTTS_TRY(conv1d(p, st));
-    MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
+    if (smp) MTTS_TRY(sample_rows(lg, lg_sb, V, B, t, *smp, codes + (t + 1), T + 1, codes_out + t, T, st));
+    else MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
   }
   return 0;
 }
@@ -880,6 +884,13 @@ int mtts_plm_infer_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb,
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
   return plm_infer(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
+int mtts_plm_infer_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
+                              int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
+                              int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
+  MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_infer(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes, (cudaStream_t)stream, s);
+}
 
 int64_t mtts_adm_infer_workspace_bytes(const mtts_adm* m, int32_t B, int32_t T) { return adm_ws_floats(m, B, T) * 4 + 8192; }
 int mtts_adm_infer_f32(const mtts_adm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
@@ -896,6 +907,14 @@ int mtts_plm_decode_causal_f32(const mtts_plm* m, const float* tc_latent, int64_
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
   return plm_decode_causal(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes,
                            (cudaStream_t)stream);
+}
+int mtts_plm_decode_causal_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                                      int32_t T, int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                                      void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
+  MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_decode_causal(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes,
+                           (cudaStream_t)stream, s);
 }
 int64_t mtts_adm_decode_causal_workspace_bytes(const mtts_adm* m, int32_t B, int32_t T) {
   return adm_causal_ws_floats(m, B, T) * 4 + 8192;

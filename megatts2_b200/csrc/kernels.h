@@ -148,6 +148,12 @@ int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const
                     cudaStream_t st);
 int argmax_rows(const float* x, int64_t ldx, int V, int rows, int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb,
                 cudaStream_t st);
+// opt-in sampler (sample.cu): validates s against V, then draws one code per row (argmax_rows when temperature == 0 or
+// top_k == 1); sampling_check alone lets a driver reject bad parameters before it enqueues anything
+int sampling_check(const mtts_sampling* s, int V);
+int sample_rows(const float* x, int64_t ldx, int V, int rows, int step, const mtts_sampling& s, int64_t* out_a,
+                int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st);
+int philox4x32_10_words(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, cudaStream_t st);
 int fill_i64(int64_t* p, int64_t stride, int n, int64_t v, cudaStream_t st);
 int fill_f32(float* p, int64_t stride, int n, float v, cudaStream_t st);
 int adm_build_input(const float* tc_emb, int64_t te_sb, int te_ld, int tc_emb_dim, const float* praw, int p_ld,

@@ -17,6 +17,7 @@ import yaml
 from .. import _lib as L
 from .. import autograd as A
 from .. import ops, pack
+from .. import sampling as S
 from ..modules.convnet import ConvNet
 from ..modules.embedding import SinePositionalEmbedding
 from ..modules.mrte import MRTE, LengthRegulator
@@ -137,9 +138,13 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         logits = ops.linear(h, pack.pack_linear(self.predict_layer.weight))
         return logits, p_codes[:, 1:]
 
-    def infer(self, tc_latent: torch.Tensor, return_logits: bool = False):
+    def infer(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None, keys=None):
         """Greedy AR decode, BOS = vq_bins, exactly T steps, NON-causal full recompute per step
-        (models/megatts2.py:165-181).  tc_latent (B,T,tc_dim) -> (B,T) int64 [, (B,T,vq_bins) logits]."""
+        (models/megatts2.py:165-181).  tc_latent (B,T,tc_dim) -> (B,T) int64 [, (B,T,vq_bins) logits].
+
+        ``sampling`` (opt-in, megatts2_b200.sampling.Sampling): each step's code is drawn on the device instead of the
+        argmax, row b keyed by ``keys[b]`` (B 64-bit integers, default arange(B)); the returned logits stay the raw ones.
+        The seed and the keys are inputs of the replayed CUDA graph, so a new seed needs no new capture."""
         _eval_only(self)
         tc = ops._dev(tc_latent, name="tc_latent")
         if tc.stride(2) != 1:
@@ -147,6 +152,8 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         B, T, _ = tc.shape
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
+        if sampling is not None:
+            return self._infer_sampled(pl, tc, return_logits, sampling, S.row_keys(keys, B, tc.device))
 
         def run(tc_):
             codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
@@ -164,13 +171,34 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         logits = out[1] if return_logits else None
         return (codes, logits) if return_logits else codes
 
-    def infer_causal(self, tc_latent: torch.Tensor, return_logits: bool = False):
+    def _infer_sampled(self, pl, tc, return_logits, sampling, keys):
+        B, T, _ = tc.shape
+        lib = L.lib()
+
+        def run(tc_, seed_, keys_):
+            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
+            logits = torch.empty(B, T, self.vq_bins, dtype=torch.float32, device=tc_.device) if return_logits else None
+            ws = ops.workspace(lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T), tc_.device)
+            s = sampling.struct(seed_, keys_)
+            L.check(lib.mtts_plm_infer_sample_f32(C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
+                                                  codes.data_ptr(), logits.data_ptr() if return_logits else None,
+                                                  C.byref(s), ws.data_ptr(), ws.numel(), ops._stream()))
+            return (codes, logits) if return_logits else (codes,)
+
+        out = self._graphs().run(("plm_sample", pl.serial, B, T, bool(return_logits), tc.stride(0), tc.stride(1),
+                                  ops.launch_policy_now(), sampling.graph_key()),
+                                 (tc, sampling.seed_tensor(tc.device), keys), run)
+        return (out[0], out[1]) if return_logits else out[0]
+
+    def infer_causal(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None,
+                     keys=None):
         """OPT-IN causal KV-cache greedy decode (SURVEY.md 8f-1) - NOT what the reference's ``infer`` computes.
 
         ``infer`` re-runs the stack bidirectionally every step (models/megatts2.py:177); this decode follows the
         *training* semantics of ``forward`` (causal=True, models/megatts2.py:158): row t attends to rows <= t, so
         each step computes one row per utterance against per-layer K/V caches (O(T) instead of O(T^2)).  Its
-        logits equal the teacher-forced ``forward`` logits evaluated on its own output.  Same I/O as ``infer``."""
+        logits equal the teacher-forced ``forward`` logits evaluated on its own output.  Same I/O as ``infer``,
+        ``sampling`` and ``keys`` included (the same noise as ``infer`` for a given seed, key and step)."""
         _eval_only(self)
         tc = ops._dev(tc_latent, name="tc_latent")
         if tc.stride(2) != 1:
@@ -181,9 +209,16 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         codes = torch.empty(B, T, dtype=torch.int64, device=tc.device)
         logits = torch.empty(B, T, self.vq_bins, dtype=torch.float32, device=tc.device) if return_logits else None
         ws = ops.workspace(lib.mtts_plm_decode_causal_workspace_bytes(C.byref(pl.struct), B, T), tc.device)
-        L.check(lib.mtts_plm_decode_causal_f32(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B, T,
-                                               codes.data_ptr(), logits.data_ptr() if return_logits else None,
-                                               ws.data_ptr(), ws.numel(), ops._stream()))
+        if sampling is None:
+            L.check(lib.mtts_plm_decode_causal_f32(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B, T,
+                                                   codes.data_ptr(), logits.data_ptr() if return_logits else None,
+                                                   ws.data_ptr(), ws.numel(), ops._stream()))
+        else:
+            seed, keys = sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device)
+            s = sampling.struct(seed, keys)
+            L.check(lib.mtts_plm_decode_causal_sample_f32(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B,
+                                                          T, codes.data_ptr(), logits.data_ptr() if return_logits else None,
+                                                          C.byref(s), ws.data_ptr(), ws.numel(), ops._stream()))
         return (codes, logits) if return_logits else codes
 
     @classmethod
@@ -516,7 +551,8 @@ class Megatts(nn.Module):
     @torch.no_grad()
     def synthesize(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                    return_intermediates: bool = False, causal_decode: bool = False, prompt_mels: torch.Tensor = None,
-                   return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None):
+                   return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None,
+                   sampling: S.Sampling = None, keys=None):
         """phone_tokens (B,Tp) int64, mels (B,Tm,80) prompt mel (frames-major) -> wav (B,1,256*(max sum d + 10)).
         Steps = models/megatts2.py:354-373; every utterance's result equals the reference's batch-1 run on it
         (utterances are independent; the only cross-utterance coupling would be the zero rows the LengthRegulator
@@ -539,15 +575,20 @@ class Megatts(nn.Module):
         range flag after the batch (one 4-byte readback) and, if any activation left the fp16 range, redo the batch on the
         bf16x3 engine.  The check keys off the default engine (``MEGATTS2_ENGINE`` / ``pack.engine_scope``): a module
         whose ``.engine`` is set by hand - e.g. only the vocoder on f16 (``hifi_gan.generator.engine =
-        pack.ENGINE_F16``) - is not guarded by it."""
+        pack.ENGINE_F16``) - is not guarded by it.
+        ``sampling`` (opt-in, megatts2_b200.sampling.Sampling): the prosody codes are sampled instead of decoded greedily
+        (``MegaPLM.infer``), utterance b keyed by ``keys[b]`` (default arange(B)); the ADM durations stay deterministic.
+        The bf16x3 rerun above draws with the same seed and keys."""
         dev = phone_tokens.device
-        out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt)
+        out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt,
+                               sampling, keys)
         if check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16) and ops.tc_overflow(dev):
             import warnings
             warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
                           "re-running this batch on the bf16x3 engine")
             with pack.engine_scope(pack.ENGINE_BF16X3):
-                out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt)
+                out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt,
+                                       sampling, keys)
         if return_intermediates:
             return out
         return (out["wav"], out["wav_lens"]) if return_lengths else out["wav"]
@@ -562,7 +603,8 @@ class Megatts(nn.Module):
                 float(os.environ.get("MEGATTS2_REVOCODE_FRAC", str(REVOCODE_FRAC_DEFAULT))),
                 os.environ.get("MEGATTS2_REVOCODE_FROM", REVOCODE_FROM_DEFAULT))
 
-    def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None):
+    def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
+                    sampling=None, keys=None):
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -603,7 +645,7 @@ class Megatts(nn.Module):
         d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
         tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
         tc8 = ops.maxpool_time(tc_expand, 8)
-        p_codes = plm_decode(tc8)
+        p_codes = plm_decode(tc8) if sampling is None else plm_decode(tc8, sampling=sampling, keys=keys)
         B, Lmax = tc_expand.shape[0], tc_expand.shape[1]
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]
@@ -636,11 +678,14 @@ class Megatts(nn.Module):
                     mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
 
     @torch.no_grad()
-    def synthesize_many(self, items, max_batch: int = 64, **kw):
+    def synthesize_many(self, items, max_batch: int = 64, sampling: S.Sampling = None, **kw):
         """Ragged front door: ``items`` = list of (phone (Tp_i,) int64, prompt mel (Tm_i, 80)).  Utterances are
         bucketed by (Tp, Tm) - the MRTE phone encoder and the prompt encoder are unmasked in the reference
         (modules/mrte.py:154-171), so padding either would change results - and each bucket runs as one batch.
-        Returns a list of 1-D waveforms (valid samples only), in input order."""
+        Returns a list of 1-D waveforms (valid samples only), in input order.  With ``sampling``, utterance i is keyed
+        by its index i in ``items``, so the bucketing and ``max_batch`` do not change what it draws."""
+        if sampling is not None:
+            kw["sampling"] = sampling
         buckets = {}
         for i, (ph, m) in enumerate(items):
             buckets.setdefault((ph.shape[0], m.shape[0]), []).append(i)
@@ -650,6 +695,8 @@ class Megatts(nn.Module):
                 chunk = ids[s:s + max_batch]
                 ph = torch.stack([items[i][0] for i in chunk])
                 mm = torch.stack([items[i][1] for i in chunk])
+                if sampling is not None:
+                    kw["keys"] = torch.tensor(chunk, dtype=torch.int64)
                 wav, lens = self.synthesize(ph, mm, return_lengths=True, **kw)
                 for j, i in enumerate(chunk):
                     out[i] = wav[j, 0, :lens[j]]

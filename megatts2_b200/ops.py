@@ -211,6 +211,37 @@ def vq_gather(idx, embed, t_out=None, repeat=1, out=None):
     return out
 
 
+# ------------------------------------------------------------------------------ sampling
+def sample_rows(logits, step, sampling, keys):
+    """logits (rows, V) fp32 with unit column stride (a row stride of 0 - ``z.expand(rows, V)`` - repeats one row), AR step
+    ``step``, a ``sampling.Sampling`` and the per-row 64-bit ``keys`` (rows,) -> the drawn code per row, (rows,) int64."""
+    from . import sampling as S
+    logits = _dev(logits, name="logits")
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        logits = logits.contiguous()
+    rows, V = logits.shape
+    seed = sampling.seed_tensor(logits.device)
+    keys = S.row_keys(keys, rows, logits.device)
+    out = torch.empty(rows, dtype=torch.int64, device=logits.device)
+    s = sampling.struct(seed, keys)
+    L.check(L.lib().mtts_sample_rows_f32(_ptr(logits), logits.stride(0), V, rows, int(step), C.byref(s), _ptr(out), 1,
+                                         _stream()))
+    return out
+
+
+def philox4x32_10(ctr, key):
+    """The sampler's generator: ctr (n, 4) and key (n, 2) uint32 words, as int64 tensors holding values < 2**32, ->
+    (n, 4) words (int64, values < 2**32)."""
+    dev = ctr.device
+    ctr32 = _dev(ctr, torch.int64, "ctr").to(torch.int32).contiguous()          # same low 32 bits
+    key32 = _dev(key, torch.int64, "key").to(torch.int32).contiguous()
+    n = ctr32.shape[0]
+    assert ctr32.shape == (n, 4) and key32.shape == (n, 2)
+    out = torch.empty(n, 4, dtype=torch.int32, device=dev)
+    L.check(L.lib().mtts_philox4x32_10_u32(_ptr(ctr32), _ptr(key32), _ptr(out), n, _stream()))
+    return out.to(torch.int64) & 0xFFFFFFFF
+
+
 # ------------------------------------------------------------------------------ misc
 def maxpool_time(x, k):
     x, x_sb, ldx = _rows(_dev(x, name="x"))
