@@ -62,8 +62,6 @@ struct ConvTcArgs {
 // through a row-shifted wgmma descriptor; only the (tiny) per-tap weight tiles stream through the stage ring.  The plain
 // form re-reads the tile once per tap (k-fold L2 -> SM traffic), which is what bounds the C = 32 / 64 HiFi-GAN stages.
 constexpr int CTC_HALO_ROWS = 192;     // rows of a halo tile buffer: 128 + dil * (k - 1) <= 192, a multiple of 8
-constexpr int CTC_THREADS = 384;       // warps 0-7: two consumer warpgroups, warps 8-11: TMA producer warpgroup
-constexpr int CTC_PRODUCER_REGS = 40, CTC_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
 template <int BN, int SWB, int NP = 3, int HALO = 0>
 struct ConvTcCfg {
   // output rows of a work item.  NP = 1 keeps 64 rows at BN = 128 although its single accumulator would fit a 128-row item:
@@ -598,6 +596,15 @@ int cur_device_sms() {
   const int all = g_dev[dev].sms;
   return g_sm_limit > 0 && g_sm_limit < all ? g_sm_limit : all;
 }
+int tc_smem_attr(const void* kernel, int slot, int bytes) {
+  const int dev = cur_device();
+  if (g_dev[dev].attr_done & (1u << slot)) return 0;
+  std::lock_guard<std::mutex> lk(g_ctc_mu);
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "conv_tc", (long long)e);
+  g_dev[dev].attr_done |= (1u << slot);
+  return 0;
+}
 int32_t* tc_ovf_ptr() { return g_dev[cur_device()].ovf; }
 int tc_overflow_bind(int32_t* flag) {
   g_dev[cur_device()].ovf = flag;
@@ -666,7 +673,7 @@ static int ctc_init_locked() {
 }
 
 // 2-byte-element tensor (d2, d1, d0) row-major, box (1, b1, b0), SWB-byte swizzle; rank 2 when d2 == 0
-static int cmap_get(const void* p, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1, int swb, int fmt,
+int cmap_get(const void* p, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1, int swb, int fmt,
                     CUtensorMap* out) {
   std::lock_guard<std::mutex> lk(g_ctc_mu);
   MTTS_TRY(ctc_init_locked());
@@ -699,16 +706,9 @@ static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, cudaStrea
   // one bit per instantiation in the per-device table (the max-dynamic-shared-memory attribute is per device)
   constexpr int slot = HALO ? 18 + (BN == 64 ? 0 : 1) + 2 * (3 - NP)
                             : (BN == 128 ? 0 : BN == 64 ? 1 : 2) + 3 * (SWB == 128 ? 0 : 1) + 6 * (3 - NP);
-  static_assert(slot < 32, "attribute slots");
-  const int dev = cur_device();
+  static_assert(slot < 24, "attribute slots (24-31: resblock_tc.cu)");
+  MTTS_TRY(tc_smem_attr((const void*)conv_tc_kernel<BN, SWB, NP, HALO>, slot, Cfg::SMEM));
   const int sms = cur_device_sms();
-  if (!(g_dev[dev].attr_done & (1u << slot))) {
-    std::lock_guard<std::mutex> lk(g_ctc_mu);
-    cudaError_t e =
-        cudaFuncSetAttribute(conv_tc_kernel<BN, SWB, NP, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "conv_tc", (long long)e);
-    g_dev[dev].attr_done |= (1u << slot);
-  }
   const int64_t items = (int64_t)a.B * cdiv64(a.T, Cfg::ROWS) * cdiv64(a.Cout, BN) * a.splits;
   const int grid = (int)(items < sms ? items : sms);
   launch_k(conv_tc_kernel<BN, SWB, NP, HALO>, grid, CTC_THREADS, Cfg::SMEM, st, maps, a);

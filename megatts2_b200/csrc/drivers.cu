@@ -643,6 +643,31 @@ static int64_t hifigan_ws_floats(const mtts_hifigan* h, int B, int T) {
   return (int64_t)B * Tp * h->in_channels + 64 + 5 * ((int64_t)B * big + 64) + 3 * (tcb / 4 + 64);
 }
 
+// MEGATTS2_RB_FUSE=0: the C <= 64 vocoder stages run each ResBlock conv as its own tap-GEMM launch (read once)
+static bool rb_fuse() {
+  static const bool on = [] {
+    const char* e = getenv("MEGATTS2_RB_FUSE");
+    return !(e && e[0] == '0');
+  }();
+  return on;
+}
+
+// a tensor-core launch outside conv1d(), timed for the profile like one (`flops`: its algorithmic work)
+template <typename F>
+static int prof_tc(double flops, cudaStream_t st, F&& launch) {
+  if (!g_prof_on) return launch();
+  ProfRec r;
+  if (cudaEventCreate(&r.a) != cudaSuccess || cudaEventCreate(&r.b) != cudaSuccess)
+    return fail(MTTS_ERR_CUDA, "%s: cudaEventCreate failed", "profile");
+  r.flops = flops; r.tc = true;
+  cudaEventRecord(r.a, st);
+  const int rc = launch();
+  cudaEventRecord(r.b, st);
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  g_prof.push_back(r);
+  return rc;
+}
+
 static int hifigan_forward(const mtts_hifigan* h, const float* mel, int64_t mel_sb, int mel_ld, int B, int T, float* wav,
                            int64_t wav_sb, void* ws, int64_t ws_bytes, cudaStream_t st) {
   MTTS_REQUIRE(h->n_ups >= 1 && h->n_ups <= 4 && h->n_kernels >= 1, "bad generator config");
@@ -708,6 +733,32 @@ static int hifigan_forward(const mtts_hifigan* h, const float* mel, int64_t mel_
     // one split of leaky(oup) with the LARGEST first-conv halo of the stage's ResBlocks; each ResBlock's first conv reads it
     // at its own row offset (three separate splits of the same signal were 6 % of the vocoder)
     const bool stage_fused = fused && (Co == 32 || Co == 64 || (Co >= 128 && Co % 32 == 0)) && (int64_t)B * Lo >= 128;
+    // C <= 64: each dilation step of each ResBlock is one resblock_pair_tc launch, reading fp32 x and writing fp32 y
+    // (x -> xr -> xt -> z: the launch reads halo rows other CTAs overwrite, so input and output never alias)
+    bool pair_fused = stage_fused && rb_fuse();
+    for (int j = 0; pair_fused && j < h->n_kernels; ++j)
+      for (int m = 0; m < 3; ++m)
+        pair_fused = pair_fused && resblock_tc_eligible(B, Lo, Co, h->resblocks[i * h->n_kernels + j].k,
+                                                        h->resblocks[i * h->n_kernels + j].dil[m], hfmt);
+    if (pair_fused) {
+      for (int j = 0; j < h->n_kernels; ++j) {
+        const mtts_hifigan_resblock& rb = h->resblocks[i * h->n_kernels + j];
+        const float* xcur = oup;
+        for (int m = 0; m < 3; ++m) {
+          float* yout = m == 2 ? z : (m == 0 ? xr : xt);
+          const float scale = m == 2 ? 1.0f / (float)h->n_kernels : 1.0f;
+          const double flops = 2.0 * 2.0 * (double)B * Lo * Co * Co * rb.k;      // both convs, algorithmic
+          MTTS_TRY(prof_tc(flops, st, [&] {
+            return resblock_pair_tc(xcur, yout, rb.w1_tc[m], rb.b1[m], rb.w2_tc[m], rb.b2[m], B, Lo, Co, rb.k, rb.dil[m],
+                                    scale, m == 2 && j > 0, hfmt, st);
+          }));
+          xcur = yout;
+        }
+      }
+      float* tswap = o; o = z; z = tswap;
+      Lc = Lo; Cc = Co;
+      continue;
+    }
     int hmax = 0;
     for (int j = 0; j < h->n_kernels; ++j) {
       const mtts_hifigan_resblock& rbj = h->resblocks[i * h->n_kernels + j];
@@ -738,7 +789,7 @@ static int hifigan_forward(const mtts_hifigan* h, const float* mel, int64_t mel_
           c1.tc_out_tp = Lo + 2 * h2; c1.tc_out_hl = h2; c1.tc_out_ld = Co;
           c1.tc_out_plane_stride = (int64_t)B * c1.tc_out_tp * Co;
           c1.tc_out_act = MTTS_ACT_LEAKY; c1.tc_out_slope = 0.1f;
-          if (!conv_tc_eligible(c1)) return fail(MTTS_ERR_UNSUPPORTED, "%s: fused ResBlock conv not eligible (C=%lld L=%lld)", "hifigan", Co, Lo);
+          if (!conv_tc_eligible(c1)) return fail(MTTS_ERR_UNSUPPORTED, "%s: fused ResBlock conv not eligible (C=%lld L=%lld)", "hifigan", (long long)Co, (long long)Lo);
           MTTS_TRY(conv1d(c1, st));
           MTTS_TRY(halo_fill(planes2, B, Lo, Co, h2, h2, MTTS_PAD_REFLECT, hfmt, st));
           const bool lastm = (m == 2);
@@ -755,7 +806,7 @@ static int hifigan_forward(const mtts_hifigan* h, const float* mel, int64_t mel_
             c2.tc_out_plane_stride = (int64_t)B * c2.tc_out_tp * Co;
             c2.tc_out_act = MTTS_ACT_LEAKY; c2.tc_out_slope = 0.1f;
           }
-          if (!conv_tc_eligible(c2)) return fail(MTTS_ERR_UNSUPPORTED, "%s: fused ResBlock conv not eligible (C=%lld L=%lld)", "hifigan", Co, Lo);
+          if (!conv_tc_eligible(c2)) return fail(MTTS_ERR_UNSUPPORTED, "%s: fused ResBlock conv not eligible (C=%lld L=%lld)", "hifigan", (long long)Co, (long long)Lo);
           MTTS_TRY(conv1d(c2, st));
           if (!lastm) MTTS_TRY(halo_fill(tc.scratch, B, Lo, Co, rb.dil[m + 1] * (rb.k - 1) / 2, rb.dil[m + 1] * (rb.k - 1) / 2, MTTS_PAD_REFLECT, hfmt, st));
           (void)h1;

@@ -1,5 +1,6 @@
 // Internal (C++) entry points shared by the drivers and the C ABI.
 #pragma once
+#include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -107,6 +108,17 @@ struct LnFuse {
   int done;
 };
 int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln = nullptr);
+// launch plumbing shared by the tensor-core kernels (conv_tc.cu): the cached TMA descriptor of a 2-byte-element tensor
+// (d2, d1, d0) with box (1, b1, b0) and SWB-byte swizzle (rank 2 when d2 == 0), and the max-dynamic-shared-memory
+// attribute of a kernel, raised once per device (slot: a bit of the per-device table, < 32)
+int cmap_get(const void* p, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, uint32_t b1, int swb, int fmt, CUtensorMap* out);
+int tc_smem_attr(const void* kernel, int slot, int bytes);
+// One HiFi-GAN ResBlock1 dilation step y = (x + conv2(leaky(conv1_dil(leaky(x))))) * out_scale (+ y if accumulate), reflect
+// padding, in one launch (resblock_tc.cu); w1_tc / w2_tc are the convs' packed planes of `fmt`.  Bit-identical to the
+// two-launch tap-GEMM flow.  Only where resblock_tc_eligible holds: C 32 | 64, f16x2 | f16, T > the two halos, B*T >= 128.
+bool resblock_tc_eligible(int B, int T, int C, int k, int dil, int fmt);
+int resblock_pair_tc(const float* x, float* y, const void* w1_tc, const float* b1, const void* w2_tc, const float* b2,
+                     int B, int T, int C, int k, int dil, float out_scale, int accumulate, int fmt, cudaStream_t st);
 int halo_fill(void* planes_base, int B, int T, int C, int hl, int hr, int pad_mode, int fmt, cudaStream_t st);
 int64_t linear_tc_scratch_bytes(int64_t rows_cap, int K);
 int linear_tc(const float* x, int ldx, int64_t M, int K, const void* w_planes, int N, const float* bias,

@@ -6,6 +6,10 @@
 
 namespace mtts {
 
+// CTA layout of the persistent tensor-core kernels (conv_tc.cu, resblock_tc.cu)
+constexpr int CTC_THREADS = 384;       // warps 0-7: two consumer warpgroups, warps 8-11: TMA producer warpgroup
+constexpr int CTC_PRODUCER_REGS = 40, CTC_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
