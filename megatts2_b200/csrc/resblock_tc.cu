@@ -6,9 +6,9 @@
 // leaves shared memory, and the fp32 input is split into operand planes by the kernel itself.
 //
 // Work item = R = 128 - 2 h2 output rows of one batch item (h1 = d (k - 1) / 2, h2 = (k - 1) / 2):
-//   1. the warpgroup reads fp32 x rows [r0 - h1 - h2, r0 + 128 + h1 - h2) (reflected about the sequence ends exactly like
-//      split_pad_kernel), applies leaky 0.1 and writes the operand planes in the K-major swizzled layout a TMA load
-//      would produce;
+//   1. the loader warps copy fp32 x rows [r0 - h1 - h2, r0 + 128 + h1 - h2) (reflected about the sequence ends exactly
+//      like split_pad_kernel) into a staging buffer with cp.async, apply leaky 0.1 and write the operand planes into an
+//      x buffer in the K-major swizzled layout a TMA load would produce;
 //   2. conv1 over 128 rows (positions [r0 - h2, r0 - h2 + 128)): tap j reads the planes through a descriptor shifted by
 //      j d rows, as the halo form of conv_tc_kernel does;
 //   3. epilogue 1 writes leaky(conv1 + bias) as operand planes over the x planes (the same buffer), then the rows at
@@ -18,13 +18,19 @@
 // Every output element sees the same MMAs on the same operands in the same order, and the same epilogue arithmetic, as
 // under the two conv_tc_kernel halo-form launches it replaces, so the result is bit-identical to them.
 //
-// One CTA = 2 consumer warpgroups (each owns its items whole: load, conv1, epilogue 1, conv2, epilogue 2) + 1 producer
-// warp that streams the per-tap weight tiles with TMA into one ring PER WARPGROUP.  Each warpgroup consumes only its own
-// ring, strictly in order, so when it waits for a slab every earlier slab of that slot has landed and been consumed: the
-// parity of the full barrier is never ambiguous, whatever the ring depth and however far the warpgroups drift apart.
-// The producer fills the rings in the order conv1 of the first item of a pair, conv1 of the second, conv2 of the first,
-// conv2 of the second, so the two warpgroups take turns on the tensor pipe: one runs its MMAs while the other loads x or
-// runs an epilogue.  Formats: f16x2 (NP = 2) and f16 (NP = 1); bf16x3 keeps the unfused flow.
+// One CTA = 2 consumer warpgroups (each owns its items' conv1, epilogue 1, conv2 and epilogue 2) + the producer
+// warpgroup: warp 8 streams the per-tap weight tiles with TMA into one ring PER WARPGROUP, warps 9-11 (the loader) do
+// step 1 for every item of the CTA, in the order the warpgroups take them, into a ring of XBUFS x buffers (item li of
+// the CTA in buffer li % XBUFS), so the x traffic of the next items runs under the MMAs and epilogues of the current
+// ones.  A buffer is handed over through two mbarriers: xfull (the loader's planes are in place) and xempty (conv2's
+// MMAs of the buffer's item have retired; epilogue 2 reads the residual from global memory, not from the buffer).
+// Each warpgroup consumes only its own weight ring, strictly in order, so when it waits for a slab every earlier slab of
+// that slot has landed and been consumed: the parity of the full barrier is never ambiguous, whatever the ring depth and
+// however far the warpgroups drift apart.  The x ring is filled and drained in item order, and the fill of item li waits
+// only for item li - XBUFS (<= li - 2, the same warpgroup's previous item or an earlier one), so its parities are
+// unambiguous too.  The producer fills the weight rings in the order conv1 of the first item of a pair, conv1 of the
+// second, conv2 of the first, conv2 of the second, so the two warpgroups take turns on the tensor pipe: one runs its MMAs
+// while the other runs an epilogue.  Formats: f16x2 (NP = 2) and f16 (NP = 1); bf16x3 keeps the unfused flow.
 #include "kernels.h"
 #include "tc_ptx.cuh"
 
@@ -43,24 +49,35 @@ struct RbTcArgs {
   int32_t* ovf;                 // f16 range flag (may be null)
 };
 
-constexpr int RB_XROWS = 192;   // rows of the per-warpgroup activation buffer: 128 + 2 h1 <= 192
+constexpr int RB_XROWS = 192;           // rows of an x buffer: 128 + 2 h1 <= 192
+constexpr int RB_LOADER_THREADS = 96;   // warps 9-11
+// barrier area: the weight rings' full / empty barriers (2 rings x 2 x 8 bytes x STAGES <= 256 bytes), then the x ring's
+// xfull / xempty barriers (2 x 8 bytes x XBUFS <= 64 bytes)
+constexpr int RB_BAR_BYTES = 256 + 64;
 
 template <int C, int NP>
 struct RbTcCfg {
   static constexpr int SWB = 2 * C;                      // one 16-bit activation row = one swizzled row (64 or 128 bytes)
   static constexpr int XPLANE = RB_XROWS * SWB;
-  static constexpr int XBUF = NP * XPLANE;               // per consumer warpgroup
+  static constexpr int XBUF = NP * XPLANE;               // one x buffer (24 KB, or 48 KB at C = 64, f16x2)
+  // two buffers per warpgroup where they are 24 KB, so the loader can run a whole item ahead of each warpgroup
+  static constexpr int XBUFS = XBUF <= 24 * 1024 ? 4 : 2;
+  // fp32 staging of one item's x rows, which cp.async fills.  Two at C = 32, where an item's MMAs take less time than
+  // one round trip to memory, so the copies of the next item are in flight while the loader converts the current one
+  static constexpr int XSTAGE = RB_XROWS * C * 4;
+  static constexpr int SBUFS = C == 32 ? 2 : 1;
   static constexpr int W_PLANE = C * SWB;                // one tap's weight tile (C x C), one plane
   static constexpr int STAGE = NP * W_PLANE;
   static constexpr int EPI_STAGE = 8 * 16 * 20 * 4;
-  static constexpr int STAGES_RAW = (227 * 1024 - 1024 - 256 - EPI_STAGE - 2 * XBUF) / (2 * STAGE);
-  // stages of EACH warpgroup's ring (2 rings x 2 barriers x 8 bytes x STAGES <= 256 bytes).  A warpgroup holds at most two
-  // slabs unreleased (the one whose MMAs run and the one it waits for), so 2 stages cannot deadlock; 3 keep the next tap's
-  // weights in flight during the current tap's MMAs
+  static constexpr int STAGES_RAW =
+      (227 * 1024 - 1024 - RB_BAR_BYTES - EPI_STAGE - XBUFS * XBUF - SBUFS * XSTAGE) / (2 * STAGE);
+  // stages of EACH warpgroup's ring.  A warpgroup holds at most two slabs unreleased (the one whose MMAs run and the one
+  // it waits for), so 2 stages cannot deadlock; 3 keep the next tap's weights in flight during the current tap's MMAs
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int SMEM = 2 * XBUF + 2 * STAGES * STAGE + 1024 + 256 + EPI_STAGE;
-  static_assert(STAGES >= 3 && SMEM <= 227 * 1024, "shared-memory budget");
-  static_assert(XPLANE % 1024 == 0 && STAGE % 1024 == 0, "swizzle-atom alignment");
+  static constexpr int SMEM = XBUFS * XBUF + SBUFS * XSTAGE + 2 * STAGES * STAGE + 1024 + RB_BAR_BYTES + EPI_STAGE;
+  static_assert(STAGES >= 2 && SMEM <= 227 * 1024, "shared-memory budget");
+  static_assert(XBUFS >= 2 && 2 * 8 * XBUFS <= 64, "x ring");
+  static_assert(XPLANE % 1024 == 0 && XSTAGE % 1024 == 0 && STAGE % 1024 == 0, "swizzle-atom alignment");
 };
 
 // element offset of column c (a multiple of 4) of row r in a K-major plane of SWB-byte rows with the SWB-byte swizzle
@@ -106,17 +123,20 @@ __global__ void __launch_bounds__(CTC_THREADS, 1)
 resblock_pair_tc_kernel(const __grid_constant__ RbTcMaps maps, const RbTcArgs g) {
   using Cfg = RbTcCfg<C, NP>;
   pdl_trigger();
-  constexpr int STAGES = Cfg::STAGES, SWB = Cfg::SWB;
+  constexpr int STAGES = Cfg::STAGES, SWB = Cfg::SWB, XBUFS = Cfg::XBUFS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t smem_x = (raw + 1023u) & ~1023u;                  // two per-warpgroup activation buffers
-  const uint32_t smem_w = smem_x + 2 * Cfg::XBUF;                  // the two weight rings (warpgroup 0, warpgroup 1)
+  const uint32_t smem_x = (raw + 1023u) & ~1023u;                  // the x ring: buffer s at smem_x + s * XBUF
+  const uint32_t smem_s = smem_x + XBUFS * Cfg::XBUF;              // fp32 staging: buffer u at smem_s + u * XSTAGE
+  const uint32_t smem_w = smem_s + Cfg::SBUFS * Cfg::XSTAGE;       // the two weight rings (warpgroup 0, warpgroup 1)
   const uint32_t bars = smem_w + 2 * STAGES * Cfg::STAGE;
   // ring w: slot s at ring(w) + s * STAGE, its barriers at full_bar(w) + 8 s / empty_bar(w) + 8 s
   auto ring = [&](int w) { return smem_w + (uint32_t)(w * STAGES * Cfg::STAGE); };
   auto full_bar = [&](int w) { return bars + (uint32_t)(w * 16 * STAGES); };
   auto empty_bar = [&](int w) { return bars + (uint32_t)(w * 16 * STAGES + 8 * STAGES); };
-  float* epi_stage = reinterpret_cast<float*>(smem_raw + (bars + 256 - raw));
+  auto xfull_bar = [&](int s) { return bars + 256u + (uint32_t)(8 * s); };
+  auto xempty_bar = [&](int s) { return bars + 256u + (uint32_t)(8 * (XBUFS + s)); };
+  float* epi_stage = reinterpret_cast<float*>(smem_raw + (bars + RB_BAR_BYTES - raw));
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -138,17 +158,65 @@ resblock_pair_tc_kernel(const __grid_constant__ RbTcMaps maps, const RbTcArgs g)
         mbar_init(full_bar(w) + 8 * s, 1);
         mbar_init(empty_bar(w) + 8 * s, 4);     // one arrive per warp of the ring's warpgroup
       }
+    for (int s = 0; s < XBUFS; ++s) {
+      mbar_init(xfull_bar(s), RB_LOADER_THREADS);
+      mbar_init(xempty_bar(s), 4);              // one arrive per warp of the item's warpgroup
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();
 
+  constexpr int PL = Cfg::XPLANE / 2;                  // plane stride (elements)
+  constexpr int fmt = 3 - NP;
+
   if (warp >= 8) {
+    setmaxnreg_dec<CTC_PRODUCER_REGS>();
+    if (warp > 8) {
+      // ================= x loader: the fp32 rows of item li of the CTA -> cp.async -> staging buffer li % SBUFS; then
+      // leaky -> operand planes of x buffer li % XBUFS.  Each thread converts exactly the float4s it copied, so its own
+      // cp.async.wait_group is all the ordering the staging buffer needs
+      constexpr int CQ = C / 4, SB = Cfg::SBUFS;
+      const int lt = threadIdx.x - 9 * 32;
+      const int total = (128 + 2 * h1) * CQ;
+      for (int li = 0; li < n_items + SB - 1; ++li) {
+        if (li < n_items) {
+          const int item = blockIdx.x + li * gridDim.x;
+          const int tb = item % num_t, b = item / num_t;
+          const float* xb = g.x + (int64_t)b * T * C;
+          const int t0 = tb * R - h1 - h2;
+          const uint32_t st = smem_s + (li % SB) * Cfg::XSTAGE;
+          for (int i = lt; i < total; i += RB_LOADER_THREADS) {
+            int t = t0 + i / CQ;
+            if (t < 0) t = -t;
+            if (t >= T) t = 2 * (T - 1) - t;
+            const bool in = t >= 0 && t < T;           // a row outside the sequence after the reflection: zeros
+            cp_async16(st + 16 * i, in ? xb + (int64_t)t * C + (i % CQ) * 4 : xb, in ? 16u : 0u);
+          }
+        }
+        cp_async_commit();                             // (an empty group past the last item)
+        const int lc = li - (SB - 1);                  // the item converted now: its copies were committed SB - 1 groups ago
+        if (lc < 0) continue;
+        cp_async_wait<SB - 1>();
+        const int s = lc % XBUFS;
+        mbar_wait(xempty_bar(s), ((lc / XBUFS) & 1) ^ 1);
+        const float4* sv = reinterpret_cast<const float4*>(smem_raw + (smem_s + (lc % SB) * Cfg::XSTAGE - raw));
+        __nv_bfloat16* xg = reinterpret_cast<__nv_bfloat16*>(smem_raw + (smem_x + s * Cfg::XBUF - raw));
+        for (int i = lt; i < total; i += RB_LOADER_THREADS) {
+          const float4 v = sv[i];
+          float f[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) f[e] = act_apply(f[e], MTTS_ACT_LEAKY, 0.1f);
+          store_planes4(xg, PL, sw_elem<SWB>(i / CQ, (i % CQ) * 4), f, fmt, g.ovf);
+        }
+        fence_proxy_async_smem();
+        mbar_arrive(xfull_bar(s));
+      }
+      return;
+    }
     // ================= weight producer: per pair of items conv1 | conv1 | conv2 | conv2, k tap tiles each, item 2p + e
     // (owned by warpgroup e) into ring e.  Waiting on ring e's empty slot cannot deadlock: before warpgroup e waits for
-    // its slab n it has released every slab up to n - 2, and the producer needs slab n - STAGES (STAGES >= 3) released
-    setmaxnreg_dec<CTC_PRODUCER_REGS>();
-    if (warp != 8) return;
+    // its slab n it has released every slab up to n - 2, and the producer needs slab n - STAGES (STAGES >= 2) released
     const bool leader = elect_one();
     int stage[2] = {0, 0}, phase[2] = {0, 0};
     for (int p = 0; 2 * p < n_items; ++p) {
@@ -174,12 +242,8 @@ resblock_pair_tc_kernel(const __grid_constant__ RbTcMaps maps, const RbTcArgs g)
   setmaxnreg_inc<CTC_CONSUMER_REGS>();
   constexpr float CS = NP == 2 ? F16X2_INV_SCALE : 1.0f;
   constexpr int NCOR = NP == 1 ? 1 : C / 2;
-  constexpr int PL = Cfg::XPLANE / 2;                  // plane stride (elements)
-  constexpr int fmt = 3 - NP;
   const int wg = warp >> 2, w4 = warp & 3, tid = threadIdx.x & 127;
   const int chunk = lane & 3, rsub = lane >> 2;
-  const uint32_t xs = smem_x + wg * Cfg::XBUF;
-  __nv_bfloat16* xg = reinterpret_cast<__nv_bfloat16*>(smem_raw + (xs - raw));
   float* stg = epi_stage + warp * (16 * 20);
   float acc[2][C / 2], cor[2][NCOR];
 
@@ -225,40 +289,12 @@ resblock_pair_tc_kernel(const __grid_constant__ RbTcMaps maps, const RbTcArgs g)
     const int tb = item % num_t, b = item / num_t;
     const int r0 = tb * R;
     const float* xb = g.x + (int64_t)b * T * C;
+    const int s = li % XBUFS;
+    const uint32_t xs = smem_x + s * Cfg::XBUF;
+    __nv_bfloat16* xg = reinterpret_cast<__nv_bfloat16*>(smem_raw + (xs - raw));
 
-    // ---- 1. x rows -> leaky -> operand planes (the previous item's MMAs have retired in every warp)
-    named_bar_sync(1 + wg, 128);
-    {
-      constexpr int CQ = C / 4;
-      const int total = (128 + 2 * h1) * CQ;
-      const int t0 = r0 - h1 - h2;
-      constexpr int NL = 12;                           // loads in flight per thread (the accumulators are dead here)
-      for (int i0 = tid; i0 < total; i0 += NL * 128) {
-        float4 v[NL];
-#pragma unroll
-        for (int u = 0; u < NL; ++u) {
-          const int i = i0 + u * 128;
-          v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (i < total) {
-            int t = t0 + i / CQ;
-            if (t < 0) t = -t;
-            if (t >= T) t = 2 * (T - 1) - t;
-            if (t >= 0 && t < T) v[u] = __ldg(reinterpret_cast<const float4*>(xb + (int64_t)t * C + (i % CQ) * 4));
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < NL; ++u) {
-          const int i = i0 + u * 128;
-          if (i >= total) break;
-          float f[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) f[e] = act_apply(f[e], MTTS_ACT_LEAKY, 0.1f);
-          store_planes4(xg, PL, sw_elem<SWB>(i / CQ, (i % CQ) * 4), f, fmt, g.ovf);
-        }
-      }
-    }
-    fence_proxy_async_smem();
-    named_bar_sync(1 + wg, 128);
+    // ---- 1. the loader's x planes of this item
+    mbar_wait(xfull_bar(s), (li / XBUFS) & 1);
 
     // ---- 2. conv1: intermediate row i = position r0 - h2 + i reads x plane rows i + j d
     run_conv((2 * (li >> 1)) * k, xs, g.dil);
@@ -308,8 +344,10 @@ resblock_pair_tc_kernel(const __grid_constant__ RbTcMaps maps, const RbTcArgs g)
     fence_proxy_async_smem();
     named_bar_sync(1 + wg, 128);
 
-    // ---- 4. conv2: output row i reads intermediate rows i + j
+    // ---- 4. conv2: output row i reads intermediate rows i + j; once its MMAs have retired the buffer goes back to the
+    // loader
     run_conv((2 * (li >> 1) + 1) * k, xs, 1);
+    if (lane == 0) mbar_arrive(xempty_bar(s));
 
     // ---- 5. epilogue 2: bias -> residual -> scale -> accumulate -> fp32 (the arithmetic of conv_tc_kernel's epilogue)
     float* yb = g.y + (int64_t)b * T * C;

@@ -56,6 +56,14 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
+// 16-byte global -> shared copy that completes asynchronously (L2 only); src_bytes = 0 zero-fills the destination
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// the executing thread's copies of all but its N most recent groups have landed
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 // generic-proxy shared-memory writes (operands staged by threads) become visible to the MMA's async proxy
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
