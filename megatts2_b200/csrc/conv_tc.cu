@@ -735,7 +735,7 @@ bool conv_tc_eligible(const mtts_conv_params& p) {
   if (p.Cin % 8 != 0 || p.Cin < 32) return false;
   if (!p.tc_presplit && (p.ldx % 4 != 0 || (p.x_batch_stride % 4) != 0 || (((uintptr_t)p.x) & 15) != 0)) return false;
   if (!(p.Cout == 32 || p.Cout == 64 || (p.Cout >= 128 && p.Cout % 32 == 0))) return false;
-  if (p.Cin < 64 && p.Cout != 32) return false;          // the SWB=64 variant is instantiated for BN=32 only
+  if (p.Cin < 64 && p.Cout != 32) return false;          // Cin < 64 (64-byte K-slabs) is planned at BN = 32 only
   if (p.y && (p.ldy % 4 != 0 || p.y_batch_stride % 4 != 0 || (((uintptr_t)p.y) & 15) != 0)) return false;
   if (!p.y && (!p.tc_out_planes || p.accumulate)) return false;
   if (p.tc_out_planes && (p.Cout % 32 != 0 || p.tc_out_ld % 4 != 0 || p.tc_out_plane_stride % 4 != 0)) return false;
@@ -912,8 +912,10 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
          : np == 2 ? conv_tc_launch<64, 128, 2, 1>(maps, a, st) : conv_tc_launch<64, 128, 3, 1>(maps, a, st);
   }
   if (splits > 1) {
-    MTTS_TRY(np == 1 ? (conv_tc_launch<128, 128, 1>(maps, a, st))
-           : np == 2 ? (conv_tc_launch<128, 128, 2>(maps, a, st)) : (conv_tc_launch<128, 128, 3>(maps, a, st)));
+    // a split launch runs at BN = 128 on the plan's K-slab width (MEGATTS2_TC_SWB64 = 1 gives it 64-byte slabs): the kernel's
+    // stage size must match the boxes the descriptors above were encoded with
+    MTTS_TRY(np == 1 ? conv_tc_dispatch<1>(maps, a, 128, SWB, st)
+           : np == 2 ? conv_tc_dispatch<2>(maps, a, 128, SWB, st) : conv_tc_dispatch<3>(maps, a, 128, SWB, st));
     // the rows' LayerNorm rides on the reduction when the caller asked for it and a row is 3 / 4 / 6 / 8 x 128 wide
     if (ln_fuse() && ln && ln->po.p && a.y && !a.op && a.out_shift == 0 && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384) &&
         p.ldy % 4 == 0 && ln->po.ld % 4 == 0 && ln->po.stride % 4 == 0) {

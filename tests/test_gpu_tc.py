@@ -29,19 +29,37 @@ CASES = [
     dict(M=4096, K=1024, N=3072, bias=True),
     dict(M=1000, K=1024, N=4096, bias=True, relu=True),            # M tail
     dict(M=2048, K=4096, N=1024, bias=True, res=True),
-    dict(M=300, K=768, N=2304, bias=True),                         # ADM qkv
-    dict(M=640, K=72, N=192),                                      # K tail, N not a multiple of 128
+    dict(M=300, K=768, N=2304, bias=True, plan=dict(BN=64)),       # ADM qkv
+    dict(M=640, K=72, N=192, plan=dict(BN=32)),                    # K tail, N not a multiple of 128
     dict(M=129, K=1024, N=1024, res=True),
-    dict(M=8192, K=4096, N=1024, bias=True, res=True),             # 256-wide tiles, long K
-    dict(M=5000, K=1024, N=768, bias=True, relu=True),             # 256-wide tiles, M tail
-    dict(M=16384, K=80, N=512, bias=True),                         # 256-wide tiles, K tail inside a 32-wide slab
+    dict(M=8192, K=4096, N=1024, bias=True, res=True, plan=dict(BN=128)),   # long K
+    dict(M=5000, K=1024, N=768, bias=True, relu=True, plan=dict(BN=128)),   # M tail
+    dict(M=16384, K=80, N=512, bias=True, plan=dict(BN=128)),      # K tail inside the second 64-wide slab
 ]
 
 
+def _ids(c):
+    return "-".join(f"{k}{v}" for k, v in c.items() if k != "plan")
+
+
+def assert_plan(c, B, T, Cin, Cout, k, dil, engine):
+    """the plan a case exists to reach (key `plan`), as the dispatcher reports it for the 132 SMs of an H100 SXM
+    (mtts_tc_plan_query; no partial-sum space: these calls cannot split K)"""
+    import ctypes
+    from megatts2_b200 import _lib as L
+    if "plan" not in c:
+        return
+    out = (ctypes.c_int32 * 5)()
+    L.check(L.lib().mtts_tc_plan_query(132, B, T, Cin, Cout, k, dil, fmt_of(engine), 0, 0, out))
+    got = dict(BN=out[0], splits=out[1], halo=out[3], swb=out[4])
+    assert {key: got[key] for key in c["plan"]} == c["plan"], (c, got)
+
+
 @pytest.mark.parametrize("engine", ENGINES)
-@pytest.mark.parametrize("c", CASES, ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
+@pytest.mark.parametrize("c", CASES, ids=_ids)
 def test_linear_tc_vs_fp64(c, engine):
     from megatts2_b200 import ops
+    assert_plan(c, 1, c["M"], c["K"], c["N"], 1, 1, engine)
     g = gen(c["M"] + c["K"] + c["N"])
     x = torch.randn(c["M"], c["K"], generator=g) * 2
     w = torch.randn(c["N"], c["K"], generator=g) / math.sqrt(c["K"])
@@ -156,28 +174,29 @@ CONV_TC_CASES = [
     dict(B=2, T=300, Cin=384, Cout=384, k=5, pre=1),                                   # VQPE ConvBlock (Cin % 64 == 0)
     dict(B=2, T=1000, Cin=256, Cout=256, k=11, dil=5, pad_mode=1, pre=2, res=True),    # HiFi-GAN stage 1
     dict(B=3, T=777, Cin=128, Cout=128, k=3, dil=3, pad_mode=1, pre=2),                # stage 2, ragged tile
-    dict(B=2, T=2000, Cin=64, Cout=64, k=7, dil=3, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3),   # BN = 64
-    dict(B=2, T=3000, Cin=32, Cout=32, k=3, pad_mode=1, pre=2),                        # BN = 32, 64-byte swizzle
+    # C = 64 at 32 tiles: plain BN = 32 (the fill rule narrows the tile)
+    dict(B=2, T=2000, Cin=64, Cout=64, k=7, dil=3, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3, plan=dict(BN=32, halo=0)),
+    dict(B=2, T=3000, Cin=32, Cout=32, k=3, pad_mode=1, pre=2, plan=dict(BN=32, swb=64, halo=1)),
     dict(B=2, T=1500, Cin=32, Cout=32, k=11, dil=1, pad_mode=1, pre=2, res=True),
     dict(B=2, T=64, Cin=512, Cout=1024, k=5, post=1),                                  # conv-FF first conv
     dict(B=2, T=64, Cin=1024, Cout=512, k=5, res=True),                                # conv-FF second conv
     dict(B=1, T=130, Cin=96, Cout=160, k=3, pad_mode=2),                               # odd sizes: K and N tails
-    # full-machine grids (>= 132 tiles), long sequences
-    dict(B=4, T=5000, Cin=64, Cout=64, k=7, dil=3, pad_mode=1, pre=2, res=True),
-    dict(B=4, T=5000, Cin=64, Cout=64, k=11, dil=5, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3),
-    dict(B=4, T=5000, Cin=64, Cout=64, k=3, dil=1, pad_mode=1, pre=2),
-    dict(B=4, T=5001, Cin=32, Cout=32, k=11, dil=5, pad_mode=1, pre=2, res=True),
-    dict(B=4, T=5000, Cin=32, Cout=32, k=3, dil=1, pad_mode=1, pre=2),
-    dict(B=4, T=4999, Cin=32, Cout=32, k=7, dil=3, pad_mode=0),
-    # 256-wide tiles (Cout >= 256 and enough tiles to fill the machine)
-    dict(B=8, T=2000, Cin=256, Cout=256, k=7, dil=3, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3),
-    dict(B=8, T=1001, Cin=512, Cout=512, k=3, pre=1, post=1),
-    dict(B=16, T=700, Cin=192, Cout=768, k=5, pad_mode=2),
+    # full-machine grids (>= 132 tiles), long sequences: the halo form
+    dict(B=4, T=5000, Cin=64, Cout=64, k=7, dil=3, pad_mode=1, pre=2, res=True, plan=dict(BN=64, halo=1)),
+    dict(B=4, T=5000, Cin=64, Cout=64, k=11, dil=5, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3, plan=dict(BN=64, halo=1)),
+    dict(B=4, T=5000, Cin=64, Cout=64, k=3, dil=1, pad_mode=1, pre=2, plan=dict(BN=64, halo=1)),
+    dict(B=4, T=5001, Cin=32, Cout=32, k=11, dil=5, pad_mode=1, pre=2, res=True, plan=dict(BN=32, swb=64, halo=1)),
+    dict(B=4, T=5000, Cin=32, Cout=32, k=3, dil=1, pad_mode=1, pre=2, plan=dict(BN=32, swb=64, halo=1)),
+    dict(B=4, T=4999, Cin=32, Cout=32, k=7, dil=3, pad_mode=0, plan=dict(BN=32, swb=64, halo=1)),
+    # BN = 128 tiles (Cout >= 256 and enough tiles to fill the machine)
+    dict(B=8, T=2000, Cin=256, Cout=256, k=7, dil=3, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3, plan=dict(BN=128)),
+    dict(B=8, T=1001, Cin=512, Cout=512, k=3, pre=1, post=1, plan=dict(BN=128)),
+    dict(B=16, T=700, Cin=192, Cout=768, k=5, pad_mode=2, plan=dict(BN=128)),
 ]
 
 
 @pytest.mark.parametrize("engine", ENGINES)
-@pytest.mark.parametrize("case", CONV_TC_CASES, ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
+@pytest.mark.parametrize("case", CONV_TC_CASES, ids=_ids)
 def test_conv_tc_vs_fp64(case, engine):
     import torch.nn.functional as F
     from megatts2_b200 import ops
@@ -185,7 +204,8 @@ def test_conv_tc_vs_fp64(case, engine):
     c.update(case)
     k, dil = c["k"], c["dil"]
     pad = dil * (k - 1) // 2
-    g = gen(sum(v if isinstance(v, int) else 1 for v in case.values()))
+    assert_plan(c, c["B"], c["T"], c["Cin"], c["Cout"], k, dil, engine)
+    g = gen(sum(v if isinstance(v, int) else 1 for key, v in case.items() if key != "plan"))
     x = torch.randn(c["B"], c["T"], c["Cin"], generator=g)
     w = torch.randn(c["Cout"], c["Cin"], k, generator=g) / math.sqrt(c["Cin"] * k)
     b = torch.randn(c["Cout"], generator=g)
