@@ -46,7 +46,6 @@ struct ConvTcArgs {
   int32_t splits; float* partial;
   int32_t fmt; int32_t* ovf;   // operand format of the plane output (== the kernel's own NP) and the f16 range flag
   int32_t row0;                // first padded row of this conv inside a shared plane buffer (0 for its own planes)
-  int32_t bo_mode;             // halo form, diagnostics: 1 = put (addr >> 7) & 7 into the descriptors' base-offset field
 };
 
 // One CTA = 2 consumer warpgroups + 1 TMA producer warpgroup, persistent over the work items, a STAGES-deep ring of
@@ -234,7 +233,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       mbar_wait(full_bar + 8 * stage, phase);
       // HALO: A is the halo tile shifted by kb * dil rows (kb == tap: one K-slab per tap).  The swizzle is a function of the
       // shared-memory ADDRESS bits (the TMA wrote with them, the MMA reads with them), so a start address that is a whole
-      // number of rows into the tile needs nothing else; bo_mode = 1 puts the row phase into the base-offset field instead.
+      // number of rows into the tile needs nothing else.
       const uint32_t a_addr = HALO ? smem_a + ab * NP * Cfg::A_PLANE + (uint32_t)(kb * g.dil) * SWB
                                    : smem_base + stage * Cfg::STAGE;
       const uint32_t b_addr = smem_base + stage * Cfg::STAGE + (HALO ? 0 : NP * Cfg::A_PLANE);
@@ -248,8 +247,8 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
 #pragma unroll
         for (int hv = 0; hv < HALVES; ++hv) {                  // rows [64 hv, 64 hv + 64) of the item
           const uint32_t aa = a_addr + hv * 64 * SWB + ks * 32;
-          const uint64_t a1 = wgmma_desc_shifted(desc_base, aa, HALO ? g.bo_mode : 0);
-          const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::A_PLANE, HALO ? g.bo_mode : 0);
+          const uint64_t a1 = wgmma_desc_shifted(desc_base, aa);
+          const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::A_PLANE);
           if constexpr (NP == 1) {
             Wgmma<BN>::template mma<BF16>(acc[hv], a1, b1, f);       // x1 w1: the only product
           } else if constexpr (NP == 2) {
@@ -257,7 +256,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
             Wgmma<BN>::template mma<BF16>(cor[hv], a2, b1, 1u);      // x2' w1
             Wgmma<BN>::template mma<BF16>(acc[hv], a1, b1, f);       // x1 w1
           } else {
-            const uint64_t a3 = wgmma_desc_shifted(desc_base, aa + 2 * Cfg::A_PLANE, HALO ? g.bo_mode : 0);
+            const uint64_t a3 = wgmma_desc_shifted(desc_base, aa + 2 * Cfg::A_PLANE);
             const uint64_t b3 = desc_base | (uint64_t)(((bb + 2 * Cfg::B_PLANE) >> 4) & 0x3FFF);
             Wgmma<BN>::template mma<BF16>(cor[hv], a2, b2, f);       // x2 w2   (smallest terms first)
             Wgmma<BN>::template mma<BF16>(cor[hv], a1, b3, 1u);      // x1 w3
@@ -611,37 +610,6 @@ int tc_overflow_bind(int32_t* flag) {
   return 0;
 }
 
-// tuning switches (diagnostics), read ONCE per process: MEGATTS2_TC_SPLITK = 0 disables split-K, _SPLITK_MAX / _SPLITK_MARGIN
-// tune its cost model, MEGATTS2_TC_SWB64 = 1 forces 64-byte swizzle rows
-struct CtcEnv { bool splitk; int sk_max; double margin; double ln_red; bool swb64; bool halo; int halo_bo; int model; };
-static const CtcEnv& ctc_env() {
-  static const CtcEnv env = [] {
-    CtcEnv e;
-    const char* ke = getenv("MEGATTS2_TC_SPLITK");
-    const char* me = getenv("MEGATTS2_TC_SPLITK_MAX");
-    const char* ge = getenv("MEGATTS2_TC_SPLITK_MARGIN");
-    const char* se = getenv("MEGATTS2_TC_SWB64");
-    e.splitk = !(ke && ke[0] == '0');
-    e.sk_max = me ? atoi(me) : 8;
-    e.margin = ge ? atof(ge) : 0.85;
-    // modelled cycles of a reduction that REPLACES the LayerNorm launch that would follow anyway (tc_splitk_reduce_ln_kernel),
-    // against 9000 for a reduction in a launch of its own
-    const char* le = getenv("MEGATTS2_TC_SPLITK_LNCOST");
-    e.ln_red = le ? atof(le) : 2000.0;
-    e.swb64 = se && se[0] == '1';
-    const char* he = getenv("MEGATTS2_TC_HALO");          // 0: every tap re-loads its activation tile (the plain form)
-    const char* be = getenv("MEGATTS2_TC_HALO_BO");       // 1: base-offset field set in the row-shifted descriptors (diagnostics)
-    e.halo = !(he && he[0] == '0');
-    e.halo_bo = be ? atoi(be) : 0;
-    // dense-layer dispatch: 0 = tile width by grid fill, 1 = tile width by modelled cost (default), 2 = tile width and K split
-    // both by modelled cost (experimental)
-    const char* mo = getenv("MEGATTS2_TC_MODEL");
-    e.model = mo ? atoi(mo) : 1;
-    return e;
-  }();
-  return env;
-}
-
 struct CMapKey {
   const void* p; uint64_t d0, d1, d2, b0, b1; int swb, dt;
   bool operator==(const CMapKey& o) const {
@@ -703,9 +671,10 @@ int cmap_get(const void* p, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, 
 template <int BN, int SWB, int NP, int HALO = 0>
 static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, cudaStream_t st) {
   using Cfg = ConvTcCfg<BN, SWB, NP, HALO>;
+  static_assert(SWB == 128 || BN == 32, "64-byte K-slabs run at BN = 32 only");
   // one bit per instantiation in the per-device table (the max-dynamic-shared-memory attribute is per device)
-  constexpr int slot = HALO ? 18 + (BN == 64 ? 0 : 1) + 2 * (3 - NP)
-                            : (BN == 128 ? 0 : BN == 64 ? 1 : 2) + 3 * (SWB == 128 ? 0 : 1) + 6 * (3 - NP);
+  constexpr int slot = HALO ? 12 + (BN == 64 ? 0 : 1) + 2 * (3 - NP)
+                            : (BN == 128 ? 0 : BN == 64 ? 1 : SWB == 128 ? 2 : 3) + 4 * (3 - NP);
   static_assert(slot < 24, "attribute slots (24-31: resblock_tc.cu)");
   MTTS_TRY(tc_smem_attr((const void*)conv_tc_kernel<BN, SWB, NP, HALO>, slot, Cfg::SMEM));
   const int sms = cur_device_sms();
@@ -718,9 +687,10 @@ static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, cudaStrea
 
 template <int NP>
 static int conv_tc_dispatch(const ConvTcMaps& maps, const ConvTcArgs& a, int BN, int SWB, cudaStream_t st) {
-  if (SWB == 64 && BN == 128) return conv_tc_launch<128, 64, NP>(maps, a, st);
-  if (SWB == 64 && BN == 64) return conv_tc_launch<64, 64, NP>(maps, a, st);
-  if (SWB == 64) return conv_tc_launch<32, 64, NP>(maps, a, st);
+  if (SWB == 64) {
+    MTTS_REQUIRE(BN == 32 && a.splits == 1, "a plan with 64-byte K-slabs runs at BN = 32 without a K split");
+    return conv_tc_launch<32, 64, NP>(maps, a, st);
+  }
   if (BN == 128) return conv_tc_launch<128, 128, NP>(maps, a, st);
   if (BN == 64) return conv_tc_launch<64, 128, NP>(maps, a, st);
   return conv_tc_launch<32, 128, NP>(maps, a, st);
@@ -757,92 +727,69 @@ bool conv_tc_eligible(const mtts_conv_params& p) {
   return 3 * rows * p.Cin * 2 + 2048 <= p.tc_scratch_bytes;
 }
 
+// Split-K cost model of tc_plan: at most CTC_SPLITK_MAX splits, taken when the split launch models below
+// CTC_SPLITK_MARGIN of the unsplit one.  CTC_SPLITK_LN_RED: modelled cycles of a reduction that REPLACES the LayerNorm
+// launch that would follow anyway (tc_splitk_reduce_ln_kernel), against 9000 for a reduction in a launch of its own.
+constexpr int CTC_SPLITK_MAX = 8;
+constexpr double CTC_SPLITK_MARGIN = 0.85;
+constexpr double CTC_SPLITK_LN_RED = 2000.0;
+
 // The launch plan of one tap-GEMM: K-slab width, N-tile width, K splits, halo form.  A pure function of the shape, the SM
-// budget and the (read-once) tuning switches, so the policy can be queried and tested without a GPU
-// (mtts_tc_plan_query, tests/test_abi_and_host.py).
+// budget, the operand format, the partial-sum space and whether a LayerNorm rides on the reduction, so the policy can be
+// queried and tested without a GPU (mtts_tc_plan_query, tests/test_abi_and_host.py).
 struct TcPlan { int SWB, BN, splits; bool halo_form; };
-static TcPlan tc_plan(const CtcEnv& env, int sms, const mtts_conv_params& p, int np, bool ln_rides) {
+static TcPlan tc_plan(int sms, const mtts_conv_params& p, int np, bool ln_rides) {
   const int halo = p.dil * (p.k - 1);
-  int SWB = p.Cin >= 64 ? 128 : 64;
-  int BN = 32;
+  const int SWB = p.Cin >= 64 ? 128 : 64;
+  int BN = 32;             // Cin < 64 (64-byte K-slabs): conv_tc_eligible admits Cout = 32 only
   int splits = 1;
-  // modelled cycles per MMA: 65 at N = 128, 55 (the per-instruction floor) at N <= 64
-  if (env.model >= 2 && p.k == 1 && SWB == 128 && !env.swb64) {
-    // EXPERIMENTAL (MEGATTS2_TC_MODEL=2): tile width and K split of a dense layer chosen together by modelled launch cost.
-    // A persistent CTA walks ceil(items / SMs) work items of ceil(nk / sk) K-slabs each; a slab is 4 k-steps x 3 | 6 MMAs.
-    // Split-K partial sums are added in split order, so results never depend on timing.
-    const int64_t rows = (int64_t)p.B * p.Tout;
+  // N-tile width.  A persistent CTA walks ceil(tiles / SMs) tiles of nk K-slabs, so the width with the cheapest walk wins
+  // (modelled cycles per MMA: 65 at N = 128, 55, the per-instruction floor, at N <= 64) and ties go to the narrower tile
+  // (under-filled grids are latency-bound: more SMs stream the weights).  The fill rule (the widest tile that still gives
+  // 80 % of the SMs a tile) would e.g. run the PLM FF2 layer of steps 19 ... 28 as two waves of N = 64 tiles where one wave
+  // of N = 128 tiles does.  Convolutions (k > 1) keep the fill rule: their grids are hundreds of waves deep and the halo
+  // form wants BN == Cout.
+  if (SWB == 128) {
     const int64_t mt = (int64_t)p.B * cdiv64(p.Tout, 128);
-    const int nk = (p.Cin + 63) / 64;
-    const double mm = 4.0 * (np == 1 ? 1 : np == 2 ? 3 : 6);        // MMAs per 64-wide K-slab
-    double best = 1e30;
     const int cands[3] = {128, 64, 32};
-    for (int i = 0; i < 3; ++i) {
-      if (cands[i] > p.Cout) continue;
-      const double c = (double)cdiv64(mt * cdiv64(p.Cout, cands[i]), sms) * nk * mm * (cands[i] == 128 ? 65.0 : 55.0);
-      if (c <= best) { best = c; BN = cands[i]; }      // ties (same number of waves at the 55-cycle floor) go to the narrower
-    }                                                   // tile: more SMs stream the weights
-    if (env.splitk && p.out_shift == 0 && p.tc_partial && p.Cout >= 128) {
-      const int64_t t128 = mt * cdiv64(p.Cout, 128);
-      for (int sk = 2; sk <= env.sk_max && sk <= nk / 2; ++sk) {
-        if ((int64_t)sk * rows * p.Cout * 4 > p.tc_partial_bytes) break;
-        // + the reduction: its own launch unless it replaces the LayerNorm launch, + the partial sums written and read back
-        // through L2 (writes counted half)
-        const double red = (ln_rides ? 1800.0 : 7300.0) + (double)sk * rows * p.Cout * 4.0 * 6.9e-4;
-        const double c = (double)cdiv64(t128 * sk, sms) * (double)cdiv64(nk, sk) * mm * 65.0 + red;
-        if (c < best) { best = c; BN = 128; splits = sk; }
+    if (p.k == 1) {
+      int64_t best = INT64_MAX;
+      for (int i = 0; i < 3; ++i) {
+        if (cands[i] > p.Cout) continue;
+        const int64_t c = cdiv64(mt * cdiv64(p.Cout, cands[i]), sms) * (cands[i] == 128 ? 65 : 55);
+        if (c <= best) { best = c; BN = cands[i]; }
+      }
+    } else {
+      for (int i = 0; i < 3; ++i) {
+        if (cands[i] > p.Cout) continue;
+        BN = cands[i];
+        if (mt * cdiv64(p.Cout, cands[i]) >= (int64_t)(sms * 4) / 5) break;
       }
     }
-  } else {
-    // N-tile width.  A persistent CTA walks ceil(tiles / SMs) tiles of nk K-slabs, so the width with the cheapest walk wins
-    // and ties go to the narrower tile (under-filled grids are latency-bound: more SMs stream the weights).  The fill rule
-    // (the widest tile that still gives 80 % of the SMs a tile, MEGATTS2_TC_MODEL=0) would e.g. run the PLM FF2 layer of
-    // steps 19 ... 28 as two waves of N = 64 tiles where one wave of N = 128 tiles does.  Convolutions (k > 1) keep the fill
-    // rule: their grids are hundreds of waves deep and the halo form wants BN == Cout.
-    if (SWB == 128) {
-      const int64_t mt = (int64_t)p.B * cdiv64(p.Tout, 128);
-      const int cands[3] = {128, 64, 32};
-      if (env.model >= 1 && p.k == 1) {
-        int64_t best = INT64_MAX;
-        for (int i = 0; i < 3; ++i) {
-          if (cands[i] > p.Cout) continue;
-          const int64_t c = cdiv64(mt * cdiv64(p.Cout, cands[i]), sms) * (cands[i] == 128 ? 65 : 55);
-          if (c <= best) { best = c; BN = cands[i]; }
-        }
-      } else {
-        for (int i = 0; i < 3; ++i) {
-          if (cands[i] > p.Cout) continue;
-          BN = cands[i];
-          if (mt * cdiv64(p.Cout, cands[i]) >= (int64_t)(sms * 4) / 5) break;
-        }
+  }
+  // split-K for dense layers with too few output tiles to fill the GPU (the early steps of the AR loops, the N = 1024
+  // layers up to ~30 steps): narrow tiles would pay the per-MMA minimum on every k-step, so K is split across CTAs at full
+  // tile width instead and a second kernel reduces the partials
+  {
+    const int64_t rows = (int64_t)p.B * p.Tout;
+    const int64_t t128 = (int64_t)p.B * cdiv64(p.Tout, 128) * cdiv64(p.Cout, 128);
+    const int nk = (p.Cin + 63) / 64;
+    if (SWB == 128 && p.k == 1 && p.out_shift == 0 && p.tc_partial && p.Cout >= 128 && t128 < (int64_t)(sms * 4) / 5) {
+      int sk = (int)(sms / t128);
+      if (sk > CTC_SPLITK_MAX) sk = CTC_SPLITK_MAX;
+      if (sk > nk / 2) sk = nk / 2;
+      if (sk >= 2 && (int64_t)sk * rows * p.Cout * 4 <= p.tc_partial_bytes) {
+        const int64_t tiles_bn = (int64_t)p.B * cdiv64(p.Tout, 128) * cdiv64(p.Cout, BN);
+        const double waves = (double)cdiv64(tiles_bn, sms);
+        const double mmas = 4.0 * (np == 1 ? 1 : 2 * np);                                   // MMAs per 64-wide K-slab (modelled)
+        const double cost_now = waves * nk * mmas * (BN == 128 ? 65.0 : 55.0);                // cycles per CTA
+        const double cost_split = (double)cdiv64(nk, sk) * mmas * 65.0 + (ln_rides ? CTC_SPLITK_LN_RED : 9000.0);   // + reduction kernel
+        if (cost_split < CTC_SPLITK_MARGIN * cost_now) { splits = sk; BN = 128; }
       }
     }
-    // split-K for dense layers with too few output tiles to fill the GPU (the early steps of the AR loops, the N = 1024
-    // layers up to ~30 steps): narrow tiles would pay the per-MMA minimum on every k-step, so K is split across CTAs at full
-    // tile width instead and a second kernel reduces the partials
-    {
-      const int64_t rows = (int64_t)p.B * p.Tout;
-      const int64_t t128 = (int64_t)p.B * cdiv64(p.Tout, 128) * cdiv64(p.Cout, 128);
-      const int nk = (p.Cin + 63) / 64;
-      if (env.splitk && SWB == 128 && p.k == 1 && p.out_shift == 0 && p.tc_partial && p.Cout >= 128 &&
-          t128 < (int64_t)(sms * 4) / 5) {
-        int sk = (int)(sms / t128);
-        if (sk > env.sk_max) sk = env.sk_max;
-        if (sk > nk / 2) sk = nk / 2;
-        if (sk >= 2 && (int64_t)sk * rows * p.Cout * 4 <= p.tc_partial_bytes) {
-          const int64_t tiles_bn = (int64_t)p.B * cdiv64(p.Tout, 128) * cdiv64(p.Cout, BN);
-          const double waves = (double)cdiv64(tiles_bn, sms);
-          const double mmas = 4.0 * (np == 1 ? 1 : 2 * np);                                   // MMAs per 64-wide K-slab (modelled)
-          const double cost_now = waves * nk * mmas * (BN == 128 ? 65.0 : 55.0);                // cycles per CTA
-          const double cost_split = (double)cdiv64(nk, sk) * mmas * 65.0 + (ln_rides ? env.ln_red : 9000.0);   // + reduction kernel
-          if (cost_split < env.margin * cost_now) { splits = sk; BN = 128; }
-        }
-      }
-    }
-    if (env.swb64) SWB = 64;
   }
   // halo form: one K-slab per tap (Cin <= SWB / 2), the activation tile + halo fits the 192-row buffer
-  const bool halo_form = env.halo && splits == 1 && p.out_shift == 0 && p.k > 1 && p.Cin <= SWB / 2 &&
+  const bool halo_form = splits == 1 && p.out_shift == 0 && p.k > 1 && p.Cin <= SWB / 2 &&
                          halo + 128 <= CTC_HALO_ROWS &&   // (the halo kernel's epilogue has no K-split / transposed-conv paths)
                          ((SWB == 64 && BN == 32) || (SWB == 128 && BN == 64)) && p.Cout == BN;
   TcPlan pl;
@@ -862,7 +809,6 @@ static bool ln_fuse() {
 
 int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   if (ln) ln->done = 0;
-  const CtcEnv& env = ctc_env();
   const int sms = cur_device_sms();
   const int fmt = p.tc_fmt;
   const int np = 3 - fmt;                                     // operand planes
@@ -881,7 +827,7 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   }
   // the reduction of a split launch can carry the LayerNorm the caller asked for when a row is 3 / 4 / 6 / 8 x 128 wide
   const bool ln_rides = ln && ln->po.p && p.y && !p.tc_out_planes && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384);
-  const TcPlan pl = tc_plan(env, sms, p, np, ln_rides);
+  const TcPlan pl = tc_plan(sms, p, np, ln_rides);
   const int SWB = pl.SWB, BN = pl.BN, splits = pl.splits;
   const bool halo_form = pl.halo_form;
   // activation box: the work item's rows (ConvTcCfg::ROWS: 64 at BN = 128, else 128), the halo form adds the halo rows
@@ -903,7 +849,7 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   a.op = reinterpret_cast<__nv_bfloat16*>(p.tc_out_planes); a.op_stride = p.tc_out_plane_stride; a.op_ld = p.tc_out_ld;
   a.op_tp = p.tc_out_tp; a.op_hl = p.tc_out_hl; a.op_act = p.tc_out_act; a.op_slope = p.tc_out_slope;
   a.splits = splits; a.partial = reinterpret_cast<float*>(p.tc_partial);
-  a.fmt = fmt; a.ovf = ovf; a.bo_mode = env.halo_bo; a.row0 = p.tc_in_row0;
+  a.fmt = fmt; a.ovf = ovf; a.row0 = p.tc_in_row0;
   if (halo_form) {
     if (SWB == 64)
       return np == 1 ? conv_tc_launch<32, 64, 1, 1>(maps, a, st)
@@ -912,8 +858,8 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
          : np == 2 ? conv_tc_launch<64, 128, 2, 1>(maps, a, st) : conv_tc_launch<64, 128, 3, 1>(maps, a, st);
   }
   if (splits > 1) {
-    // a split launch runs at BN = 128 on the plan's K-slab width (MEGATTS2_TC_SWB64 = 1 gives it 64-byte slabs): the kernel's
-    // stage size must match the boxes the descriptors above were encoded with
+    // a split launch runs at BN = 128 on the plan's K-slab width: the kernel's stage size must match the boxes the
+    // descriptors above were encoded with
     MTTS_TRY(np == 1 ? conv_tc_dispatch<1>(maps, a, 128, SWB, st)
            : np == 2 ? conv_tc_dispatch<2>(maps, a, 128, SWB, st) : conv_tc_dispatch<3>(maps, a, 128, SWB, st));
     // the rows' LayerNorm rides on the reduction when the caller asked for it and a row is 3 / 4 / 6 / 8 x 128 wide
@@ -948,7 +894,7 @@ int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int 
   static float dummy;
   p.y = &dummy;
   if (partial_bytes > 0) { p.tc_partial = &dummy; p.tc_partial_bytes = partial_bytes; }
-  const TcPlan pl = tc_plan(ctc_env(), sms, p, 3 - fmt, ln_rides != 0);
+  const TcPlan pl = tc_plan(sms, p, 3 - fmt, ln_rides != 0);
   out5[0] = pl.BN; out5[1] = pl.splits; out5[2] = 0; out5[3] = pl.halo_form ? 1 : 0; out5[4] = pl.SWB;
   return 0;
 }

@@ -95,15 +95,6 @@ static int lin_planes(const TcScratch* tc, __nv_bfloat16* planes, int64_t M, int
   return rc;
 }
 
-// MEGATTS2_LAST_ROW_TC=0: the final layer's last-row work stays on the exact FFMA engine (read once)
-static bool last_row_tc() {
-  static const bool on = [] {
-    const char* e = getenv("MEGATTS2_LAST_ROW_TC");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
 // dense layer dispatch: one tap-GEMM call; conv1d() picks the wgmma engine when planes + scratch are attached
 // and the shape is eligible (M >= 128), else the exact FFMA engine
 static int lin(const mtts_encoder* e, const TcScratch* tc, const float* x, int ldx, int64_t M, int K, int N,
@@ -226,7 +217,7 @@ static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int 
       // final layer, last position only (exact: nothing else is consumed downstream)
       ap.q = qkv + (int64_t)(T - 1) * 3 * D; ap.q_sb = (int64_t)T * 3 * D; ap.q_st = 3 * D; ap.Tq = 1;
       if (mask) ap.mask = mask + (int64_t)(T - 1) * mask_sq;
-      if (fused && B >= 32 && last_row_tc()) {
+      if (fused && B >= 32) {
         // the B last rows as one half-filled 128-row tile on the tensor cores (split-K fills the SMs): the attention rows,
         // LN2 and FF1 write operand planes like the full-sequence layers.  The exact-FFMA form below took 21 + 5 us per
         // dense layer at B = 64 (weight streaming through the FP32 pipe), 4 layers per AR step.

@@ -402,16 +402,10 @@ int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t s
   // tensor-core path (attn_tc.cu): the head dims of the AR stacks once a sequence has more than 64 queries.  At the C4 step
   // shapes (Tq = Tk <= 64) a head is a 64 x 64 x 64 problem, all latency, so the AR steps of the benchmark stay on this fp32
   // kernel; longer sequences (teacher-forced forwards, config C3) go to the tensor cores.
-  // (MEGATTS2_ATTN_TC = 0 disables it, MEGATTS2_ATTN_TC_MIN sets the minimum Tq; read once per process)
   // That kernel splits Q, K and V into f16x2 planes, so only callers on an fp16-range engine take it; the bf16x3 and
   // FFMA engines keep the full fp32 range here.
   if (allow_f16_operands) {
-    static const int tc_min = [] {
-      const char* e = getenv("MEGATTS2_ATTN_TC");
-      if (e && e[0] == '0') return 1 << 30;
-      const char* m = getenv("MEGATTS2_ATTN_TC_MIN");
-      return m ? atoi(m) : 65;
-    }();
+    constexpr int tc_min = 65;
     if (p.Tq >= tc_min && attention_tc_eligible(p)) return attention_tc(p, st);
     // AR steps (Tq == Tk <= 64) on the tensor cores: one 64-row tile per head.  The operand conversions, not the MMAs, are
     // what a 64 x 64 x 64 head costs, so it is opt-in (mtts_set_attention_pair_min / MEGATTS2_ATTN_PAIR_MIN: shortest

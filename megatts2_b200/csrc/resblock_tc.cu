@@ -104,11 +104,11 @@ __device__ __forceinline__ void rb_tap(float (&acc)[2][C / 2], float (&cor)[2][N
 #pragma unroll
     for (int hv = 0; hv < 2; ++hv) {
       const uint32_t aa = a_addr + hv * 64 * Cfg::SWB + ks * 32;
-      const uint64_t a1 = wgmma_desc_shifted(desc_base, aa, 0);
+      const uint64_t a1 = wgmma_desc_shifted(desc_base, aa);
       if constexpr (NP == 1) {
         Wgmma<C>::template mma<false>(acc[hv], a1, b1, f);
       } else {
-        const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::XPLANE, 0);
+        const uint64_t a2 = wgmma_desc_shifted(desc_base, aa + Cfg::XPLANE);
         Wgmma<C>::template mma<false>(cor[hv], a1, b2, f);
         Wgmma<C>::template mma<false>(cor[hv], a2, b1, 1u);
         Wgmma<C>::template mma<false>(acc[hv], a1, b1, f);

@@ -420,9 +420,7 @@ int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st) {
     if (p.k == 1 && p.stride == 1 && p.pad == 0 && p.out_shift == 0 && !p.in_lens && M <= 256 && tiles64 <= sms &&
         nk >= 16 && p.tc_scratch) {
       // two CTAs per SM: a lone 8-warp CTA cannot hide the L2 latency of its one-chunk-ahead prefetch
-      static const int target_env = []() { const char* e = getenv("MEGATTS2_SPLITK_CTAS"); return e ? atoi(e) : 0; }();
-      const int target = target_env > 0 ? target_env : 2 * sms;
-      int splits = (int)(target / tiles64);
+      int splits = (int)(2 * sms / tiles64);
       if (splits > 16) splits = 16;
       if (splits > nk / 4) splits = nk / 4;
       if (splits >= 2 && (int64_t)splits * M * p.Cout * 4 + 256 <= p.tc_scratch_bytes) {

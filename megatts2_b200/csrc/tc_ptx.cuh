@@ -96,12 +96,11 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
   d |= (uint64_t)(SWB == 128 ? 1 : 2) << 62;           // SWIZZLE_128B : SWIZZLE_64B
   return d;
 }
-// descriptor of an operand whose start address is shifted by whole rows inside a swizzled tile: low word = address,
-// base offset (bits 49..51) = the row phase of the start address inside the 8-row swizzle pattern when bo_mode is set
-__device__ __forceinline__ uint64_t wgmma_desc_shifted(uint64_t desc_base, uint32_t smem_addr, int bo_mode) {
-  uint64_t d = desc_base | (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  if (bo_mode) d |= (uint64_t)((smem_addr >> 7) & 7) << 49;
-  return d;
+// descriptor of an operand whose start address is shifted by whole rows inside a swizzled tile: only the address changes.
+// The swizzle is a function of the shared-memory address bits, so the base-offset field (bits 49..51) stays 0; putting
+// the row phase there fails the parity tests on H100.
+__device__ __forceinline__ uint64_t wgmma_desc_shifted(uint64_t desc_base, uint32_t smem_addr) {
+  return desc_base | (uint64_t)((smem_addr >> 4) & 0x3FFF);
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -71,8 +71,9 @@ def _plan(M, K, N, ln=0, k=1, B=1, dil=1, partial=64 << 20, sms=132):
 
 def test_tap_gemm_launch_plan_policy():
     """The dispatcher's plan is a pure host function (csrc/conv_tc.cu tc_plan): dense-layer tile widths minimise
-    ceil(tiles / SMs) x per-MMA cost (65 cycles at N = 128, 55 below; ties to the narrower tile), splits need partial-sum
-    space, the small-channel vocoder convs take the halo form, and no plan uses CTA pairs (none exist on sm_90)."""
+    ceil(tiles / SMs) x per-MMA cost (65 cycles at N = 128, 55 below; ties to the narrower tile), convolutions take the
+    widest tile that fills 80 % of the SMs, splits need partial-sum space, Cin < 64 runs at BN = 32 on 64-byte K-slabs,
+    the small-channel vocoder convs take the halo form, and the ABI's CTA-pair slot stays 0."""
     from megatts2_b200 import ops
     sms = 132
     cd = lambda a, b: (a + b - 1) // b
@@ -99,6 +100,18 @@ def test_tap_gemm_launch_plan_policy():
     assert _plan(66816, 32, 32, k=7, B=64, dil=3, partial=0) == dict(BN=32, splits=1, pair=0, halo=1, swb=64)
     assert _plan(33408, 64, 64, k=7, B=64, dil=3, partial=0) == dict(BN=64, splits=1, pair=0, halo=1, swb=128)
     assert _plan(33408, 128, 128, k=11, B=64, dil=5, partial=0)["halo"] == 0
+    # convolutions (k > 1) keep the fill rule: 80 tiles of N = 128 leave more than a fifth of 132 SMs idle, so N = 64,
+    # where the dense-layer cost rule would take one wave of N = 128
+    for s in (16, 66, 100, 132):
+        fill = next((bn for bn in (128, 64) if cd(10240, 128) * cd(128, bn) >= s * 4 // 5), 32)
+        assert _plan(10240, 128, 128, k=3, partial=0, sms=s) == dict(BN=fill, splits=1, pair=0, halo=0, swb=128), s
+    assert _plan(10240, 128, 128, k=3, partial=0)["BN"] == 64
+    # Cin < 64 (64-byte K-slabs; the engine takes Cout = 32 only there): BN = 32 and no K split at every budget
+    for Cin in (32, 40, 48, 56):
+        for k, dil in ((1, 1), (2, 1), (3, 1), (3, 33), (7, 3), (11, 5)):
+            for s in (1, 3, 16, 66, 132):
+                pl = _plan(5000, Cin, 32, k=k, B=2, dil=dil, sms=s)
+                assert (pl["swb"], pl["BN"], pl["splits"], pl["pair"]) == (64, 32, 1, 0), (Cin, k, dil, s, pl)
 
 
 def test_no_cpu_fallback():

@@ -1,27 +1,22 @@
 """Every launch plan of the wgmma tap-GEMM (csrc/conv_tc.cu) against fp64.
 
 ``tc_plan()`` picks the instantiation of a call - tile width BN 128 / 64 / 32, K-slab width SWB 128 / 64 bytes, the plain
-or halo form, a K split with a fixed-order reduction - from the shape, the SM budget of the calling thread
-(``ops.launch_policy``) and the tuning switches (MEGATTS2_TC_HALO / _SWB64 / _SPLITK / _MODEL, read once per process).
-One table of cases runs on all three operand formats at SM budgets 1, 3, 16, 100 and the full device, and under each
-switch in a subprocess; every run logs the plan ``mtts_tc_plan_query`` reports for it and its error as a fraction of
-the bar:
+or halo form, a K split with a fixed-order reduction - from the shape, the operand format, the partial-sum space and the
+SM budget of the calling thread (``ops.launch_policy``).  One table of cases runs on all three operand formats at SM
+budgets 1, 3, 16, 100 and the full device; every run logs the plan ``mtts_tc_plan_query`` reports for it and its error as
+a fraction of the bar:
   * bf16x3 / f16x2: fp64 reference, fp32-grade bar 3e-5 * max(1, max|ref|);
   * f16: fp64 over the fp16-rounded operands, bar 1e-5 * max|ref| (only fp32 accumulation is left);
   * runs of one case and format whose plans are equal are bit-identical whatever the budget (each output element comes
     from one work item, or from a split reduction in a fixed order).
-The CPU test at the end checks that the table, over the budgets and switches, reaches every instantiation conv_tc() can
-launch, so a dispatcher change that orphans one fails without a GPU."""
+The CPU test at the end checks that the table, over the budgets, reaches every instantiation conv_tc() can launch and no
+other, so a dispatcher change that orphans one fails without a GPU."""
 import ctypes as C
 import functools
 import json
 import math
-import os
-import subprocess
-import sys
 import zlib
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -30,7 +25,6 @@ from megatts2_b200 import _lib as L
 from megatts2_b200 import pack
 
 DEV = "cuda"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 gpu = pytest.mark.gpu
 FMTS = [L.TC_BF16X3, L.TC_F16X2, L.TC_F16]
 FMT_NAMES = {L.TC_BF16X3: "bf16x3", L.TC_F16X2: "f16x2", L.TC_F16: "f16"}
@@ -82,27 +76,6 @@ CASES = {
     "split_m200_k4096_n512": _dense(200, 4096, 512, bias=True, post=LEAKY, partial=True),
     "split_m200_k4096_n384": _dense(200, 4096, 384, res=True, pre=RELU, op=NONE, partial=True),
 }
-DENSE = [n for n, c in CASES.items() if c["kind"] == "dense"]
-CONV = [n for n, c in CASES.items() if c["kind"] != "dense"]
-
-# the tuning switches, one process each: environment, the cases whose plans they can change, and what every plan must show
-SWITCHES = {
-    # MEGATTS2_RB_FUSE=0 as well: the vocoder's C = 32 / 64 ResBlock convs then run as tap-GEMMs in the plain form
-    "halo0": dict(env={"MEGATTS2_TC_HALO": "0", "MEGATTS2_RB_FUSE": "0"}, cases=CONV),
-    "swb64": dict(env={"MEGATTS2_TC_SWB64": "1"}, cases=list(CASES)),
-    "splitk0": dict(env={"MEGATTS2_TC_SPLITK": "0"}, cases=DENSE),
-    "model0": dict(env={"MEGATTS2_TC_MODEL": "0"}, cases=DENSE),
-    "model2": dict(env={"MEGATTS2_TC_MODEL": "2"}, cases=DENSE),
-}
-
-
-def _check_switch_plan(switch, plan):
-    if switch == "halo0":
-        assert not plan["halo"]
-    elif switch == "swb64":
-        assert plan["swb"] == 64
-    elif switch == "splitk0":
-        assert plan["splits"] == 1
 
 
 # ------------------------------------------------------------------------------------------ plans (host only)
@@ -133,11 +106,6 @@ def instantiation(pl, fmt):
     """the conv_tc_kernel<BN, SWB, NP, HALO> a plan launches, with the split-K flag"""
     form = "halo" if pl["halo"] else ("split" if pl["splits"] > 1 else "plain")
     return form, pl["BN"], pl["swb"], 3 - fmt
-
-
-def _plan_table(names):
-    return [dict(case=n, fmt=f, sms=s, plan=plan_of(CASES[n], f, s))
-            for n in names for f in FMTS for s in (1, 3, 16, 100, H100_SMS)]
 
 
 # ------------------------------------------------------------------------------------------ inputs and references
@@ -375,90 +343,20 @@ def test_splitk_layernorm_reduction_vs_fp64(D, H, fmt):
     assert torch.equal(y, enc(x.to(DEV))), "the split-K reduction order is fixed"
 
 
-# ------------------------------------------------------------------------------------------ GPU: forced switches
-def _model_checks(switch):
-    """model-level runs under a switch: PLM ids at B = 16 on engines 1 and 2 (golden), and with the halo form off the
-    HiFi-GAN waveform on bf16x3 against the oracle"""
-    import helpers
-    from oracle import ref_megatts2 as R
-    from oracle import weights as W
-    res = {}
-    with np.load(os.path.join(ROOT, "tests", "golden", "plm.npz")) as z:
-        g = {k: torch.from_numpy(z[k]) for k in z.files}
-    plm = helpers.build_plm(W.plm_state_dict(), DEV)
-    big = torch.cat([g["tc8"]] * 8, 0).to(DEV)
-    for engine in (1, 2):
-        plm.plm.engine = engine
-        ids = plm.infer(big)
-        res[f"plm_ids_engine{engine}"] = bool(torch.equal(ids.cpu(), torch.cat([g["ids"]] * 8, 0)))
-    if switch == "halo0":
-        sd = W.hifigan_state_dict()
-        hifi = helpers.build_hifigan(sd, DEV)
-        mel = torch.randn(2, 80, 30, generator=_gen("hifigan")) * 2 - 4
-        ref = R.hifigan_generator(sd, mel, W.HIFIGAN_CFG)
-        hifi.generator.engine = pack.ENGINE_BF16X3
-        res["hifigan_err"] = (hifi.decode_batch(mel.to(DEV)).cpu() - ref).abs().max().item()
-    return res
-
-
-def _switch_worker(switch, path):
-    """(subprocess entry) the switch's cases on every format and budget, then the model checks -> json at `path`"""
-    out = dict(records=[], failures=[])
-    for name in SWITCHES[switch]["cases"]:
-        for fmt in FMTS:
-            try:
-                out["records"] += run_case(name, fmt)
-            except AssertionError as e:
-                out["failures"].append(f"{name} {FMT_NAMES[fmt]}: {e}")
-    out["model"] = _model_checks(switch)
-    with open(path, "w") as f:
-        json.dump(out, f)
-
-
-def _in_subprocess(env, code, timeout):
-    src = f"import sys; sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'tests')!r}]\nimport test_gpu_tc_plans as T\n{code}"
-    return subprocess.run([sys.executable, "-c", src], check=True, env=dict(os.environ, **env), cwd=ROOT, timeout=timeout,
-                          stdout=subprocess.PIPE, text=True).stdout
-
-
-@gpu
-@pytest.mark.timeout(900)
-@pytest.mark.parametrize("switch", list(SWITCHES))
-def test_tap_gemm_plans_under_switch(switch, tmp_path):
-    path = str(tmp_path / f"{switch}.json")
-    log = _in_subprocess(SWITCHES[switch]["env"], f"T._switch_worker({switch!r}, {path!r})", 800)
-    print(log)
-    with open(path) as f:
-        out = json.load(f)
-    assert not out["failures"], out["failures"]
-    assert len(out["records"]) == len(SWITCHES[switch]["cases"]) * len(FMTS) * len(BUDGETS)
-    for rec in out["records"]:
-        _check_switch_plan(switch, rec["plan"])
-    m = out["model"]
-    assert m["plm_ids_engine1"] and m["plm_ids_engine2"], m
-    if switch == "halo0":
-        assert m["hifigan_err"] < 1e-4, m
-
-
 # ------------------------------------------------------------------------------------------ CPU: coverage of the table
-def test_table_reaches_every_instantiation():
-    """The plans of the table's cases - at budgets 1, 3, 16, 100 and 132 SMs, under the default switches and under each
-    forced switch (a subprocess each: the switches are read once per process) - together launch every conv_tc_kernel
-    instantiation conv_tc() has, and no split plan runs at a tile width other than 128."""
-    tables = {"default": _plan_table(list(CASES))}
-    for sw, spec in SWITCHES.items():
-        out = _in_subprocess(spec["env"], f"import json; print(json.dumps(T._plan_table({spec['cases']!r})))", 300)
-        tables[sw] = json.loads(out.strip().splitlines()[-1])
+def test_default_table_reaches_every_instantiation():
+    """The plans of the table's cases, at budgets 1, 3, 16, 100 and 132 SMs, together launch every conv_tc_kernel
+    instantiation conv_tc() has and no other, and no split plan runs at a tile width other than 128."""
     reached = set()
-    for sw, table in tables.items():
-        for r in table:
-            pl = r["plan"]
-            assert pl["splits"] == 1 or pl["BN"] == 128, (sw, r)
-            if sw in SWITCHES:
-                _check_switch_plan(sw, pl)
-            reached.add(instantiation(pl, r["fmt"]))
-    want = {("plain", bn, swb, npl) for bn in (128, 64, 32) for swb in (128, 64) for npl in (1, 2, 3)}
+    for n in CASES:
+        for fmt in FMTS:
+            for sms in (1, 3, 16, 100, H100_SMS):
+                pl = plan_of(CASES[n], fmt, sms)
+                assert pl["splits"] == 1 or pl["BN"] == 128, (n, fmt, sms, pl)
+                reached.add(instantiation(pl, fmt))
+    want = {("plain", bn, 128, npl) for bn in (128, 64, 32) for npl in (1, 2, 3)}
+    want |= {("plain", 32, 64, npl) for npl in (1, 2, 3)}
     want |= {("halo", bn, swb, npl) for bn, swb in ((32, 64), (64, 128)) for npl in (1, 2, 3)}
-    want |= {("split", 128, swb, npl) for swb in (128, 64) for npl in (1, 2, 3)}
+    want |= {("split", 128, 128, npl) for npl in (1, 2, 3)}
     assert not want - reached, sorted(want - reached)
     assert not reached - want, sorted(reached - want)       # a plan outside the instantiations conv_tc() can launch
