@@ -445,6 +445,21 @@ int mtts_plm_decode_causal_sample_f32(const mtts_plm* m, const float* tc_latent,
                                       int32_t B, int32_t T, int64_t* codes_out, float* logits_out, const mtts_sampling* s,
                                       void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Resumable MegaPLM.infer (greedy / sampled): runs AR steps [t0, t1) of the T-step decode, 0 <= t0 <= t1 <= T, against a
+ * caller-owned code state `code_state` (B, T+1) int64, row stride T+1: column 0 holds BOS (vq_bins) and columns 1..t0 the
+ * codes of steps < t0; step t writes column t+1.  codes_out (B,T) and logits_out (optional, (B,T,vq_bins)) are laid out as
+ * in mtts_plm_infer_f32; only columns [t0, t1) are written.  Step t reads only tc_latent[:, :t+1] and codes < t, and a
+ * sampled draw is keyed by (seed, key, t), so any split of [0, T) into consecutive ranges yields the codes and logits of
+ * one mtts_plm_infer_f32 / mtts_plm_infer_sample_f32 call.  Same workspace size: mtts_plm_infer_workspace_bytes(m, B, T);
+ * the workspace holds nothing between ranges. */
+int mtts_plm_infer_range_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                             int32_t B, int32_t T, int32_t t0, int32_t t1, int64_t* code_state,
+                             int64_t* codes_out, float* logits_out, void* workspace, int64_t workspace_bytes, void* stream);
+int mtts_plm_infer_range_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                    int32_t B, int32_t T, int32_t t0, int32_t t1, int64_t* code_state,
+                                    int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                                    void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ConvNet family (modules/convnet.py).  One ConvBlock = ReLU -> Conv1d(C,C,k,same) -> LN(C). */
 typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv_block;   /* w packed (k,C,C); w_tc (3,k,C,C) bf16 or NULL */
 

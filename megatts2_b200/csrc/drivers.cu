@@ -267,13 +267,19 @@ static int64_t plm_ws_floats(const mtts_plm* m, int B, int T) {
          2 * ((int64_t)B * (T + 1) + 64) + 6 * 64;
 }
 
-// smp == nullptr: greedy (argmax_rows); otherwise each step's codes are drawn by the opt-in sampler (sample.cu)
-static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
-                     float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st, const mtts_sampling* smp = nullptr) {
+// Steps [t0, t1) of the decode.  state == nullptr: the workspace's own code state, filled with BOS here (the whole decode,
+// t0 = 0); otherwise the caller's (B, T+1) code state, column 0 = BOS and columns 1..t0 = the codes of steps < t0.  Step t
+// reads columns <= t and writes column t+1 only, so any split of [0, T) into ranges enqueues the same kernels on the same
+// data as one call.  smp == nullptr: greedy (argmax_rows); otherwise each step's codes are drawn by the opt-in sampler
+// (sample.cu), keyed by the step index t, so the split does not change the draws either.
+static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int t0, int t1,
+                           int64_t* state, int64_t* codes_out, float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
+                           const mtts_sampling* smp) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
-  if (B <= 0 || T <= 0) return 0;
+  MTTS_REQUIRE(0 <= t0 && t0 <= t1 && t1 <= (T > 0 ? T : 0), "step range outside [0, T]");
+  if (B <= 0 || T <= 0 || t0 == t1) return 0;
   Arena top(ws, ws_bytes);
   float* X = top.take<float>((int64_t)B * T * D);
   float* xl = top.take<float>((int64_t)B * D);
@@ -285,8 +291,9 @@ static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_l
   if (enc_off + encoder_ws_floats(&m->enc, B, T) * 4 > ws_bytes)
     return fail(MTTS_ERR_WORKSPACE, "%s: workspace too small (need %lld bytes)", "plm_infer",
                 enc_off + encoder_ws_floats(&m->enc, B, T) * 4);
-  MTTS_TRY(fill_i64(codes, T + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
-  for (int t = 0; t < T; ++t) {
+  if (state) codes = state;
+  else MTTS_TRY(fill_i64(codes, T + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
+  for (int t = t0; t < t1; ++t) {
     const int S = t + 1;
     MTTS_TRY(plm_build_input(tc, tc_sb, tc_ld, m->tc_dim, codes, T + 1, m->pc_embedding, m->vq_dim, V + 2, m->pe,
                              m->pe_alpha, B, S, X, st));
@@ -306,6 +313,11 @@ static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_l
     else MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
   }
   return 0;
+}
+
+static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
+                     float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st, const mtts_sampling* smp = nullptr) {
+  return plm_infer_steps(m, tc, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, ws, ws_bytes, st, smp);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -932,6 +944,22 @@ int mtts_plm_infer_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
   MTTS_TRY(sampling_check(s, m->vq_bins));
   return plm_infer(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes, (cudaStream_t)stream, s);
+}
+int mtts_plm_infer_range_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
+                             int32_t t0, int32_t t1, int64_t* code_state, int64_t* codes_out, float* logits_out,
+                             void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && code_state, "null pointer");
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, nullptr);
+}
+int mtts_plm_infer_range_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                                    int32_t T, int32_t t0, int32_t t1, int64_t* code_state, int64_t* codes_out,
+                                    float* logits_out, const mtts_sampling* s, void* workspace, int64_t workspace_bytes,
+                                    void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && code_state, "null pointer");
+  MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s);
 }
 
 int64_t mtts_adm_infer_workspace_bytes(const mtts_adm* m, int32_t B, int32_t T) { return adm_ws_floats(m, B, T) * 4 + 8192; }

@@ -9,6 +9,7 @@ hard-wired to B = 1 at :170-171, :262-263); ``Megatts.synthesize`` is the tensor
 ``Megatts.forward`` (:353-373) for a batch of utterances."""
 import ctypes as C
 import glob
+import math
 
 import torch
 import torch.nn as nn
@@ -190,6 +191,70 @@ class MegaPLM(pack.PlanMixin, nn.Module):
                                  (tc, sampling.seed_tensor(tc.device), keys), run)
         return (out[0], out[1]) if return_logits else out[0]
 
+    def begin_decode(self, tc_latent: torch.Tensor, sampling: S.Sampling = None, keys=None) -> "PLMDecode":
+        """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
+        any number of ranges gives ``infer``'s codes and logits (same ``sampling`` and ``keys``)."""
+        _eval_only(self)
+        tc = ops._dev(tc_latent, name="tc_latent")
+        if tc.stride(2) != 1:
+            tc = tc.contiguous()
+        B, T, _ = tc.shape
+        state = torch.full((B, T + 1), self.vq_bins, dtype=torch.int64, device=tc.device)   # column 0 = BOS
+        if sampling is None:
+            return PLMDecode(tc, state, None, None, None)
+        return PLMDecode(tc, state, sampling, sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device))
+
+    def decode_until(self, dec: "PLMDecode", t1: int, return_logits: bool = False):
+        """Run steps [dec.t, t1) of the decode begun by ``begin_decode`` -> the new codes (B, t1 - dec.t) int64 [, their
+        logits (B, t1 - dec.t, vq_bins)].  Each range replays as a CUDA graph keyed by (B, T, t0, t1), from a cache of its
+        own (``_range_graphs``), so streaming never evicts ``infer``'s graphs; a captured range pins a private workspace of
+        ``mtts_plm_infer_workspace_bytes(B, T)`` bytes."""
+        _eval_only(self)
+        tc, B, T, t0 = dec.tc, dec.B, dec.T, dec.t
+        t1 = int(t1)
+        if not t0 <= t1 <= T:
+            raise L.MttsError(f"decode_until: t1 = {t1} outside [{t0}, {T}]")
+        V = self.vq_bins
+        if t1 == t0:
+            codes = torch.empty(B, 0, dtype=torch.int64, device=tc.device)
+            return (codes, torch.empty(B, 0, V, device=tc.device)) if return_logits else codes
+        pl = self._plan_get(tc.device, T)
+        lib = L.lib()
+        nbytes = lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T)
+
+        def run(tc_, state_, *smp):
+            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
+            logits = torch.empty(B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
+            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=tc_.device)   # private: a captured range pins it
+            args = (C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T, t0, t1, state_.data_ptr(),
+                    codes.data_ptr(), logits.data_ptr() if return_logits else None)
+            if smp:
+                s = dec.sampling.struct(*smp)
+                L.check(lib.mtts_plm_infer_range_sample_f32(*args, C.byref(s), ws.data_ptr(), nbytes, ops._stream()))
+            else:
+                L.check(lib.mtts_plm_infer_range_f32(*args, ws.data_ptr(), nbytes, ops._stream()))
+            return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
+
+        smp_key = None if dec.sampling is None else dec.sampling.graph_key()
+        inputs = (tc, dec.state) if dec.sampling is None else (tc, dec.state, dec.seed, dec.keys)
+        out = self._range_graphs().run(("plm_range", pl.serial, B, T, t0, t1, bool(return_logits), tc.stride(0),
+                                        tc.stride(1), ops.launch_policy_now(), smp_key), inputs, run)
+        dec.state[:, t0 + 1:t1 + 1].copy_(out[0])     # a replay advanced the graph's copy of the state, not dec.state
+        dec.t = t1
+        return (out[0], out[1]) if return_logits else out[0]
+
+    def _range_graphs(self):
+        g = self.__dict__.get("_range_graph_cache")
+        if g is None:
+            from .. import graphs
+            g = self.__dict__["_range_graph_cache"] = graphs.GraphedCall()
+        return g
+
+    def __getstate__(self):
+        d = super().__getstate__()
+        d.pop("_range_graph_cache", None)
+        return d
+
     def infer_causal(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None,
                      keys=None):
         """OPT-IN causal KV-cache greedy decode (SURVEY.md 8f-1) - NOT what the reference's ``infer`` computes.
@@ -228,6 +293,22 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         sd = {k[4:]: v for k, v in torch.load(ckpt, map_location="cpu")['state_dict'].items() if k.startswith('plm.')}
         plm.load_state_dict(sd, strict=True)
         return plm
+
+
+class PLMDecode:
+    """State of one resumable PLM decode (``MegaPLM.begin_decode``): the latent ``tc`` (B, T, tc_dim), the code state
+    (B, T+1) int64 (column 0 = BOS, column t+1 = the code of step t once decoded), the sampling parameters with the seed
+    and row keys as device tensors (None for greedy), and ``t``, the number of steps decoded."""
+
+    def __init__(self, tc, state, sampling, seed, keys):
+        self.tc, self.state, self.sampling, self.seed, self.keys = tc, state, sampling, seed, keys
+        self.B, self.T = tc.shape[0], tc.shape[1]
+        self.t = 0
+
+    @property
+    def codes(self):
+        """The codes decoded so far, (B, t) (a view of the state)."""
+        return self.state[:, 1:self.t + 1]
 
 
 class MegaADM(pack.PlanMixin, nn.Module):
@@ -423,6 +504,23 @@ class HifiganGenerator(pack.PlanMixin, nn.Module):
             self._plan = pl
         return self._plan
 
+    def receptive_field(self) -> int:
+        """Half-width in mel frames of what one output sample depends on, rounded up: conv_pre, then per stage the
+        transposed conv's reach and the widest ResBlock (two convs per dilation), and conv_post, each converted from
+        samples at that stage's rate to frames.  A window of mel frames vocoded on its own gives the whole sequence's
+        samples for the frames at least this far from each window edge that is not a sequence edge."""
+        from fractions import Fraction
+        c = self.cfg
+        r = Fraction((self.conv_pre.kernel_size[0] - 1) // 2)
+        rate = 1                                                  # samples per mel frame at the current stage
+        for u, k in zip(c["upsample_factors"], c["upsample_kernel_sizes"]):
+            r += Fraction(k - 1 - (k - u) // 2, u * rate)         # output j reads inputs down to (j + pad - k + 1) / u
+            rate *= u
+            r += Fraction(max(sum((rk - 1) // 2 * (d + 1) for d in dils)
+                              for rk, dils in zip(c["resblock_kernel_sizes"], c["resblock_dilation_sizes"])), rate)
+        r += Fraction((self.conv_post.kernel_size[0] - 1) // 2, rate)
+        return math.ceil(r)
+
     def out_len(self, T):
         n = T + 2 * self.cfg["inference_padding"]
         for u in self.cfg["upsample_factors"]:
@@ -525,6 +623,10 @@ class HIFIGAN(nn.Module):
 
     def decode_batch_cl(self, mel_cl: torch.Tensor) -> torch.Tensor:
         return self.generator.inference_cl(mel_cl)
+
+
+class _RangeRestart(Exception):
+    """An fp16 range flag raised before a stream yielded its first synthesized chunk."""
 
 
 class Megatts(nn.Module):
@@ -676,6 +778,134 @@ class Megatts(nn.Module):
             wav_lens = [n + pw.shape[-1] for n in wav_lens]
         return dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
                     mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
+
+    def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
+                          prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
+                          chunk_frames: int = 64, **unsupported):
+        """``synthesize`` as a generator of waveform chunks, each yielded as soon as the prosody LM has decoded the codes
+        its samples depend on.  Arguments as in ``synthesize``; ``chunk_frames`` mel frames (hop = 256 samples each) per
+        chunk.  Each chunk is a dict: ``wav`` (B, 1, n) device tensor, ``offset`` (its first sample's index in the waveform
+        ``synthesize`` returns), ``valid`` (per utterance, the samples of this chunk inside its waveform; the rest are
+        zeros), ``last``; the last chunk also has ``p_codes``, ``dt``, ``mel`` and ``wav_lens``.  With ``prompt_mels`` the
+        first chunk is the re-vocoded prompt.  The chunks, concatenated, are ``synthesize``'s waveform (same codes and
+        durations; samples within rounding: a window can take another tensor-core plan than the whole sequence).
+
+        The stream runs MRTE and the ADM, then alternates a PLM range (``MegaPLM.decode_until``), the mel rows that range
+        made computable (decoder windows with a halo of ``generator.decoder.receptive_field()`` frames) and the chunk's
+        vocoder window (halo ``hifi_gan.generator.receptive_field()``); megatts2_b200/stream.py has the schedule.  Ragged
+        totals: the utterances whose clipped windows are equal run as one batch.
+
+        ``check_range`` (fp16 operand engines): the range flag is read after every PLM range and every chunk, and nothing
+        is yielded before the first read.  Raised before the first synthesized chunk is yielded: the stream warns and
+        restarts on bf16x3, and then equals ``synthesize``'s rerun.  Raised later: it warns, recomputes the current step on
+        bf16x3 and finishes there, keeping the codes and chunks it has emitted - so such a stream can differ from
+        ``synthesize``, which reruns the whole batch.  ``causal_decode`` and ``overlap_prompt`` are not supported."""
+        if unsupported:
+            raise L.MttsError(f"synthesize_stream: unsupported argument(s) {sorted(unsupported)} "
+                              "(the causal decode and the overlapped prompt re-vocode are not streamed)")
+        if int(chunk_frames) < 1:
+            raise L.MttsError(f"synthesize_stream: chunk_frames must be >= 1, got {chunk_frames}")
+        guard = check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16)
+        return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
+                                  int(chunk_frames))
+
+    def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames):
+        try:
+            yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames)
+        except _RangeRestart:
+            import warnings
+            warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
+                          "restarting this stream on the bf16x3 engine")
+            yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, False, chunk_frames,
+                                    engine=pack.ENGINE_BF16X3)
+
+    def _stream(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames, engine=None):
+        # The engine scope is entered around each computing step only, never across a yield: the caller's own work between
+        # chunks keeps its engine.
+        from .. import stream as SCH
+        import contextlib
+
+        def scope():
+            return pack.engine_scope(engine) if engine is not None else contextlib.nullcontext()
+
+        dev = phone_tokens.device
+        gen, voc = self.generator, self.hifi_gan.generator
+        hop, pad = HIFIGAN_HOP_LENGTH, voc.cfg["inference_padding"]
+        hd, hv = gen.decoder.receptive_field(), voc.receptive_field()
+        with torch.no_grad(), scope():
+            tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
+            dt = self.adm.infer(tc_latent)[..., 0]
+            d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
+            tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
+            tc8 = ops.maxpool_time(tc_expand, 8)
+            dec = self.plm.begin_decode(tc8, sampling=sampling, keys=keys)
+            pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
+        B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], tc8.shape[1]
+        if Lmax < 1:
+            raise L.MttsError("synthesize_stream: every utterance has zero frames")
+        mel = torch.zeros(B, Lmax, gen.mrte.mel_bins, dtype=torch.float32, device=dev)
+        plans = [SCH.schedule(t, chunk_frames, hd, hv, pad, Lmax) for t in totals]
+        P = SCH.chunk_positions(Lmax, chunk_frames, pad)
+        K = len(P) - 1
+        off0 = 0 if pw is None else pw.shape[-1]
+        emitted = False
+
+        def flag_raised():
+            nonlocal guard, engine
+            if not guard or not ops.tc_overflow(dev):
+                return False
+            if not emitted:
+                raise _RangeRestart()
+            import warnings
+            warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; finishing this "
+                          "stream on the bf16x3 engine (its chunks can differ from synthesize's rerun)")
+            guard, engine = False, pack.ENGINE_BF16X3
+            return True
+
+        def groups(k, key):
+            """utterances with equal key(chunk) for chunk k -> [(key, index tensor or slice)]"""
+            by = {}
+            for i, pl in enumerate(plans):
+                c = pl[k]
+                if c is not None and key(c) is not None:
+                    by.setdefault(key(c), []).append(i)
+            return [(kk, slice(None) if len(ids) == B else torch.tensor(ids, device=dev)) for kk, ids in by.items()]
+
+        def synth_chunk(k):
+            n = hop * (P[k + 1] - P[k])
+            wav = torch.zeros(B, 1, n, dtype=torch.float32, device=dev)
+            for (rows, win), idx in groups(k, lambda c: (c.rows, c.dec) if c.dec is not None else None):
+                (r0, r1), (da, db) = rows, win
+                m = gen.decode_mel_cl(tc_expand[idx, da:db].contiguous(), dec.state[idx, 1 + da // 8:1 + -(-db // 8)])
+                mel[idx, r0:r1] = m[:, r0 - da:r1 - da]
+            for (p0, p1, va, vb), idx in groups(k, lambda c: (c.p0, c.p1) + c.voc):
+                w = self.hifi_gan.decode_batch_cl(mel[idx, va:vb])
+                wav[idx, :, :hop * (p1 - p0)] = w[:, :, hop * (p0 - va):hop * (p1 - va)]
+            return wav
+
+        for k in range(K):
+            t_need = T if k == K - 1 else max(pl[k].t1 for pl in plans if pl[k] is not None)
+            while True:
+                t_prev = dec.t
+                with torch.no_grad(), scope():
+                    self.plm.decode_until(dec, max(t_need, dec.t))
+                if not flag_raised():
+                    break
+                dec.t = t_prev                               # redo this range on bf16x3
+            while True:
+                with torch.no_grad(), scope():
+                    wav = synth_chunk(k)
+                if not flag_raised():
+                    break
+            if pw is not None and not emitted:
+                yield dict(wav=pw, offset=0, valid=[pw.shape[-1]] * B, last=False)
+            emitted = True
+            valid = [0 if pl[k] is None else hop * (pl[k].p1 - pl[k].p0) for pl in plans]
+            chunk = dict(wav=wav, offset=off0 + hop * P[k], valid=valid, last=k == K - 1)
+            if k == K - 1:
+                chunk.update(p_codes=dec.state[:, 1:].clone(), dt=dt, mel=mel,
+                             wav_lens=[hop * (t + 2 * pad) + off0 for t in totals])
+            yield chunk
 
     @torch.no_grad()
     def synthesize_many(self, items, max_batch: int = 64, sampling: S.Sampling = None, **kw):

@@ -118,6 +118,13 @@ class ConvNet(pack.PlanMixin, nn.Module):
             self._plan = pl
         return self._plan
 
+    def receptive_field(self) -> int:
+        """Half-width in frames of what one output frame depends on: first_layer, every ConvBlock and last_layer are
+        'same' convolutions of kernel k (20 for k = 5 with 4 x 2 blocks).  A window of frames run on its own gives the
+        whole sequence's outputs for the frames at least this far from each window edge that is not a sequence edge."""
+        _, _, _, k, ns, nb = self.cfg
+        return (k - 1) // 2 * (2 + ns * nb)
+
     def forward_cl(self, x_cl):
         """(B, T, Cin) -> (B, T, Cout)  (ConvNet.forward, convnet.py:115-119)."""
         if self.training:
