@@ -70,8 +70,8 @@ int mtts_tc_overflow_bind(int32_t* flag_dev);
  * size their grids from it, so work enqueued on two streams can share the device (the prompt re-vocode of Megatts.forward
  * runs beside the latency-bound AR loops). */
 int mtts_set_sm_limit(int32_t n_sms);
-/* Launch policy of the calling host thread while two streams share the device: SM budget (as above), allow_pairs (kept for
- * ABI compatibility: the sm_90 tap-GEMM launches single CTAs only), and whether launches carry the
+/* Launch policy of the calling host thread while two streams share the device: SM budget (as above), allow_pairs (0 keeps
+ * the tap-GEMM on single CTAs instead of 2-CTA clusters, which need two free SMs of one GPC), and whether launches carry the
  * programmatic-dependent-launch attribute (a long kernel's successor would otherwise be scheduled early onto the SMs left
  * free for the other stream).  (0, 1, 1) restores the defaults.  Megatts.synthesize uses it to re-vocode the prompt
  * (models/megatts2.py:371-372 of the reference) beside the MRTE + ADM stages. */
@@ -82,6 +82,11 @@ int mtts_set_launch_policy(int32_t sm_limit, int32_t allow_pairs, int32_t allow_
  * halo form (0 | 1), K-slab bytes}. */
 int mtts_tc_plan_query(int32_t n_sms, int32_t B, int32_t T, int32_t Cin, int32_t Cout, int32_t k, int32_t dil, int32_t fmt,
                        int64_t partial_bytes, int32_t ln_rides, int32_t* out5);
+/* As mtts_tc_plan_query, for a thread whose launch policy allows 2-CTA clusters (allow_pairs) or not.  out7 = out5, then
+ * CTAs per cluster (2: the CTAs of a cluster share the weight tile through TMA multicast; 1: single CTAs) and the CTAs of
+ * the grid (even when clustered; a clustered launch is further capped at the clusters the device can hold at once). */
+int mtts_tc_plan_query_ex(int32_t n_sms, int32_t B, int32_t T, int32_t Cin, int32_t Cout, int32_t k, int32_t dil,
+                          int32_t fmt, int64_t partial_bytes, int32_t ln_rides, int32_t allow_pairs, int32_t* out7);
 
 /* activation / padding codes */
 enum { MTTS_ACT_NONE = 0, MTTS_ACT_RELU = 1, MTTS_ACT_LEAKY = 2, MTTS_ACT_TANH = 3 };

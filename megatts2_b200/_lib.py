@@ -125,6 +125,7 @@ SIGNATURES = {
     "mtts_set_sm_limit": (C.c_int, [i32]),
     "mtts_set_launch_policy": (C.c_int, [i32, i32, i32]),
     "mtts_tc_plan_query": (C.c_int, [i32, i32, i32, i32, i32, i32, i32, i32, i64, i32, C.POINTER(i32)]),
+    "mtts_tc_plan_query_ex": (C.c_int, [i32, i32, i32, i32, i32, i32, i32, i32, i64, i32, i32, C.POINTER(i32)]),
     "mtts_set_attention_pair_min": (C.c_int, [i32]),
     "mtts_mask_tail_f32": (C.c_int, [vp, i32, i32, i32, vp, vp]),
     "mtts_resample_f32": (C.c_int, [vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, vp, i64, i32, vp, vp]),

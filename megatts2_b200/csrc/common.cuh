@@ -57,15 +57,27 @@ __device__ __forceinline__ void pdl_entry() {
 }
 bool pdl_enabled();
 void set_thread_pdl(bool on);
+// `cluster` > 1: thread-block clusters of that many CTAs along x (the grid's x extent must be a multiple of it)
 template <typename... KArgs, typename... Args>
-inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline void launch_kc(int cluster, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cudaLaunchAttribute at[2];
+  int n = 0;
+  if (pdl_enabled()) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cluster > 1) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n].val.clusterDim.x = (unsigned)cluster; at[n].val.clusterDim.y = 1; at[n++].val.clusterDim.z = 1;
+  }
+  cfg.attrs = at; cfg.numAttrs = n;
   cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);      // a failure is picked up by MTTS_CHECK_LAUNCH
+}
+template <typename... KArgs, typename... Args>
+inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  launch_kc(1, kern, grid, block, smem, st, static_cast<Args&&>(args)...);
 }
 
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }

@@ -18,6 +18,7 @@
 // slab, plane), no im2col, the k-fold re-reads are served by L2.  Weights are packed per tap as (k, Cout, Cin) bf16
 // planes (K-major B).  Variants: tile width BN 128 / 64 / 32, split-K with a fixed-order reduction kernel for
 // under-filled dense layers.  DESIGN.md section 4 has the anatomy.
+#include <algorithm>
 #include <mutex>
 #include <unordered_map>
 
@@ -60,6 +61,12 @@ struct ConvTcArgs {
 // its 128 rows plus the dil * (k - 1) halo rows - is loaded ONCE into a multi-buffered region and every tap reads it
 // through a row-shifted wgmma descriptor; only the (tiny) per-tap weight tiles stream through the stage ring.  The plain
 // form re-reads the tile once per tap (k-fold L2 -> SM traffic), which is what bounds the C = 32 / 64 HiFi-GAN stages.
+// CL = 2 (plain form, no K split): 2-CTA clusters share the weight tile.  A cluster walks pair items (row-tile pair, N tile);
+// rank 0 takes row tile 2p, rank 1 row tile 2p + 1 (past the last row tile: a dummy item on row tile 2p that runs the whole
+// barrier protocol and stores nothing).  Each CTA loads its own activation tile and half of the weight rows, multicast into
+// both CTAs at the same offset, so a stage moves NP * (A_PLANE + B_PLANE / 2) bytes from L2 into each SM instead of
+// NP * (A_PLANE + B_PLANE).  Either CTA's producer writes a stage slot of both, so a slot is refilled only once the owning
+// warpgroups of BOTH CTAs have released it (each consumer warp arrives on the local and the peer's empty barrier).
 constexpr int CTC_HALO_ROWS = 192;     // rows of a halo tile buffer: 128 + dil * (k - 1) <= 192, a multiple of 8
 template <int BN, int SWB, int NP = 3, int HALO = 0>
 struct ConvTcCfg {
@@ -83,10 +90,11 @@ struct ConvTcCfg {
   static_assert(SMEM <= 227 * 1024 && STAGES_RAW >= 2, "shared-memory budget");
 };
 
-template <int BN, int SWB, int NP, int HALO>
+template <int BN, int SWB, int NP, int HALO, int CL>
 __global__ void __launch_bounds__(CTC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   using Cfg = ConvTcCfg<BN, SWB, NP, HALO>;
+  static_assert(CL == 1 || (CL == 2 && !HALO), "clusters run the plain form");
   pdl_trigger();                                           // the next kernel may be scheduled; it waits for this grid itself
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -101,7 +109,12 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   const int lane = threadIdx.x & 31;
   constexpr int ROWS = Cfg::ROWS, HALVES = Cfg::HALVES;
   const int num_t = (g.T + ROWS - 1) / ROWS, num_n = (g.Cout + BN - 1) / BN;
-  const int num_tiles = g.B * num_t * num_n * g.splits;      // work items: (tile, K split)
+  const int num_rt = g.B * num_t;                            // row tiles
+  const int splits = (HALO || CL == 2) ? 1 : g.splits;
+  // work items: (row tile, N tile, K split), N fastest; under CL = 2 (row-tile pair, N tile), walked by the cluster
+  const int num_tiles = CL == 2 ? (num_rt + 1) / 2 * num_n : num_rt * num_n * splits;
+  const int rank = CL == 2 ? (int)cluster_ctarank() : 0;
+  const int item0 = (int)blockIdx.x / CL, istride = (int)gridDim.x / CL;   // CL = 2: the cluster's index and count
   const int ncb = (g.Cin + Cfg::BK - 1) / Cfg::BK;
   const int num_k = g.k * ncb;
 
@@ -113,7 +126,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 4);          // one arrive per warp of the consumer warpgroup that owns the item
+      mbar_init(empty_bar + 8 * s, 4 * CL);     // one arrive per warp of the owning consumer warpgroup of each CTA
     }
     if constexpr (HALO) {
       for (int s = 0; s < Cfg::A_BUFS; ++s) {
@@ -123,20 +136,28 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  // CL = 2: the peer's barriers are initialised before any multicast or remote arrive reaches them.  The exits below meet in
+  // a second cluster barrier, so that no CTA leaves while its peer can still multicast into it or arrive on its barriers.
+  if constexpr (CL == 2) cluster_sync();
+  else __syncthreads();
   pdl_wait();        // everything above (barriers, descriptor prefetch) overlapped the previous kernel's tail
 
   if (warp >= 8) {
     // ================= TMA producer (warp 8 walks the loops, one elected lane issues) =================
     setmaxnreg_dec<CTC_PRODUCER_REGS>();
-    if (warp != 8) return;
+    if (warp != 8) {
+      if constexpr (CL == 2) cluster_sync();
+      return;
+    }
     const bool leader = elect_one();
     int stage = 0, phase = 0;
     [[maybe_unused]] int ait = 0;
-    for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
-      const int sp = item % g.splits, tile = item / g.splits;
-      const int kb0 = (int)((int64_t)sp * num_k / g.splits), kb1 = (int)((int64_t)(sp + 1) * num_k / g.splits);
-      const int nb = tile % num_n, r = tile / num_n;
+    for (int item = item0; item < num_tiles; item += istride) {
+      const int sp = item % splits, tile = item / splits;
+      const int kb0 = (int)((int64_t)sp * num_k / splits), kb1 = (int)((int64_t)(sp + 1) * num_k / splits);
+      const int nb = tile % num_n;
+      int r = tile / num_n;
+      if constexpr (CL == 2) r = min(2 * r + rank, num_rt - 1);     // a dummy item loads row tile 2p (valid rows)
       const int tb = r % num_t, b = r / num_t;
       const int trow = tb * ROWS + g.row0;     // the item's first (padded) input row
       if constexpr (HALO) {
@@ -172,13 +193,24 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
             mbar_expect_tx(fb, Cfg::STAGE);
 #pragma unroll
             for (int q = 0; q < NP; ++q) tma_load_3d(sa + q * Cfg::A_PLANE, &maps.a[q], fb, cb * Cfg::BK, trow + j * g.dil, b);
+            if constexpr (CL == 2) {
+              // weight rows [rank * BN / 2, (rank + 1) * BN / 2) of the tile into both CTAs (whole 8-row swizzle atoms);
+              // the peer's half completes the other BN / 2 rows' bytes on this CTA's full barrier
+              const uint32_t ho = (uint32_t)(rank * (BN / 2) * SWB);
 #pragma unroll
-            for (int q = 0; q < NP; ++q) tma_load_2d(sb + q * Cfg::B_PLANE, &maps.b[q], fb, cb * Cfg::BK, j * g.Cout + nb * BN);
+              for (int q = 0; q < NP; ++q)
+                tma_load_2d_mc(sb + q * Cfg::B_PLANE + ho, &maps.b[q], fb, cb * Cfg::BK, j * g.Cout + nb * BN + rank * (BN / 2),
+                               (uint16_t)0x3);
+            } else {
+#pragma unroll
+              for (int q = 0; q < NP; ++q) tma_load_2d(sb + q * Cfg::B_PLANE, &maps.b[q], fb, cb * Cfg::BK, j * g.Cout + nb * BN);
+            }
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
+    if constexpr (CL == 2) cluster_sync();
     return;
   }
 
@@ -189,7 +221,6 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   constexpr int NCOR = NP == 1 ? 1 : BN / 2;               // NP = 1: no correction accumulator
   const int wg = warp >> 2, w4 = warp & 3;
   const int chunk = lane & 3, rsub = lane >> 2;
-  const int splits = HALO ? 1 : g.splits;
   const int64_t out_shift = HALO ? (int64_t)0 : g.out_shift;
   const bool partial_out = splits > 1;          // raw partial sums; bias / activation / residual run in the reduction kernel
   const bool has_bias = g.bias != nullptr && !partial_out;
@@ -208,10 +239,20 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
   // Turns on the tensor pipe: warpgroup wg waits on barrier 1 + wg before it issues the MMAs of its item li (li > 0); the
   // other warpgroup arrives there once it has issued all MMAs of item li - 1.  Arrivals are made only for an item that
   // exists, so no barrier is left half-arrived when the CTA exits.
-  const int n_items = num_tiles > (int)blockIdx.x ? (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+  // The two CTAs of a cluster walk the same items, so their stages, phases and warpgroup turns match.
+  const int n_items = num_tiles > item0 ? (num_tiles - item0 + istride - 1) / istride : 0;
+  // release of a stage: CL = 2 on this CTA's empty barrier and the peer's, whose producer also writes this slot
+  auto release = [&](int s) {
+    if constexpr (CL == 2) {
+      mbar_arrive_cluster(empty_bar + 8 * s, 0);
+      mbar_arrive_cluster(empty_bar + 8 * s, 1);
+    } else {
+      mbar_arrive(empty_bar + 8 * s);
+    }
+  };
   int stage = 0, phase = 0;
   for (int li = 0; li < n_items; ++li) {
-    const int item = blockIdx.x + li * gridDim.x;
+    const int item = item0 + li * istride;
     const int sp = item % splits, tile = item / splits;
     const int kb0 = (int)((int64_t)sp * num_k / splits), kb1 = (int)((int64_t)(sp + 1) * num_k / splits);
     if ((li & 1) != wg) {                       // the other warpgroup's item: step over its stages of the ring
@@ -220,7 +261,13 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       stage = s % STAGES;
       continue;
     }
-    const int nb = tile % num_n, r = tile / num_n;
+    const int nb = tile % num_n;
+    int r = tile / num_n;
+    bool dummy = false;
+    if constexpr (CL == 2) {
+      r = 2 * r + rank;
+      dummy = r >= num_rt;
+    }
     const int tb = r % num_t, b = r / num_t;
     [[maybe_unused]] int ab = 0;
     if (li > 0) named_bar_sync(1 + wg, 256);
@@ -269,7 +316,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       }
       wgmma_commit();
       wgmma_wait<1>();                                         // the previous stage's MMAs have retired: release it
-      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + 8 * prev);
+      if (prev >= 0 && lane == 0) release(prev);
       prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
@@ -281,9 +328,10 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       if constexpr (NP > 1) wgmma_fence_regs(cor[hv]);
     }
     if (lane == 0) {
-      if (prev >= 0) mbar_arrive(empty_bar + 8 * prev);
+      if (prev >= 0) release(prev);
       if constexpr (HALO) mbar_arrive(aempty_bar + 8 * ab);     // the halo tile is free once this tile's MMAs have retired
     }
+    if (dummy) continue;
 
     // ---- epilogue of this warp's 16 rows of each 64-row half
 #pragma unroll
@@ -352,6 +400,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcMaps maps, const ConvTcArgs g) {
       }
     }
   }
+  if constexpr (CL == 2) cluster_sync();
 }
 
 // split-K reduction: sums the partial tiles in a FIXED order (bit-reproducible) and applies the tap-GEMM epilogue
@@ -554,9 +603,10 @@ static EncodeTiledFn g_enc = nullptr;
 static std::mutex g_ctc_mu;          // guards g_enc, the descriptor cache and the per-device table (not the launches)
 
 // per-device state: SM count, which kernel instantiations have had their shared-memory attribute raised (the attribute
-// is per device), and the caller-registered f16 range flag
+// is per device), how many 2-CTA clusters of each clustered instantiation can be resident at once, and the
+// caller-registered f16 range flag
 constexpr int MAX_DEV = 64;
-struct DevState { int sms = 0; uint32_t attr_done = 0; int32_t* ovf = nullptr; };
+struct DevState { int sms = 0; uint64_t attr_done = 0; int max_clusters[12] = {}; int32_t* ovf = nullptr; };
 static DevState g_dev[MAX_DEV];
 
 int cur_device() {
@@ -578,9 +628,11 @@ int set_sm_limit(int n) {
 //  * the budgets of the two streams add up to the device (a persistent grid sized for all SMs waits for the other stream's CTAs);
 //  * no programmatic dependent launch on the stream with the long kernels: its NEXT kernel's CTAs would be scheduled early onto
 //    the SMs left free for the other stream and sit there in griddepcontrol.wait until the current kernel has finished.
-// `allow_pairs` is kept in the ABI: the tap-GEMM launches single CTAs only (the sm_90 build has no CTA-pair kernels).
+// `allow_pairs` = 0 keeps the tap-GEMM on single CTAs: a 2-CTA cluster needs two free SMs of one GPC at once, which a
+// stream sharing the device with long persistent kernels of another may not find.
+static thread_local bool g_allow_pairs = true;
 int set_launch_policy(int sm_limit, int allow_pairs, int allow_pdl) {
-  (void)allow_pairs;
+  g_allow_pairs = allow_pairs != 0;
   g_sm_limit = sm_limit > 0 ? sm_limit : 0;
   set_thread_pdl(allow_pdl != 0);
   return 0;
@@ -597,11 +649,33 @@ int cur_device_sms() {
 }
 int tc_smem_attr(const void* kernel, int slot, int bytes) {
   const int dev = cur_device();
-  if (g_dev[dev].attr_done & (1u << slot)) return 0;
+  if (g_dev[dev].attr_done & (1ull << slot)) return 0;
   std::lock_guard<std::mutex> lk(g_ctc_mu);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "conv_tc", (long long)e);
-  g_dev[dev].attr_done |= (1u << slot);
+  g_dev[dev].attr_done |= (1ull << slot);
+  return 0;
+}
+// 2-CTA clusters of a clustered tap-GEMM instantiation (index idx < 12) that the device can hold at once; queried once per
+// device after the shared-memory attribute is set.  On H100 this may be fewer than SMs / 2: a cluster's CTAs share a GPC.
+static int tc_max_clusters(const void* kernel, int idx, int smem, int* out) {
+  int& mc = g_dev[cur_device()].max_clusters[idx];
+  *out = mc;
+  if (mc > 0) return 0;
+  std::lock_guard<std::mutex> lk(g_ctc_mu);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2); cfg.blockDim = dim3(CTC_THREADS); cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute at;
+  at.id = cudaLaunchAttributeClusterDimension;
+  at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+  cfg.attrs = &at; cfg.numAttrs = 1;
+  int n = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kernel, &cfg);
+  if (e != cudaSuccess || n < 1)
+    return fail(MTTS_ERR_CUDA, "%s: no 2-CTA cluster fits (cudaOccupancyMaxActiveClusters: error %lld, %lld clusters)",
+                "conv_tc", (long long)e, (long long)n);
+  mc = n;
+  *out = n;
   return 0;
 }
 int32_t* tc_ovf_ptr() { return g_dev[cur_device()].ovf; }
@@ -668,32 +742,37 @@ int cmap_get(const void* p, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t b0, 
   return 0;
 }
 
-template <int BN, int SWB, int NP, int HALO = 0>
-static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, cudaStream_t st) {
+// `ctas`: the plan's grid (TcPlan::ctas); a clustered launch is further capped at the clusters the device can hold at once
+template <int BN, int SWB, int NP, int HALO = 0, int CL = 1>
+static int conv_tc_launch(const ConvTcMaps& maps, const ConvTcArgs& a, int ctas, cudaStream_t st) {
   using Cfg = ConvTcCfg<BN, SWB, NP, HALO>;
   static_assert(SWB == 128 || BN == 32, "64-byte K-slabs run at BN = 32 only");
   // one bit per instantiation in the per-device table (the max-dynamic-shared-memory attribute is per device)
-  constexpr int slot = HALO ? 12 + (BN == 64 ? 0 : 1) + 2 * (3 - NP)
-                            : (BN == 128 ? 0 : BN == 64 ? 1 : SWB == 128 ? 2 : 3) + 4 * (3 - NP);
-  static_assert(slot < 24, "attribute slots (24-31: resblock_tc.cu)");
-  MTTS_TRY(tc_smem_attr((const void*)conv_tc_kernel<BN, SWB, NP, HALO>, slot, Cfg::SMEM));
-  const int sms = cur_device_sms();
-  const int64_t items = (int64_t)a.B * cdiv64(a.T, Cfg::ROWS) * cdiv64(a.Cout, BN) * a.splits;
-  const int grid = (int)(items < sms ? items : sms);
-  launch_k(conv_tc_kernel<BN, SWB, NP, HALO>, grid, CTC_THREADS, Cfg::SMEM, st, maps, a);
+  constexpr int plain = (BN == 128 ? 0 : BN == 64 ? 1 : SWB == 128 ? 2 : 3) + 4 * (3 - NP);
+  constexpr int slot = HALO ? 12 + (BN == 64 ? 0 : 1) + 2 * (3 - NP) : CL == 2 ? 32 + plain : plain;
+  static_assert(slot < 24 || slot >= 32, "attribute slots (24-31: resblock_tc.cu)");
+  const void* kern = (const void*)conv_tc_kernel<BN, SWB, NP, HALO, CL>;
+  MTTS_TRY(tc_smem_attr(kern, slot, Cfg::SMEM));
+  int grid = ctas;
+  if constexpr (CL == 2) {
+    int mc = 0;
+    MTTS_TRY(tc_max_clusters(kern, plain, Cfg::SMEM, &mc));
+    if (grid > 2 * mc) grid = 2 * mc;
+  }
+  launch_kc(CL, conv_tc_kernel<BN, SWB, NP, HALO, CL>, grid, CTC_THREADS, Cfg::SMEM, st, maps, a);
   MTTS_CHECK_LAUNCH();
   return 0;
 }
 
-template <int NP>
-static int conv_tc_dispatch(const ConvTcMaps& maps, const ConvTcArgs& a, int BN, int SWB, cudaStream_t st) {
+template <int NP, int CL>
+static int conv_tc_dispatch(const ConvTcMaps& maps, const ConvTcArgs& a, int BN, int SWB, int ctas, cudaStream_t st) {
   if (SWB == 64) {
     MTTS_REQUIRE(BN == 32 && a.splits == 1, "a plan with 64-byte K-slabs runs at BN = 32 without a K split");
-    return conv_tc_launch<32, 64, NP>(maps, a, st);
+    return conv_tc_launch<32, 64, NP, 0, CL>(maps, a, ctas, st);
   }
-  if (BN == 128) return conv_tc_launch<128, 128, NP>(maps, a, st);
-  if (BN == 64) return conv_tc_launch<64, 128, NP>(maps, a, st);
-  return conv_tc_launch<32, 128, NP>(maps, a, st);
+  if (BN == 128) return conv_tc_launch<128, 128, NP, 0, CL>(maps, a, ctas, st);
+  if (BN == 64) return conv_tc_launch<64, 128, NP, 0, CL>(maps, a, ctas, st);
+  return conv_tc_launch<32, 128, NP, 0, CL>(maps, a, ctas, st);
 }
 
 bool conv_tc_eligible(const mtts_conv_params& p) {
@@ -734,11 +813,12 @@ constexpr int CTC_SPLITK_MAX = 8;
 constexpr double CTC_SPLITK_MARGIN = 0.85;
 constexpr double CTC_SPLITK_LN_RED = 2000.0;
 
-// The launch plan of one tap-GEMM: K-slab width, N-tile width, K splits, halo form.  A pure function of the shape, the SM
-// budget, the operand format, the partial-sum space and whether a LayerNorm rides on the reduction, so the policy can be
-// queried and tested without a GPU (mtts_tc_plan_query, tests/test_abi_and_host.py).
-struct TcPlan { int SWB, BN, splits; bool halo_form; };
-static TcPlan tc_plan(int sms, const mtts_conv_params& p, int np, bool ln_rides) {
+// The launch plan of one tap-GEMM: K-slab width, N-tile width, K splits, halo form, CTAs per cluster (1 | 2) and grid.  A
+// pure function of the shape, the SM budget, the operand format, the partial-sum space, whether a LayerNorm rides on the
+// reduction and whether clusters are allowed, so the policy can be queried and tested without a GPU (mtts_tc_plan_query_ex,
+// tests/test_abi_and_host.py, tests/test_gpu_tc_cluster.py).
+struct TcPlan { int SWB, BN, splits; bool halo_form; int cluster, ctas; };
+static TcPlan tc_plan(int sms, const mtts_conv_params& p, int np, bool ln_rides, bool pairs) {
   const int halo = p.dil * (p.k - 1);
   const int SWB = p.Cin >= 64 ? 128 : 64;
   int BN = 32;             // Cin < 64 (64-byte K-slabs): conv_tc_eligible admits Cout = 32 only
@@ -792,8 +872,20 @@ static TcPlan tc_plan(int sms, const mtts_conv_params& p, int np, bool ln_rides)
   const bool halo_form = splits == 1 && p.out_shift == 0 && p.k > 1 && p.Cin <= SWB / 2 &&
                          halo + 128 <= CTC_HALO_ROWS &&   // (the halo kernel's epilogue has no K-split / transposed-conv paths)
                          ((SWB == 64 && BN == 32) || (SWB == 128 && BN == 64)) && p.Cout == BN;
+  // 2-CTA clusters sharing the weight tile: the plain form without a K split, at least one row-tile pair and two SMs.
+  // Split launches (the early, latency-bound AR steps) and the halo form (its weight tiles are small) stay single CTAs.
+  const int64_t row_tiles = (int64_t)p.B * cdiv64(p.Tout, (BN == 128 && !halo_form) ? 64 : 128);
+  const int64_t n_tiles = cdiv64(p.Cout, BN);
+  const int cluster = (pairs && !halo_form && splits == 1 && row_tiles >= 2 && sms >= 2) ? 2 : 1;
+  int64_t ctas;
+  if (cluster == 2) {
+    const int64_t pair_items = cdiv64(row_tiles, 2) * n_tiles;
+    ctas = 2 * std::min<int64_t>(pair_items, sms / 2);          // an odd SM budget leaves one SM unused
+  } else {
+    ctas = std::min<int64_t>(row_tiles * n_tiles * splits, sms);
+  }
   TcPlan pl;
-  pl.SWB = SWB; pl.BN = BN; pl.splits = splits; pl.halo_form = halo_form;
+  pl.SWB = SWB; pl.BN = BN; pl.splits = splits; pl.halo_form = halo_form; pl.cluster = cluster; pl.ctas = (int)ctas;
   return pl;
 }
 
@@ -827,8 +919,8 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   }
   // the reduction of a split launch can carry the LayerNorm the caller asked for when a row is 3 / 4 / 6 / 8 x 128 wide
   const bool ln_rides = ln && ln->po.p && p.y && !p.tc_out_planes && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384);
-  const TcPlan pl = tc_plan(sms, p, np, ln_rides);
-  const int SWB = pl.SWB, BN = pl.BN, splits = pl.splits;
+  const TcPlan pl = tc_plan(sms, p, np, ln_rides, g_allow_pairs);
+  const int SWB = pl.SWB, BN = pl.BN, splits = pl.splits, ctas = pl.ctas;
   const bool halo_form = pl.halo_form;
   // activation box: the work item's rows (ConvTcCfg::ROWS: 64 at BN = 128, else 128), the halo form adds the halo rows
   const int a_rows = halo_form ? 128 + halo : (BN == 128 ? 64 : 128);
@@ -836,8 +928,9 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   for (int q = 0; q < np; ++q) {
     MTTS_TRY(cmap_get(planes + q * plane_stride, (uint64_t)p.Cin, (uint64_t)Tp_map, (uint64_t)p.B, SWB / 2,
                       a_rows, SWB, fmt, &maps.a[q]));
+    // weight box: the N tile, or the half of it that each CTA of a 2-CTA cluster loads
     MTTS_TRY(cmap_get((const __nv_bfloat16*)p.w_tc + (int64_t)q * p.k * p.Cout * p.Cin, (uint64_t)p.Cin,
-                      (uint64_t)p.k * p.Cout, 0, SWB / 2, BN, SWB, fmt, &maps.b[q]));
+                      (uint64_t)p.k * p.Cout, 0, SWB / 2, BN / pl.cluster, SWB, fmt, &maps.b[q]));
   }
   for (int q = np; q < 3; ++q) { maps.a[q] = maps.a[np - 1]; maps.b[q] = maps.b[np - 1]; }   // unused
   ConvTcArgs a;
@@ -852,16 +945,16 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
   a.fmt = fmt; a.ovf = ovf; a.row0 = p.tc_in_row0;
   if (halo_form) {
     if (SWB == 64)
-      return np == 1 ? conv_tc_launch<32, 64, 1, 1>(maps, a, st)
-           : np == 2 ? conv_tc_launch<32, 64, 2, 1>(maps, a, st) : conv_tc_launch<32, 64, 3, 1>(maps, a, st);
-    return np == 1 ? conv_tc_launch<64, 128, 1, 1>(maps, a, st)
-         : np == 2 ? conv_tc_launch<64, 128, 2, 1>(maps, a, st) : conv_tc_launch<64, 128, 3, 1>(maps, a, st);
+      return np == 1 ? conv_tc_launch<32, 64, 1, 1>(maps, a, ctas, st)
+           : np == 2 ? conv_tc_launch<32, 64, 2, 1>(maps, a, ctas, st) : conv_tc_launch<32, 64, 3, 1>(maps, a, ctas, st);
+    return np == 1 ? conv_tc_launch<64, 128, 1, 1>(maps, a, ctas, st)
+         : np == 2 ? conv_tc_launch<64, 128, 2, 1>(maps, a, ctas, st) : conv_tc_launch<64, 128, 3, 1>(maps, a, ctas, st);
   }
   if (splits > 1) {
     // a split launch runs at BN = 128 on the plan's K-slab width: the kernel's stage size must match the boxes the
     // descriptors above were encoded with
-    MTTS_TRY(np == 1 ? conv_tc_dispatch<1>(maps, a, 128, SWB, st)
-           : np == 2 ? conv_tc_dispatch<2>(maps, a, 128, SWB, st) : conv_tc_dispatch<3>(maps, a, 128, SWB, st));
+    MTTS_TRY((np == 1 ? conv_tc_dispatch<1, 1>(maps, a, 128, SWB, ctas, st)
+            : np == 2 ? conv_tc_dispatch<2, 1>(maps, a, 128, SWB, ctas, st) : conv_tc_dispatch<3, 1>(maps, a, 128, SWB, ctas, st)));
     // the rows' LayerNorm rides on the reduction when the caller asked for it and a row is 3 / 4 / 6 / 8 x 128 wide
     if (ln_fuse() && ln && ln->po.p && a.y && !a.op && a.out_shift == 0 && (p.Cout == 1024 || p.Cout == 768 || p.Cout == 512 || p.Cout == 384) &&
         p.ldy % 4 == 0 && ln->po.ld % 4 == 0 && ln->po.stride % 4 == 0) {
@@ -879,14 +972,19 @@ int conv_tc(const mtts_conv_params& p, cudaStream_t st, LnFuse* ln) {
     MTTS_CHECK_LAUNCH();
     return 0;
   }
-  return np == 1 ? conv_tc_dispatch<1>(maps, a, BN, SWB, st)
-       : np == 2 ? conv_tc_dispatch<2>(maps, a, BN, SWB, st) : conv_tc_dispatch<3>(maps, a, BN, SWB, st);
+  if (pl.cluster == 2)
+    return np == 1 ? conv_tc_dispatch<1, 2>(maps, a, BN, SWB, ctas, st)
+         : np == 2 ? conv_tc_dispatch<2, 2>(maps, a, BN, SWB, ctas, st) : conv_tc_dispatch<3, 2>(maps, a, BN, SWB, ctas, st);
+  return np == 1 ? conv_tc_dispatch<1, 1>(maps, a, BN, SWB, ctas, st)
+       : np == 2 ? conv_tc_dispatch<2, 1>(maps, a, BN, SWB, ctas, st) : conv_tc_dispatch<3, 1>(maps, a, BN, SWB, ctas, st);
 }
 
-// diagnostics: the plan conv_tc() would pick for a stride-1 tap-GEMM of this shape on `sms` SMs; out = {BN, splits, CTA pair
-// (always 0: no pair kernels on sm_90), halo form (0 | 1), K-slab bytes}
-int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides, int32_t* out5) {
-  MTTS_REQUIRE(out5 && sms > 0 && B > 0 && T > 0 && Cin > 0 && Cout > 0 && k > 0 && dil > 0, "bad arguments");
+// diagnostics: the plan conv_tc() would pick for a stride-1 tap-GEMM of this shape on `sms` SMs; out7 = {BN, splits, CTA
+// pair (always 0: no CTA-pair MMA kernels on sm_90), halo form (0 | 1), K-slab bytes, CTAs per cluster (1 | 2), CTAs of the
+// grid (before a clustered launch is capped at the clusters the device can hold)}
+int tc_plan_query_ex(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides,
+                     int allow_pairs, int32_t* out7) {
+  MTTS_REQUIRE(out7 && sms > 0 && B > 0 && T > 0 && Cin > 0 && Cout > 0 && k > 0 && dil > 0, "bad arguments");
   MTTS_REQUIRE(fmt == MTTS_TC_BF16X3 || fmt == MTTS_TC_F16X2 || fmt == MTTS_TC_F16, "unknown operand format");
   mtts_conv_params p;
   memset(&p, 0, sizeof(p));
@@ -894,8 +992,17 @@ int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int 
   static float dummy;
   p.y = &dummy;
   if (partial_bytes > 0) { p.tc_partial = &dummy; p.tc_partial_bytes = partial_bytes; }
-  const TcPlan pl = tc_plan(sms, p, 3 - fmt, ln_rides != 0);
-  out5[0] = pl.BN; out5[1] = pl.splits; out5[2] = 0; out5[3] = pl.halo_form ? 1 : 0; out5[4] = pl.SWB;
+  const TcPlan pl = tc_plan(sms, p, 3 - fmt, ln_rides != 0, allow_pairs != 0);
+  out7[0] = pl.BN; out7[1] = pl.splits; out7[2] = 0; out7[3] = pl.halo_form ? 1 : 0; out7[4] = pl.SWB;
+  out7[5] = pl.cluster; out7[6] = pl.ctas;
+  return 0;
+}
+// the first five fields of tc_plan_query_ex with clusters allowed
+int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides, int32_t* out5) {
+  MTTS_REQUIRE(out5, "bad arguments");
+  int32_t out7[7];
+  MTTS_TRY(tc_plan_query_ex(sms, B, T, Cin, Cout, k, dil, fmt, partial_bytes, ln_rides, 1, out7));
+  memcpy(out5, out7, 5 * sizeof(int32_t));
   return 0;
 }
 

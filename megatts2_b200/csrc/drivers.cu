@@ -931,6 +931,10 @@ int mtts_tc_plan_query(int32_t n_sms, int32_t B, int32_t T, int32_t Cin, int32_t
                        int64_t partial_bytes, int32_t ln_rides, int32_t* out5) {
   return tc_plan_query(n_sms, B, T, Cin, Cout, k, dil, fmt, partial_bytes, ln_rides, out5);
 }
+int mtts_tc_plan_query_ex(int32_t n_sms, int32_t B, int32_t T, int32_t Cin, int32_t Cout, int32_t k, int32_t dil, int32_t fmt,
+                          int64_t partial_bytes, int32_t ln_rides, int32_t allow_pairs, int32_t* out7) {
+  return tc_plan_query_ex(n_sms, B, T, Cin, Cout, k, dil, fmt, partial_bytes, ln_rides, allow_pairs, out7);
+}
 
 int64_t mtts_plm_infer_workspace_bytes(const mtts_plm* m, int32_t B, int32_t T) { return plm_ws_floats(m, B, T) * 4 + 8192; }
 int mtts_plm_infer_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,

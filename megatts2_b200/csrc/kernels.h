@@ -88,6 +88,8 @@ int cur_device_sms();
 int set_sm_limit(int n);
 int set_launch_policy(int sm_limit, int allow_pairs, int allow_pdl);
 int tc_plan_query(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides, int32_t* out5);
+int tc_plan_query_ex(int sms, int B, int T, int Cin, int Cout, int k, int dil, int fmt, int64_t partial_bytes, int ln_rides,
+                     int allow_pairs, int32_t* out7);
 // engine 1 | 2 | 3 (bf16x3 | f16x2 | f16) -> operand format; the one place that maps engines to formats
 static inline int tc_fmt_of_engine(int engine) {
   return engine == 3 ? MTTS_TC_F16 : engine == 2 ? MTTS_TC_F16X2 : MTTS_TC_BF16X3;

@@ -45,6 +45,40 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// the 2-D load multicast to the CTAs of `mask` in the cluster: the box lands at the same shared-memory offset in each of
+// them and completes bytes on the mbarrier at the same offset in each
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
+
+// ---- thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster: writes (barrier inits, remote arrives) before it are visible after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at shared-memory offset `bar` of CTA `rank` of the cluster (this CTA's own included).  The arrive
+// keeps the default .release.cta semantics: it releases a stage whose reads (wgmma, completed by wgmma.wait_group) are
+// done, and orders no memory traffic of this thread for the peer.  A .release.cluster arrive compiles to MEMBAR.ALL.GPU,
+// which waits for the thread's outstanding global stores, in the MMA-issuing warps once per stage: it made the clustered
+// kernel two to three times slower on H100.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t"
+      ".reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
+      "}" ::"r"(bar), "r"(rank)
+      : "memory");
+}
+
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(

@@ -423,9 +423,9 @@ def launch_policy_now():
 
 class launch_policy:
     """``with ops.launch_policy(sm_limit, pairs=..., pdl=...)``: the enclosed enqueues of this thread size their persistent
-    grids for ``sm_limit`` SMs, optionally without programmatic dependent launch (``pairs`` is accepted and ignored:
-    no CTA-pair kernels on sm_90) (include/megatts2_b200.h,
-    mtts_set_launch_policy).  Restored on exit, also when the body raises."""
+    grids for ``sm_limit`` SMs, optionally without 2-CTA clusters on the tap-GEMM (``pairs=False``) or without
+    programmatic dependent launch (include/megatts2_b200.h, mtts_set_launch_policy).  Restored on exit, also when the
+    body raises."""
 
     def __init__(self, sm_limit, pairs=True, pdl=True):
         self.new = (int(sm_limit), int(bool(pairs)), int(bool(pdl)))

@@ -3,7 +3,8 @@
 For each shape runs the op `reps` times inside the library's event trace and reports the main kernel's
 time per launch (the activation split is traced separately) and its rate in fp32-equivalent TFLOP/s
 (2*M*N*K*k; the tensor pipe executes 6 | 3 | 1 16-bit MMAs per product under bf16x3 | f16x2 | f16, so the dense
-16-bit rate is that multiple of it).
+16-bit rate is that multiple of it), and the operand bytes the launch plan moves from L2 into the SMs (modelled from the
+plan, not measured) with their rate.
 """
 import ctypes as C
 import math
@@ -34,6 +35,26 @@ SHAPES = [
     dict(name="adm qkv  M4096 K768  N2304", B=1, T=4096, Cin=768, Cout=2304, k=1),
     dict(name="adm ff1  M4096 K768  N1024", B=1, T=4096, Cin=768, Cout=1024, k=1),
 ]
+
+
+def operand_bytes(s, fmt, sms):
+    """L2 -> SM operand bytes of one launch, modelled from the plan (mtts_tc_plan_query_ex): every CTA work item loads,
+    per K-slab, its activation tile and the weight tile (or, in a 2-CTA cluster, half of it; a dummy item included) of
+    each operand plane; the halo form loads the activation tile with its halo once per item.  Returns (bytes, plan)."""
+    k, dil = s["k"], s.get("dil", 1)
+    out = (C.c_int32 * 7)()
+    L.check(L.lib().mtts_tc_plan_query_ex(sms, s["B"], s["T"], s["Cin"], s["Cout"], k, dil, fmt, 0, 0,
+                                          ops.launch_policy_now()[1], out))
+    bn, splits, halo, swb, cl = out[0], out[1], out[3], out[4], out[5]
+    npl = 3 - fmt
+    rows = 128 if (halo or bn != 128) else 64
+    rt = s["B"] * -(-s["T"] // rows)
+    nt = -(-s["Cout"] // bn)
+    nk = k * -(-s["Cin"] // (swb // 2))
+    if halo:
+        return rt * nt * npl * ((128 + dil * (k - 1)) * swb + nk * bn * swb), out
+    cta_items = (2 * -(-rt // 2) if cl == 2 else rt) * nt
+    return cta_items * nk * npl * (rows * swb + bn * swb // cl), out
 
 
 def trace_ms(fn, reps):
@@ -75,8 +96,10 @@ def main():
         out = torch.empty(s["B"], s["T"], s["Cout"], device=DEV)
         flops = 2.0 * s["B"] * s["T"] * s["Cin"] * s["Cout"] * k
         ms = trace_ms(lambda: ops.conv1d(x, wp, b, out=out, w_tc=wt, k=k, dil=dil, pad=pad, pad_mode=1 if k > 1 else 0), reps)
+        nbytes, plan = operand_bytes(s, fmt, ops.sm_count(torch.device(DEV)))
         print(f"{s['name']:30s} {ms:8.3f} ms  {flops / ms / 1e9:7.1f} TFLOP/s per product "
-              f"({nm * flops / ms / 1e9:7.0f} dense 16-bit, {args.fmt})", flush=True)
+              f"({nm * flops / ms / 1e9:7.0f} dense 16-bit, {args.fmt})  L2->SM {nbytes / 1e9:6.2f} GB "
+              f"{nbytes / ms / 1e9:5.2f} TB/s  (BN {plan[0]}, cluster {plan[5]})", flush=True)
         del x, out
         torch.cuda.empty_cache()
 
