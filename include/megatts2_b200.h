@@ -465,6 +465,42 @@ int mtts_plm_infer_range_sample_f32(const mtts_plm* m, const float* tc_latent, i
                                     int64_t* codes_out, float* logits_out, const mtts_sampling* s,
                                     void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Prosody interpolation: the PLM decoded from a weighted mixture of K prompts' code distributions (Mega-TTS 2,
+ * arXiv 2307.07218).  Utterance b has K >= 1 sources; source k is a latent tc^(k)[b] (T, tc_dim), all with the same T, and
+ * b has a weight row w[b, 0..K) (fp32, every weight >= 0 and finite, row sum > 0; normalised on the device: w^ = w / sum).
+ * All K sources share one code history, BOS then c_0 .. c_{t-1}.  At step t:
+ *   1. each source runs the reference-faithful step (mtts_plm_infer_f32's non-causal full recompute) over its own latent
+ *      and the shared history -> logits z^(k);
+ *   2. l_i = log sum_k w^_k softmax(z^(k))_i, a log-sum-exp over the sources in fp32.  NaN and -inf have zero mass in
+ *      their source; a source with a +inf logit puts all its mass on its lowest +inf index; a source with no candidate
+ *      contributes nothing; without any candidate l is -inf everywhere (and the pick is 0);
+ *   3. if exactly one weight of the row is positive, l is that source's raw logits row, copied bit for bit (so a one-hot
+ *      row decodes exactly what mtts_plm_infer_f32 decodes from that source alone);
+ *   4. c_t is picked from l by the greedy argmax or, with `s`, by the sampler (mtts_sampling) keyed by (seed, keys[b], t),
+ *      and appended to the shared history.
+ * A weight row without a positive weight gives l = -inf.  K <= 8 and vq_bins <= 4096 (MTTS_ERR_UNSUPPORTED above). */
+
+/* l (B, V) into out (row stride ld_out) from logits rows (row stride ld): source k of utterance b is row k * B + b;
+ * weights (B, K) contiguous, device. */
+int mtts_mix_logprob_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t K, int32_t B, const float* weights,
+                              float* out, int64_t ld_out, void* stream);
+/* The mixed decode.  tc_latent is the (K*B, T, tc_dim) stack of the sources, row k*B + b = source k of utterance b (batch
+ * stride tc_sb, row stride tc_ld); weights (B, K) device; codes_out (B, T); logits_out optional, (K*B, T, vq_bins), the
+ * raw per-source logits; s NULL = greedy.  Each step runs the encoder and the predict layer once over the K*B rows.  The
+ * weights, the seed and the keys are read from device memory at every step, so a replayed CUDA graph picks up new values.
+ * With K = 1 the codes and logits equal mtts_plm_infer_f32 / mtts_plm_infer_sample_f32 bit for bit. */
+int64_t mtts_plm_infer_mix_workspace_bytes(const mtts_plm* m, int32_t K, int32_t B, int32_t T);
+int mtts_plm_infer_mix_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                           int32_t B, int32_t T, const float* weights, int64_t* codes_out, float* logits_out,
+                           const mtts_sampling* s, void* workspace, int64_t workspace_bytes, void* stream);
+/* Steps [t0, t1) of the mixed decode against the shared (B, T+1) code state, as mtts_plm_infer_range_f32: any split of
+ * [0, T) into consecutive ranges yields the codes and logits of one mtts_plm_infer_mix_f32 call.  Same workspace size. */
+int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                 int32_t B, int32_t T, const float* weights, int32_t t0, int32_t t1, int64_t* code_state,
+                                 int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                                 void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ConvNet family (modules/convnet.py).  One ConvBlock = ReLU -> Conv1d(C,C,k,same) -> LN(C). */
 typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv_block;   /* w packed (k,C,C); w_tc (3,k,C,C) bf16 or NULL */
 

@@ -178,6 +178,12 @@ SIGNATURES = {
     "mtts_plm_infer_range_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, vp, i64, vp]),
     "mtts_plm_infer_range_sample_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, i32, i32, vp, vp, vp,
                                                   C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_mix_logprob_rows_f32": (C.c_int, [vp, i64, i32, i32, i32, vp, vp, i64, vp]),
+    "mtts_plm_infer_mix_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32, i32]),
+    "mtts_plm_infer_mix_f32": (C.c_int, [C.POINTER(PLM), i32, vp, i64, i32, i32, i32, vp, vp, vp, C.POINTER(Sampling), vp,
+                                         i64, vp]),
+    "mtts_plm_infer_mix_range_f32": (C.c_int, [C.POINTER(PLM), i32, vp, i64, i32, i32, i32, vp, i32, i32, vp, vp, vp,
+                                               C.POINTER(Sampling), vp, i64, vp]),
     "mtts_convnet_workspace_bytes": (i64, [C.POINTER(ConvNet), i32, i32]),
     "mtts_convnet_forward_f32": (C.c_int, [C.POINTER(ConvNet), vp, i64, i32, vp, i64, i32, i32, i32, vp, i64, vp]),
     "mtts_convnet_double_out_len": (i32, [C.POINTER(ConvNetDouble), i32]),

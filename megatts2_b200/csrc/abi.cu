@@ -114,6 +114,11 @@ int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t row
   return sample_rows(logits, ld, V, rows, step, *s, out, ld_out, nullptr, 0, (cudaStream_t)stream);
 }
 
+int mtts_mix_logprob_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t K, int32_t B, const float* weights,
+                              float* out, int64_t ld_out, void* stream) {
+  return mix_logprob_rows(logits, ld, V, K, B, weights, out, ld_out, (cudaStream_t)stream);
+}
+
 int mtts_philox4x32_10_u32(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, void* stream) {
   return philox4x32_10_words(ctr, key, out, n, (cudaStream_t)stream);
 }

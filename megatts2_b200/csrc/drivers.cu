@@ -272,33 +272,41 @@ static int64_t plm_ws_floats(const mtts_plm* m, int B, int T) {
 // reads columns <= t and writes column t+1 only, so any split of [0, T) into ranges enqueues the same kernels on the same
 // data as one call.  smp == nullptr: greedy (argmax_rows); otherwise each step's codes are drawn by the opt-in sampler
 // (sample.cu), keyed by the step index t, so the split does not change the draws either.
+// Prosody mix (weights != nullptr): tc holds K sources stacked as K*B rows (row k*B + b = source k of utterance b), all
+// reading the shared (B, T+1) code state.  Each step runs the encoder and the predict layer once over the K*B rows, then
+// mix_logprob_rows turns each utterance's K logits rows and its row of the (B, K) weights into l (B, V), and the pick
+// reads l.  logits_out, when given, is (K*B, T, V): the raw per-source logits.  K = 1 without weights is the plain decode.
 static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int t0, int t1,
                            int64_t* state, int64_t* codes_out, float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
-                           const mtts_sampling* smp) {
+                           const mtts_sampling* smp, int K = 1, const float* weights = nullptr) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
   MTTS_REQUIRE(0 <= t0 && t0 <= t1 && t1 <= (T > 0 ? T : 0), "step range outside [0, T]");
+  MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
+  if (weights) MTTS_TRY(mix_logprob_check(V, K));
   if (B <= 0 || T <= 0 || t0 == t1) return 0;
+  const int R = K * B;                                       // latent rows: the K sources of the B utterances
   Arena top(ws, ws_bytes);
-  float* X = top.take<float>((int64_t)B * T * D);
-  float* xl = top.take<float>((int64_t)B * D);
-  float* logits = top.take<float>((int64_t)B * V);
-  int64_t* codes = top.take<int64_t>((int64_t)B * (T + 1));
-  TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, (int64_t)B * T), (int64_t)B * T, tc_fmt_of_engine(m->enc.engine)};
+  float* X = top.take<float>((int64_t)R * T * D);
+  float* xl = top.take<float>((int64_t)R * D);
+  float* logits = top.take<float>((int64_t)R * V);
+  int64_t* codes = top.take<int64_t>((int64_t)R * (T + 1));
+  TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, (int64_t)R * T), (int64_t)R * T, tc_fmt_of_engine(m->enc.engine)};
   if (tcs.bytes) tcs.p = top.take<char>(tcs.bytes);
+  float* mixed = weights ? top.take<float>((int64_t)B * V) : nullptr;
   const int64_t enc_off = align_up(top.off, 256);
-  if (enc_off + encoder_ws_floats(&m->enc, B, T) * 4 > ws_bytes)
+  if (enc_off + encoder_ws_floats(&m->enc, R, T) * 4 > ws_bytes)
     return fail(MTTS_ERR_WORKSPACE, "%s: workspace too small (need %lld bytes)", "plm_infer",
-                enc_off + encoder_ws_floats(&m->enc, B, T) * 4);
+                enc_off + encoder_ws_floats(&m->enc, R, T) * 4);
   if (state) codes = state;
   else MTTS_TRY(fill_i64(codes, T + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
   for (int t = t0; t < t1; ++t) {
     const int S = t + 1;
-    MTTS_TRY(plm_build_input(tc, tc_sb, tc_ld, m->tc_dim, codes, T + 1, m->pc_embedding, m->vq_dim, V + 2, m->pe,
-                             m->pe_alpha, B, S, X, st));
+    MTTS_TRY(plm_build_input(tc, tc_sb, tc_ld, m->tc_dim, codes, T + 1, B, m->pc_embedding, m->vq_dim, V + 2, m->pe,
+                             m->pe_alpha, R, S, X, st));
     Arena ar((char*)ws + enc_off, ws_bytes - enc_off);
-    MTTS_TRY(encoder_forward(&m->enc, X, xl, B, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
+    MTTS_TRY(encoder_forward(&m->enc, X, xl, R, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
     float* lg = logits_out ? logits_out + (int64_t)t * V : logits;
     const int64_t lg_sb = logits_out ? (int64_t)T * V : V;
     mtts_conv_params p;
@@ -306,11 +314,17 @@ static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, in
     p.x = xl; p.ldx = D; p.x_batch_stride = D;
     p.w = m->w_predict;
     p.y = lg; p.ldy = V; p.y_batch_stride = lg_sb;
-    p.B = B; p.Tin = 1; p.Tout = 1; p.Cin = D; p.Cout = V; p.k = 1; p.stride = 1; p.dil = 1; p.out_scale = 1.0f;
+    p.B = R; p.Tin = 1; p.Tout = 1; p.Cin = D; p.Cout = V; p.k = 1; p.stride = 1; p.dil = 1; p.out_scale = 1.0f;
     if (tcs.p) { p.tc_scratch = tcs.p; p.tc_scratch_bytes = tcs.bytes; }
     MTTS_TRY(conv1d(p, st));
-    if (smp) MTTS_TRY(sample_rows(lg, lg_sb, V, B, t, *smp, codes + (t + 1), T + 1, codes_out + t, T, st));
-    else MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
+    const float* pick_from = lg;
+    int64_t pick_ld = lg_sb;
+    if (weights) {
+      MTTS_TRY(mix_logprob_rows(lg, lg_sb, V, K, B, weights, mixed, V, st));
+      pick_from = mixed; pick_ld = V;
+    }
+    if (smp) MTTS_TRY(sample_rows(pick_from, pick_ld, V, B, t, *smp, codes + (t + 1), T + 1, codes_out + t, T, st));
+    else MTTS_TRY(argmax_rows(pick_from, pick_ld, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
   }
   return 0;
 }
@@ -318,6 +332,10 @@ static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, in
 static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
                      float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st, const mtts_sampling* smp = nullptr) {
   return plm_infer_steps(m, tc, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, ws, ws_bytes, st, smp);
+}
+
+static int64_t plm_mix_ws_bytes(const mtts_plm* m, int K, int B, int T) {
+  return plm_ws_floats(m, K * B, T) * 4 + ((int64_t)B * m->vq_bins + 64) * 4 + 8192;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -459,8 +477,8 @@ static int plm_decode_causal(const mtts_plm* m, const float* tc, int64_t tc_sb, 
   MTTS_TRY(fill_i64(codes, T + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
   for (int t = 0; t < T; ++t) {
     // row t of the input: cat(tc[:, t], emb[codes[:, t]]) + alpha * pe[t]   (megatts2.py:154-157)
-    MTTS_TRY(plm_build_input(tc + (int64_t)t * tc_ld, tc_sb, tc_ld, m->tc_dim, codes + t, T + 1, m->pc_embedding, m->vq_dim,
-                             V + 2, m->pe + (int64_t)t * D, m->pe_alpha, B, 1, cb.x, st));
+    MTTS_TRY(plm_build_input(tc + (int64_t)t * tc_ld, tc_sb, tc_ld, m->tc_dim, codes + t, T + 1, B, m->pc_embedding,
+                             m->vq_dim, V + 2, m->pe + (int64_t)t * D, m->pe_alpha, B, 1, cb.x, st));
     MTTS_TRY(causal_step(&m->enc, B, T, t, cb, st));
     float* lg = logits_out ? logits_out + (int64_t)t * V : logits;
     const int64_t lg_sb = logits_out ? (int64_t)T * V : V;
@@ -964,6 +982,27 @@ int mtts_plm_infer_range_sample_f32(const mtts_plm* m, const float* tc_latent, i
   MTTS_TRY(sampling_check(s, m->vq_bins));
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
                          workspace_bytes, (cudaStream_t)stream, s);
+}
+
+int64_t mtts_plm_infer_mix_workspace_bytes(const mtts_plm* m, int32_t K, int32_t B, int32_t T) {
+  return plm_mix_ws_bytes(m, K, B, T);
+}
+int mtts_plm_infer_mix_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                           int32_t T, const float* weights, int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                           void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && weights, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, K, weights);
+}
+int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                 int32_t B, int32_t T, const float* weights, int32_t t0, int32_t t1, int64_t* code_state,
+                                 int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
+                                 int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && weights && code_state, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, K, weights);
 }
 
 int64_t mtts_adm_infer_workspace_bytes(const mtts_adm* m, int32_t B, int32_t T) { return adm_ws_floats(m, B, T) * 4 + 8192; }

@@ -157,9 +157,10 @@ int mel_spectrogram(const float* wav, int64_t wav_sb, int B, int L, const int32_
                     const float* fb_w, const int32_t* fb_off, const int32_t* fb_start, int n_mels, float clamp_min,
                     float* out, int64_t out_sb, int64_t out_sm, int64_t out_sf, cudaStream_t st);
 // AR-loop helpers
+// latent row r reads code row r % B_codes (B_codes = B: one code row per latent row; fewer: sources sharing a history)
 int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const int64_t* codes, int codes_ld,
-                    const float* emb, int vq_dim, int vocab, const float* pe, float alpha, int B, int S, float* X,
-                    cudaStream_t st);
+                    int B_codes, const float* emb, int vq_dim, int vocab, const float* pe, float alpha, int B, int S,
+                    float* X, cudaStream_t st);
 int argmax_rows(const float* x, int64_t ldx, int V, int rows, int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb,
                 cudaStream_t st);
 // opt-in sampler (sample.cu): validates s against V, then draws one code per row (argmax_rows when temperature == 0 or
@@ -168,6 +169,11 @@ int sampling_check(const mtts_sampling* s, int V);
 int sample_rows(const float* x, int64_t ldx, int V, int rows, int step, const mtts_sampling& s, int64_t* out_a,
                 int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st);
 int philox4x32_10_words(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, cudaStream_t st);
+// prosody mix (sample.cu): l (B, V) from K source rows per utterance and (B, K) weights; mix_logprob_check validates
+// (V, K) before a driver enqueues anything
+int mix_logprob_check(int V, int K);
+int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const float* w, float* out, int64_t ldo,
+                     cudaStream_t st);
 int fill_i64(int64_t* p, int64_t stride, int n, int64_t v, cudaStream_t st);
 int fill_f32(float* p, int64_t stride, int n, float v, cudaStream_t st);
 int adm_build_input(const float* tc_emb, int64_t te_sb, int te_ld, int tc_emb_dim, const float* praw, int p_ld,

@@ -745,7 +745,7 @@ int mask_tail(float* x, int B, int rows, int L, const int32_t* keep, cudaStream_
 
 // PLM step input (models/megatts2.py:173-175): X[b,s,:] = cat(tc[b,s,:], emb[codes[b,s]]) + alpha*pe[s]
 __global__ void plm_build_input_kernel(const float* __restrict__ tc, int64_t tc_sb, int tc_ld, int tc_dim,
-                                       const int64_t* __restrict__ codes, int codes_ld,
+                                       const int64_t* __restrict__ codes, int codes_ld, int B_codes,
                                        const float* __restrict__ emb, int vq_dim, int vocab,
                                        const float* __restrict__ pe, float alpha, int S, float* __restrict__ X,
                                        int64_t total) {
@@ -761,7 +761,7 @@ __global__ void plm_build_input_kernel(const float* __restrict__ tc, int64_t tc_
   if (d < tc_dim) {
     v = tc[(int64_t)b * tc_sb + (int64_t)s * tc_ld + d];
   } else {
-    int64_t id = codes[(int64_t)b * codes_ld + s];
+    int64_t id = codes[(int64_t)(b % B_codes) * codes_ld + s];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     v = __ldg(emb + id * vq_dim + (d - tc_dim));
   }
@@ -769,11 +769,13 @@ __global__ void plm_build_input_kernel(const float* __restrict__ tc, int64_t tc_
 }
 
 int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const int64_t* codes, int codes_ld,
-                    const float* emb, int vq_dim, int vocab, const float* pe, float alpha, int B, int S, float* X,
-                    cudaStream_t st) {
+                    int B_codes, const float* emb, int vq_dim, int vocab, const float* pe, float alpha, int B, int S,
+                    float* X, cudaStream_t st) {
   const int64_t total = (int64_t)B * S * (tc_dim + vq_dim);
   if (total <= 0) return 0;
-  launch_k(plm_build_input_kernel, (unsigned)cdiv64(total, 256), 256, 0, st, tc, tc_sb, tc_ld, tc_dim, codes, codes_ld, emb, vq_dim, vocab, pe, alpha, S, X, total);
+  MTTS_REQUIRE(B_codes >= 1, "B_codes must be >= 1");
+  launch_k(plm_build_input_kernel, (unsigned)cdiv64(total, 256), 256, 0, st, tc, tc_sb, tc_ld, tc_dim, codes, codes_ld,
+           B_codes, emb, vq_dim, vocab, pe, alpha, S, X, total);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

@@ -12,6 +12,7 @@ namespace mtts {
 constexpr int SAMPLE_THREADS = 256;
 constexpr int SAMPLE_WARPS = SAMPLE_THREADS / 32;
 constexpr int SAMPLE_MAX_V = 4096;      // a filtered row is staged as 8-byte keys: at most 32 KB of shared memory
+constexpr int MIX_MAX_K = SAMPLE_WARPS; // the mix reduces one source per warp
 
 // Philox4x32-10 (Salmon et al., SC'11, with the Random123 / cuRAND constants)
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
@@ -185,6 +186,101 @@ sample_rows_kernel(const float* __restrict__ x, int64_t ldx, int V, int step, fl
   }
 }
 
+// (max, sum of exp(z - max)) of two parts of a row; (-inf, 0) is the empty part
+__device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os) {
+  if (om == -INFINITY) return;
+  if (m == -INFINITY) { m = om; s = os; return; }
+  if (om > m) { s = s * expf(m - om) + os; m = om; }
+  else s += os * expf(om - m);
+}
+
+// One CTA per utterance b: l_i = log sum_k w^_k softmax(z_k)_i over the K rows z_k = x[(k B + b) ldx ..] (the contract is
+// stated with mtts_mix_logprob_rows_f32 in include/megatts2_b200.h).  Warp k reduces source k's (max, sum of exps) and its
+// lowest +inf index with shuffles; then every thread combines the sources for its tokens as a log-sum-exp in fp32.  The
+// rows were just written by the predict layer and are read from L2: each lane issues MIX_CHUNK loads before it uses one,
+// so a row costs V / (32 MIX_CHUNK) load latencies instead of V / 32.
+constexpr int MIX_CHUNK = 16;
+__global__ void __launch_bounds__(SAMPLE_THREADS)
+mix_logprob_rows_kernel(const float* __restrict__ x, int64_t ldx, int V, int K, int B, const float* __restrict__ w,
+                        float* __restrict__ out, int64_t ldo) {
+  __shared__ float s_lw[MIX_MAX_K], s_m[MIX_MAX_K];          // log w^_k - log sum_k, max_k
+  __shared__ int s_inf[MIX_MAX_K], s_on[MIX_MAX_K];
+  pdl_entry();
+  const int b = blockIdx.x, lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+  const float* wr = w + (int64_t)b * K;
+  float wk[MIX_MAX_K];
+#pragma unroll
+  for (int k = 0; k < MIX_MAX_K; ++k) wk[k] = k < K ? wr[k] : 0.f;
+  float wsum = 0.f;
+  int npos = 0, kpos = 0;
+#pragma unroll
+  for (int k = 0; k < MIX_MAX_K; ++k)
+    if (wk[k] > 0.f) { wsum += wk[k]; ++npos; kpos = k; }
+  float* orow = out + (int64_t)b * ldo;
+  if (npos == 1) {                                           // one weighted source: its raw row, bit for bit
+    const float* z = x + ((int64_t)kpos * B + b) * ldx;
+#pragma unroll 4
+    for (int i = threadIdx.x; i < V; i += SAMPLE_THREADS) orow[i] = z[i];
+    return;
+  }
+  if (wp < K) {
+    const float* z = x + ((int64_t)wp * B + b) * ldx;
+    float m = -INFINITY, s = 0.f;
+    int inf_i = INT_MAX;
+    for (int i0 = lane; i0 < V; i0 += 32 * MIX_CHUNK) {
+      float v[MIX_CHUNK];
+#pragma unroll
+      for (int j = 0; j < MIX_CHUNK; ++j) v[j] = i0 + 32 * j < V ? z[i0 + 32 * j] : -INFINITY;
+      float cm = -INFINITY, cs = 0.f;
+#pragma unroll
+      for (int j = 0; j < MIX_CHUNK; ++j) {
+        if (v[j] == INFINITY) inf_i = min(inf_i, i0 + 32 * j);
+        else if (isfinite(v[j])) cm = fmaxf(cm, v[j]);
+      }
+      if (cm != -INFINITY) {
+#pragma unroll
+        for (int j = 0; j < MIX_CHUNK; ++j)
+          if (isfinite(v[j])) cs += expf(v[j] - cm);
+      }
+      lse_merge(m, s, cm, cs);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      lse_merge(m, s, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, s, o));
+      inf_i = min(inf_i, __shfl_xor_sync(0xffffffffu, inf_i, o));
+    }
+    if (lane == 0) {
+      const float v = wr[wp];
+      s_inf[wp] = inf_i;
+      s_m[wp] = m;
+      // NaN weights fail v > 0 and, like a source without a candidate, contribute nothing
+      s_on[wp] = v > 0.f && (inf_i != INT_MAX || m != -INFINITY);
+      s_lw[wp] = logf(v / wsum) - (inf_i != INT_MAX ? 0.f : logf(s));
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < V; i += SAMPLE_THREADS) {
+    float v[MIX_MAX_K];
+#pragma unroll
+    for (int k = 0; k < MIX_MAX_K; ++k) v[k] = k < K ? x[((int64_t)k * B + b) * ldx + i] : 0.f;
+    float m = -INFINITY, s = 0.f;
+#pragma unroll
+    for (int k = 0; k < MIX_MAX_K; ++k) {
+      if (k >= K || !s_on[k]) continue;
+      float t;
+      if (s_inf[k] != INT_MAX) {
+        if (i != s_inf[k]) continue;
+        t = s_lw[k];
+      } else {
+        if (!isfinite(v[k])) continue;                       // NaN or -inf: zero mass in its source
+        t = (v[k] - s_m[k]) + s_lw[k];
+      }
+      lse_merge(m, s, t, 1.f);
+    }
+    orow[i] = m == -INFINITY ? -INFINITY : m + logf(s);
+  }
+}
+
 __global__ void philox_kernel(const uint32_t* __restrict__ ctr, const uint32_t* __restrict__ key, uint32_t* __restrict__ out,
                               int64_t n) {
   pdl_entry();
@@ -221,6 +317,27 @@ int sample_rows(const float* x, int64_t ldx, int V, int rows, int step, const mt
   while (n_sort < V) n_sort <<= 1;
   launch_k(sample_rows_kernel, (unsigned)rows, SAMPLE_THREADS, filter ? (size_t)n_sort * 8 : 0, st, x, ldx, V, step,
            s.temperature, s.top_k, s.top_p, filter, n_sort, s.seed, s.keys, out_a, lda, out_b, ldb);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
+int mix_logprob_check(int V, int K) {
+  MTTS_REQUIRE(K >= 1, "K must be >= 1");
+  MTTS_REQUIRE(V >= 1, "V must be >= 1");
+  if (K > MIX_MAX_K)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: K = %lld sources is above the bound of %lld", "mix_logprob_rows", K, MIX_MAX_K);
+  if (V > SAMPLE_MAX_V)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: V = %lld is above the bound of %lld tokens", "mix_logprob_rows", V, SAMPLE_MAX_V);
+  return 0;
+}
+
+int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const float* w, float* out, int64_t ldo,
+                     cudaStream_t st) {
+  MTTS_TRY(mix_logprob_check(V, K));
+  MTTS_REQUIRE(ldx >= 0 && ldo >= 0, "ld must be >= 0");
+  if (B <= 0) return 0;
+  MTTS_REQUIRE(x && w && out, "null pointer");
+  launch_k(mix_logprob_rows_kernel, (unsigned)B, SAMPLE_THREADS, 0, st, x, ldx, V, K, B, w, out, ldo);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

@@ -191,57 +191,125 @@ class MegaPLM(pack.PlanMixin, nn.Module):
                                  (tc, sampling.seed_tensor(tc.device), keys), run)
         return (out[0], out[1]) if return_logits else out[0]
 
-    def begin_decode(self, tc_latent: torch.Tensor, sampling: S.Sampling = None, keys=None) -> "PLMDecode":
-        """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
-        any number of ranges gives ``infer``'s codes and logits (same ``sampling`` and ``keys``)."""
+    def _mix_sources(self, tc_latents, weights):
+        """K source latents, each (B, T, tc_dim), and their weights -> (the (K*B, T, tc_dim) stack, (B, K) device weights)."""
+        if isinstance(tc_latents, torch.Tensor) or not len(tc_latents):
+            raise L.MttsError("prosody mix: tc_latents must be a non-empty list of (B, T, tc_dim) tensors")
+        tcs = [ops._dev(t, name=f"tc_latents[{k}]") for k, t in enumerate(tc_latents)]
+        shape = tuple(tcs[0].shape)
+        if len(shape) != 3 or shape[2] != self.tc_latent_dim or any(tuple(t.shape) != shape for t in tcs):
+            raise L.MttsError(f"prosody mix: every source must be (B, T, {self.tc_latent_dim}) with the same B and T, got "
+                              f"{[tuple(t.shape) for t in tcs]}")
+        if any(t.device != tcs[0].device for t in tcs):
+            raise L.MttsError("prosody mix: the sources must be on one device")
+        w = S.mix_weights(weights, len(tcs), shape[0]).to(tcs[0].device)
+        return torch.cat(tcs, 0), w
+
+    def infer_mix(self, tc_latents, weights, return_logits: bool = False, sampling: S.Sampling = None, keys=None):
+        """Prosody interpolation (Mega-TTS 2): the ``infer`` decode of B utterances from a weighted mixture of K sources'
+        code distributions.  ``tc_latents``: K tensors (B, T, tc_dim), one per source (e.g. ``tc_latent`` from different
+        prosody prompts); ``weights``: (K,) or (B, K), >= 0, each row with a positive sum (normalised per utterance).  All
+        sources share one code history; step t picks c_t from l = log sum_k w^_k softmax(logits of source k), greedily or
+        by ``sampling`` / ``keys`` as in ``infer``; with exactly one positive weight in a row, l is that source's raw
+        logits row (include/megatts2_b200.h states the contract).  -> codes (B, T) int64 [, logits (K, B, T, vq_bins), the
+        raw per-source logits].  Replays as a CUDA graph whose inputs are the latents, the weights, the seed and the keys,
+        so new weight values need no new capture."""
         _eval_only(self)
-        tc = ops._dev(tc_latent, name="tc_latent")
-        if tc.stride(2) != 1:
-            tc = tc.contiguous()
-        B, T, _ = tc.shape
+        tc, w = self._mix_sources(tc_latents, weights)
+        K, (B, T, _) = len(tc_latents), tc_latents[0].shape
+        V = self.vq_bins
+        pl = self._plan_get(tc.device, T)
+        lib = L.lib()
+
+        def run(tc_, w_, *smp):
+            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
+            logits = torch.empty(K * B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
+            ws = ops.workspace(lib.mtts_plm_infer_mix_workspace_bytes(C.byref(pl.struct), K, B, T), tc_.device)
+            s = C.byref(sampling.struct(*smp)) if smp else None
+            L.check(lib.mtts_plm_infer_mix_f32(C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
+                                               w_.data_ptr(), codes.data_ptr(),
+                                               logits.data_ptr() if return_logits else None, s, ws.data_ptr(), ws.numel(),
+                                               ops._stream()))
+            return (codes, logits) if return_logits else (codes,)
+
+        inputs = (tc, w) if sampling is None else (tc, w, sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device))
+        out = self._graphs().run(("plm_mix", pl.serial, K, B, T, bool(return_logits), tc.stride(0), tc.stride(1),
+                                  ops.launch_policy_now(), None if sampling is None else sampling.graph_key()),
+                                 inputs, run)
+        return (out[0], out[1].view(K, B, T, V)) if return_logits else out[0]
+
+    def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None) -> "PLMDecode":
+        """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
+        any number of ranges gives ``infer``'s codes and logits (same ``sampling`` and ``keys``).  With ``weights``,
+        ``tc_latent`` is the list of K sources of ``infer_mix`` and the ranges give ``infer_mix``'s codes and logits."""
+        _eval_only(self)
+        K, w = 1, None
+        if weights is not None:
+            K = len(tc_latent)
+            tc, w = self._mix_sources(tc_latent, weights)
+        else:
+            tc = ops._dev(tc_latent, name="tc_latent")
+            if tc.stride(2) != 1:
+                tc = tc.contiguous()
+        B, T = tc.shape[0] // K, tc.shape[1]
         state = torch.full((B, T + 1), self.vq_bins, dtype=torch.int64, device=tc.device)   # column 0 = BOS
         if sampling is None:
-            return PLMDecode(tc, state, None, None, None)
-        return PLMDecode(tc, state, sampling, sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device))
+            return PLMDecode(tc, state, None, None, None, w)
+        return PLMDecode(tc, state, sampling, sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device), w)
 
     def decode_until(self, dec: "PLMDecode", t1: int, return_logits: bool = False):
         """Run steps [dec.t, t1) of the decode begun by ``begin_decode`` -> the new codes (B, t1 - dec.t) int64 [, their
         logits (B, t1 - dec.t, vq_bins)].  Each range replays as a CUDA graph keyed by (B, T, t0, t1), from a cache of its
         own (``_range_graphs``), so streaming never evicts ``infer``'s graphs; a captured range pins a private workspace of
-        ``mtts_plm_infer_workspace_bytes(B, T)`` bytes."""
+        ``mtts_plm_infer_workspace_bytes(B, T)`` bytes.  A mixed decode (``begin_decode(..., weights=...)``) returns the
+        logits as (K, B, t1 - dec.t, vq_bins) and replays with the weights as a graph input."""
         _eval_only(self)
         tc, B, T, t0 = dec.tc, dec.B, dec.T, dec.t
         t1 = int(t1)
         if not t0 <= t1 <= T:
             raise L.MttsError(f"decode_until: t1 = {t1} outside [{t0}, {T}]")
         V = self.vq_bins
+        K, mix = dec.K, dec.weights is not None
         if t1 == t0:
             codes = torch.empty(B, 0, dtype=torch.int64, device=tc.device)
-            return (codes, torch.empty(B, 0, V, device=tc.device)) if return_logits else codes
+            lg_shape = (K, B, 0, V) if mix else (B, 0, V)
+            return (codes, torch.empty(*lg_shape, device=tc.device)) if return_logits else codes
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
-        nbytes = lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T)
+        nbytes = (lib.mtts_plm_infer_mix_workspace_bytes(C.byref(pl.struct), K, B, T) if mix else
+                  lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T))
 
-        def run(tc_, state_, *smp):
+        def run(tc_, state_, *rest):
             codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
-            logits = torch.empty(B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
+            logits = torch.empty(K * B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
             ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=tc_.device)   # private: a captured range pins it
+            lg = logits.data_ptr() if return_logits else None
+            if mix:
+                w_, smp = rest[0], rest[1:]
+                s = C.byref(dec.sampling.struct(*smp)) if smp else None
+                L.check(lib.mtts_plm_infer_mix_range_f32(C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0),
+                                                         tc_.stride(1), B, T, w_.data_ptr(), t0, t1, state_.data_ptr(),
+                                                         codes.data_ptr(), lg, s, ws.data_ptr(), nbytes, ops._stream()))
+                return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
             args = (C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T, t0, t1, state_.data_ptr(),
-                    codes.data_ptr(), logits.data_ptr() if return_logits else None)
-            if smp:
-                s = dec.sampling.struct(*smp)
+                    codes.data_ptr(), lg)
+            if rest:
+                s = dec.sampling.struct(*rest)
                 L.check(lib.mtts_plm_infer_range_sample_f32(*args, C.byref(s), ws.data_ptr(), nbytes, ops._stream()))
             else:
                 L.check(lib.mtts_plm_infer_range_f32(*args, ws.data_ptr(), nbytes, ops._stream()))
             return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
 
         smp_key = None if dec.sampling is None else dec.sampling.graph_key()
-        inputs = (tc, dec.state) if dec.sampling is None else (tc, dec.state, dec.seed, dec.keys)
-        out = self._range_graphs().run(("plm_range", pl.serial, B, T, t0, t1, bool(return_logits), tc.stride(0),
-                                        tc.stride(1), ops.launch_policy_now(), smp_key), inputs, run)
+        inputs = (tc, dec.state) + ((dec.weights,) if mix else ()) + (() if dec.sampling is None else (dec.seed, dec.keys))
+        key = ("plm_range", pl.serial, B, T, t0, t1, bool(return_logits), tc.stride(0), tc.stride(1),
+               ops.launch_policy_now(), smp_key)
+        out = self._range_graphs().run(key + (("mix", K),) if mix else key, inputs, run)
         dec.state[:, t0 + 1:t1 + 1].copy_(out[0])     # a replay advanced the graph's copy of the state, not dec.state
         dec.t = t1
-        return (out[0], out[1]) if return_logits else out[0]
+        if not return_logits:
+            return out[0]
+        return (out[0], out[1].reshape(K, B, t1 - t0, V)) if mix else (out[0], out[1])
 
     def _range_graphs(self):
         g = self.__dict__.get("_range_graph_cache")
@@ -298,11 +366,14 @@ class MegaPLM(pack.PlanMixin, nn.Module):
 class PLMDecode:
     """State of one resumable PLM decode (``MegaPLM.begin_decode``): the latent ``tc`` (B, T, tc_dim), the code state
     (B, T+1) int64 (column 0 = BOS, column t+1 = the code of step t once decoded), the sampling parameters with the seed
-    and row keys as device tensors (None for greedy), and ``t``, the number of steps decoded."""
+    and row keys as device tensors (None for greedy), and ``t``, the number of steps decoded.  A mixed decode also holds
+    the (B, K) device ``weights``, and ``tc`` is then the (K*B, T, tc_dim) stack of its K sources."""
 
-    def __init__(self, tc, state, sampling, seed, keys):
+    def __init__(self, tc, state, sampling, seed, keys, weights=None):
         self.tc, self.state, self.sampling, self.seed, self.keys = tc, state, sampling, seed, keys
-        self.B, self.T = tc.shape[0], tc.shape[1]
+        self.weights = weights
+        self.K = 1 if weights is None else weights.shape[1]
+        self.B, self.T = state.shape[0], tc.shape[1]
         self.t = 0
 
     @property
@@ -654,7 +725,7 @@ class Megatts(nn.Module):
     def synthesize(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                    return_intermediates: bool = False, causal_decode: bool = False, prompt_mels: torch.Tensor = None,
                    return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None,
-                   sampling: S.Sampling = None, keys=None):
+                   sampling: S.Sampling = None, keys=None, prosody_mels=None, prosody_weights=None):
         """phone_tokens (B,Tp) int64, mels (B,Tm,80) prompt mel (frames-major) -> wav (B,1,256*(max sum d + 10)).
         Steps = models/megatts2.py:354-373; every utterance's result equals the reference's batch-1 run on it
         (utterances are independent; the only cross-utterance coupling would be the zero rows the LengthRegulator
@@ -680,17 +751,23 @@ class Megatts(nn.Module):
         pack.ENGINE_F16``) - is not guarded by it.
         ``sampling`` (opt-in, megatts2_b200.sampling.Sampling): the prosody codes are sampled instead of decoded greedily
         (``MegaPLM.infer``), utterance b keyed by ``keys[b]`` (default arange(B)); the ADM durations stay deterministic.
-        The bf16x3 rerun above draws with the same seed and keys."""
+        The bf16x3 rerun above draws with the same seed and keys.
+        ``prosody_mels`` (opt-in prosody interpolation): a list of (B, Tm_k, 80) prosody prompts, with ``prosody_weights``
+        (K,) or (B, K), K = 1 + len(prosody_mels); weight 0 belongs to ``mels``.  Each prompt gives a source latent
+        ``mrte.tc_latent(phone_tokens, prompt)``, length-regulated and max-pooled with the target's durations, and the
+        codes come from ``MegaPLM.infer_mix`` over the K sources.  The durations, the mel decoder and the vocoder keep
+        the target's (``mels``) latent, so the timbre stays the target's.  Not with ``causal_decode``."""
         dev = phone_tokens.device
-        out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt,
-                               sampling, keys)
+        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode)
+        args = (phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt, sampling, keys,
+                prosody_mels, prosody_weights)
+        out = self._synthesize(*args)
         if check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16) and ops.tc_overflow(dev):
             import warnings
             warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
                           "re-running this batch on the bf16x3 engine")
             with pack.engine_scope(pack.ENGINE_BF16X3):
-                out = self._synthesize(phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt,
-                                       sampling, keys)
+                out = self._synthesize(*args)
         if return_intermediates:
             return out
         return (out["wav"], out["wav_lens"]) if return_lengths else out["wav"]
@@ -705,8 +782,26 @@ class Megatts(nn.Module):
                 float(os.environ.get("MEGATTS2_REVOCODE_FRAC", str(REVOCODE_FRAC_DEFAULT))),
                 os.environ.get("MEGATTS2_REVOCODE_FROM", REVOCODE_FROM_DEFAULT))
 
+    def _check_prosody(self, phone_tokens, prosody_mels, prosody_weights, causal_decode):
+        if prosody_mels is None:
+            if prosody_weights is not None:
+                raise L.MttsError("prosody_weights without prosody_mels")
+            return
+        if causal_decode:
+            raise L.MttsError("prosody interpolation runs on the reference-faithful decode, not with causal_decode=True")
+        if isinstance(prosody_mels, torch.Tensor) or not len(prosody_mels):
+            raise L.MttsError("prosody_mels must be a non-empty list of (B, Tm, mel_bins) tensors")
+        if prosody_weights is None:
+            raise L.MttsError("prosody_mels needs prosody_weights: (K,) or (B, K), K = 1 + len(prosody_mels)")
+        B, nb = phone_tokens.shape[0], self.generator.mrte.mel_bins
+        for k, m in enumerate(prosody_mels):
+            ops._dev(m, name=f"prosody_mels[{k}]")
+            if m.dim() != 3 or m.shape[0] != B or m.shape[2] != nb or m.shape[1] < 1:
+                raise L.MttsError(f"prosody_mels[{k}]: expected ({B}, Tm, {nb}), got {tuple(m.shape)}")
+        S.mix_weights(prosody_weights, 1 + len(prosody_mels), B)
+
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
-                    sampling=None, keys=None):
+                    sampling=None, keys=None, prosody_mels=None, prosody_weights=None):
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -747,7 +842,11 @@ class Megatts(nn.Module):
         d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
         tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
         tc8 = ops.maxpool_time(tc_expand, 8)
-        p_codes = plm_decode(tc8) if sampling is None else plm_decode(tc8, sampling=sampling, keys=keys)
+        if prosody_mels is not None:
+            srcs = [tc8] + self._prosody_sources(phone_tokens, prosody_mels, d_used, tc_expand.shape[1])
+            p_codes = self.plm.infer_mix(srcs, prosody_weights, sampling=sampling, keys=keys)
+        else:
+            p_codes = plm_decode(tc8) if sampling is None else plm_decode(tc8, sampling=sampling, keys=keys)
         B, Lmax = tc_expand.shape[0], tc_expand.shape[1]
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]
@@ -779,9 +878,16 @@ class Megatts(nn.Module):
         return dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
                     mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
 
+    def _prosody_sources(self, phone_tokens, prosody_mels, d_used, Lmax):
+        """The PLM latent of each prosody prompt: MRTE on (phone_tokens, prompt), length-regulated with the target's
+        durations to Lmax frames, max-pooled by 8."""
+        mrte = self.generator.mrte
+        return [ops.maxpool_time(ops.length_regulate(mrte.tc_latent(phone_tokens, m), d_used, l_out=Lmax)[0], 8)
+                for m in prosody_mels]
+
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
-                          chunk_frames: int = 64, **unsupported):
+                          chunk_frames: int = 64, prosody_mels=None, prosody_weights=None, **unsupported):
         """``synthesize`` as a generator of waveform chunks, each yielded as soon as the prosody LM has decoded the codes
         its samples depend on.  Arguments as in ``synthesize``; ``chunk_frames`` mel frames (hop = 256 samples each) per
         chunk.  Each chunk is a dict: ``wav`` (B, 1, n) device tensor, ``offset`` (its first sample's index in the waveform
@@ -805,21 +911,25 @@ class Megatts(nn.Module):
                               "(the causal decode and the overlapped prompt re-vocode are not streamed)")
         if int(chunk_frames) < 1:
             raise L.MttsError(f"synthesize_stream: chunk_frames must be >= 1, got {chunk_frames}")
+        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False)
         guard = check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16)
         return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
-                                  int(chunk_frames))
+                                  int(chunk_frames), (prosody_mels, prosody_weights))
 
-    def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames):
+    def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
+                      prosody):
         try:
-            yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames)
+            yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
+                                    prosody)
         except _RangeRestart:
             import warnings
             warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
                           "restarting this stream on the bf16x3 engine")
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, False, chunk_frames,
-                                    engine=pack.ENGINE_BF16X3)
+                                    prosody, engine=pack.ENGINE_BF16X3)
 
-    def _stream(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames, engine=None):
+    def _stream(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames, prosody,
+                engine=None):
         # The engine scope is entered around each computing step only, never across a yield: the caller's own work between
         # chunks keeps its engine.
         from .. import stream as SCH
@@ -838,7 +948,12 @@ class Megatts(nn.Module):
             d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
             tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
             tc8 = ops.maxpool_time(tc_expand, 8)
-            dec = self.plm.begin_decode(tc8, sampling=sampling, keys=keys)
+            prosody_mels, prosody_weights = prosody
+            if prosody_mels is not None:
+                srcs = [tc8] + self._prosody_sources(phone_tokens, prosody_mels, d_used, tc_expand.shape[1])
+                dec = self.plm.begin_decode(srcs, sampling=sampling, keys=keys, weights=prosody_weights)
+            else:
+                dec = self.plm.begin_decode(tc8, sampling=sampling, keys=keys)
             pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
         B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], tc8.shape[1]
         if Lmax < 1:
@@ -913,7 +1028,10 @@ class Megatts(nn.Module):
         bucketed by (Tp, Tm) - the MRTE phone encoder and the prompt encoder are unmasked in the reference
         (modules/mrte.py:154-171), so padding either would change results - and each bucket runs as one batch.
         Returns a list of 1-D waveforms (valid samples only), in input order.  With ``sampling``, utterance i is keyed
-        by its index i in ``items``, so the bucketing and ``max_batch`` do not change what it draws."""
+        by its index i in ``items``, so the bucketing and ``max_batch`` do not change what it draws.  Prosody prompts
+        (``prosody_mels``) are not taken here: call ``synthesize`` per batch."""
+        if "prosody_mels" in kw or "prosody_weights" in kw:
+            raise L.MttsError("synthesize_many does not take prosody prompts; call synthesize per batch")
         if sampling is not None:
             kw["sampling"] = sampling
         buckets = {}

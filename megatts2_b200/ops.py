@@ -229,6 +229,23 @@ def sample_rows(logits, step, sampling, keys):
     return out
 
 
+def mix_logprob_rows(logits, weights):
+    """The prosody mix of one step: logits (K, B, V) fp32 (source k of utterance b) and weights (K,) or (B, K) ->
+    l (B, V), l = log sum_k w^_k softmax(logits[k, b]) (include/megatts2_b200.h, mtts_mix_logprob_rows_f32)."""
+    from . import sampling as S
+    logits = _dev(logits, name="logits")
+    if logits.dim() != 3:
+        raise L.MttsError(f"logits: expected (K, B, V), got shape {tuple(logits.shape)}")
+    K, B, V = logits.shape
+    x = logits.reshape(K * B, V)
+    if x.stride(1) != 1:
+        x = x.contiguous()
+    w = S.mix_weights(weights, K, B).to(logits.device)
+    out = torch.empty(B, V, dtype=_F32, device=logits.device)
+    L.check(L.lib().mtts_mix_logprob_rows_f32(_ptr(x), x.stride(0), V, K, B, _ptr(w), _ptr(out), V, _stream()))
+    return out
+
+
 def philox4x32_10(ctr, key):
     """The sampler's generator: ctr (n, 4) and key (n, 2) uint32 words, as int64 tensors holding values < 2**32, ->
     (n, 4) words (int64, values < 2**32)."""
