@@ -161,6 +161,20 @@ int mtts_linear_tc_f32(const float* x, int32_t ldx, int64_t M, int32_t K, const 
  * activations; the host side uses it to pack weights once).  C %% 4 == 0, x 16-byte aligned. */
 int mtts_split_planes_f32(const float* x, int32_t ldx, int64_t rows, int32_t C, void* planes, int32_t fmt, void* stream);
 
+/* One HiFi-GAN ResBlock1 dilation step in one launch (the C = 32 / 64 vocoder stages; x, y (B, T, C) contiguous):
+ *   y = (x + conv2(leaky(conv1_dil(leaky(x)) + b1)) + b2) * out_scale (+ y_old if accumulate)
+ * leaky slope 0.1, both convs "same" with reflect padding, conv1 at dilation `dil`, conv2 at dilation 1.  w1_tc / w2_tc are
+ * the (3 - fmt, k, C, C) operand planes of the (C, C, k) conv weights (the layout pack_conv_tc_planes writes); fmt is
+ * MTTS_TC_F16X2 or MTTS_TC_F16, and the fp16 range flag of mtts_tc_overflow_bind is raised when an element of leaky(x) or of
+ * leaky(conv1 + b1) at a position t in [0, T) is beyond 65504.  x and y must not alias; x, y, b1, b2 16-byte aligned.  MTTS_ERR_UNSUPPORTED outside
+ * mtts_resblock_step_eligible. */
+int mtts_resblock_step_f32(const float* x, float* y, const void* w1_tc, const float* b1, const void* w2_tc, const float* b2,
+                           int32_t B, int32_t T, int32_t C, int32_t k, int32_t dil, float out_scale, int32_t accumulate,
+                           int32_t fmt, void* stream);
+/* Host only (no CUDA call): 1 if mtts_resblock_step_f32 accepts the shape - fmt f16x2 | f16, C 32 | 64, odd k >= 3 with
+ * h2 = (k - 1) / 2 <= 31 and h1 = dil * h2 <= 32, T > h1 + h2, B * T >= 128 - else 0. */
+int mtts_resblock_step_eligible(int32_t B, int32_t T, int32_t C, int32_t k, int32_t dil, int32_t fmt);
+
 /* LayerNorm over the last dim (nn.LayerNorm, eps 1e-5; modules/convnet.py:28-30,
  * modules/transformer.py:67-68, modules/mrte.py:136):
  *   v = LN(x[row]) * gamma + beta;  v = post(v);  v += res[row];  v += y_old (accumulate) */

@@ -121,6 +121,8 @@ SIGNATURES = {
     "mtts_linear_tc_scratch_bytes": (i64, [i64, i32]),
     "mtts_linear_tc_f32": (C.c_int, [vp, i32, i64, i32, vp, i32, vp, vp, i32, vp, i32, i32, f32, i32, vp, i64, i64, i32, vp]),
     "mtts_split_planes_f32": (C.c_int, [vp, i32, i64, i32, vp, i32, vp]),
+    "mtts_resblock_step_f32": (C.c_int, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, i32, vp]),
+    "mtts_resblock_step_eligible": (C.c_int, [i32, i32, i32, i32, i32, i32]),
     "mtts_tc_overflow_bind": (C.c_int, [vp]),
     "mtts_set_sm_limit": (C.c_int, [i32]),
     "mtts_set_launch_policy": (C.c_int, [i32, i32, i32]),

@@ -92,6 +92,16 @@ int mtts_conv1d_f32(const mtts_conv_params* p, void* stream) {
   return conv1d(*p, (cudaStream_t)stream);
 }
 
+int mtts_resblock_step_f32(const float* x, float* y, const void* w1_tc, const float* b1, const void* w2_tc, const float* b2,
+                           int32_t B, int32_t T, int32_t C, int32_t k, int32_t dil, float out_scale, int32_t accumulate,
+                           int32_t fmt, void* stream) {
+  return resblock_pair_tc(x, y, w1_tc, b1, w2_tc, b2, B, T, C, k, dil, out_scale, accumulate, fmt, (cudaStream_t)stream);
+}
+
+int mtts_resblock_step_eligible(int32_t B, int32_t T, int32_t C, int32_t k, int32_t dil, int32_t fmt) {
+  return resblock_tc_eligible(B, T, C, k, dil, fmt) ? 1 : 0;
+}
+
 int mtts_layernorm_f32(const float* x, int32_t ldx, const float* gamma, const float* beta, const float* res, int32_t ldr,
                        float* y, int32_t ldy, int64_t rows, int32_t C, float eps, int32_t post_act, int32_t accumulate,
                        void* stream) {
