@@ -329,13 +329,9 @@ static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, in
   return 0;
 }
 
-static int plm_infer(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
-                     float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st, const mtts_sampling* smp = nullptr) {
-  return plm_infer_steps(m, tc, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, ws, ws_bytes, st, smp);
-}
-
-static int64_t plm_mix_ws_bytes(const mtts_plm* m, int K, int B, int T) {
-  return plm_ws_floats(m, K * B, T) * 4 + ((int64_t)B * m->vq_bins + 64) * 4 + 8192;
+// Workspace of a decode of K sources of B utterances, whole or any range of it; a mixed decode also holds the (B, V) mixture.
+static int64_t plm_infer_ws_bytes(const mtts_plm* m, int K, int B, int T, bool mix) {
+  return plm_ws_floats(m, K * B, T) * 4 + (mix ? ((int64_t)B * m->vq_bins + 64) * 4 : 0) + 8192;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -954,18 +950,20 @@ int mtts_tc_plan_query_ex(int32_t n_sms, int32_t B, int32_t T, int32_t Cin, int3
   return tc_plan_query_ex(n_sms, B, T, Cin, Cout, k, dil, fmt, partial_bytes, ln_rides, allow_pairs, out7);
 }
 
-int64_t mtts_plm_infer_workspace_bytes(const mtts_plm* m, int32_t B, int32_t T) { return plm_ws_floats(m, B, T) * 4 + 8192; }
+int64_t mtts_plm_infer_workspace_bytes(const mtts_plm* m, int32_t B, int32_t T) { return plm_infer_ws_bytes(m, 1, B, T, false); }
 int mtts_plm_infer_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
                        int64_t* codes_out, float* logits_out, void* workspace, int64_t workspace_bytes, void* stream) {
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
-  return plm_infer(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes, (cudaStream_t)stream);
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, nullptr);
 }
 int mtts_plm_infer_sample_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
                               int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
                               int64_t workspace_bytes, void* stream) {
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
   MTTS_TRY(sampling_check(s, m->vq_bins));
-  return plm_infer(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes, (cudaStream_t)stream, s);
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s);
 }
 int mtts_plm_infer_range_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
                              int32_t t0, int32_t t1, int64_t* code_state, int64_t* codes_out, float* logits_out,
@@ -985,7 +983,7 @@ int mtts_plm_infer_range_sample_f32(const mtts_plm* m, const float* tc_latent, i
 }
 
 int64_t mtts_plm_infer_mix_workspace_bytes(const mtts_plm* m, int32_t K, int32_t B, int32_t T) {
-  return plm_mix_ws_bytes(m, K, B, T);
+  return plm_infer_ws_bytes(m, K, B, T, true);
 }
 int mtts_plm_infer_mix_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
                            int32_t T, const float* weights, int64_t* codes_out, float* logits_out, const mtts_sampling* s,

@@ -34,6 +34,41 @@ def _eval_only(m):
                           "MegaADM (SURVEY.md 8f-4), the generator trainer's path (conv stacks, VQ EMA) is not built")
 
 
+def _dev_rows(t, name):
+    """A CUDA fp32 (B, T, C) input with unit channel stride: ``t`` itself, or a contiguous copy."""
+    t = ops._dev(t, name=name)
+    return t if t.stride(2) == 1 else t.contiguous()
+
+
+def _sampling_inputs(sampling, keys, rows, device):
+    """(sampling, seed, keys) of a sampled decode, with the seed and the row keys as device tensors; None when greedy."""
+    if sampling is None:
+        return None
+    return sampling, sampling.seed_tensor(device), S.row_keys(keys, rows, device)
+
+
+def _ar_plan(model, enc, pos, struct, device, T, fill):
+    """The weight plan of an AR model (MegaPLM / MegaADM), rebuilt when its weights or engine changed or when its
+    positional table has fewer than T rows: the encoder ``enc``, then ``fill(plan, s)`` for the model's own fields of the
+    ctypes ``struct``, then the table of ``pos`` with max(T, 4000) rows."""
+    sig = pack.signature(list(model.parameters())) + (getattr(enc, "engine", None), pack.default_engine())
+    if model._plan is None or model._plan.sig != sig or model._plan.pe_rows < T:
+        pl = pack.Plan()
+        pl.sig = sig
+        enc_pl = encoder_plan(enc, list(enc.layers))
+        pl.hold(enc_pl)
+        s = struct()
+        s.enc = enc_pl.enc
+        fill(pl, s)
+        pe = pos.table(device, max(T, 4000))
+        pl.pe_rows = pe.shape[0]
+        s.pe = pl.p(pe)
+        s.pe_alpha = pos.alpha_host()
+        pl.struct = s
+        model._plan = pl
+    return model._plan
+
+
 class MegaG(nn.Module):
     def __init__(self, mrte: MRTE, vqpe: VQProsodyEncoder, kernel_size: int = 5, activation: str = 'ReLU',
                  hidden_size: int = 512, decoder_n_stack: int = 4, decoder_n_block: int = 2):
@@ -102,24 +137,11 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         self._plan = None
 
     def _plan_get(self, device, T):
-        sig = pack.signature(list(self.parameters())) + (getattr(self.plm, "engine", None), pack.default_engine())
-        if self._plan is None or self._plan.sig != sig or self._plan.pe_rows < T:
-            pl = pack.Plan()
-            pl.sig = sig
-            enc_pl = encoder_plan(self.plm, list(self.plm.layers))
-            pl.hold(enc_pl)
-            s = L.PLM()
-            s.enc = enc_pl.enc
+        def fill(pl, s):
             s.pc_embedding = pl.p(self.pc_embedding.weight)
             s.w_predict = pl.p(pack.pack_linear(self.predict_layer.weight))
-            pe = self.pos.table(device, max(T, 4000))
-            pl.pe_rows = pe.shape[0]
-            s.pe = pl.p(pe)
-            s.pe_alpha = self.pos.alpha_host()
             s.vq_bins, s.vq_dim, s.tc_dim = self.vq_bins, self.vq_dim, self.tc_latent_dim
-            pl.struct = s
-            self._plan = pl
-        return self._plan
+        return _ar_plan(self, self.plm, self.pos, L.PLM, device, T, fill)
 
     def forward(self, tc_latent: torch.Tensor, p_codes: torch.Tensor, lens: torch.Tensor):
         """Teacher-forced logits with the causal + padding mask (models/megatts2.py:148-163).  In training mode the
@@ -147,49 +169,60 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         argmax, row b keyed by ``keys[b]`` (B 64-bit integers, default arange(B)); the returned logits stay the raw ones.
         The seed and the keys are inputs of the replayed CUDA graph, so a new seed needs no new capture."""
         _eval_only(self)
-        tc = ops._dev(tc_latent, name="tc_latent")
-        if tc.stride(2) != 1:
-            tc = tc.contiguous()
+        tc = _dev_rows(tc_latent, "tc_latent")
         B, T, _ = tc.shape
+        return self._decode(tc, 1, None, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits)
+
+    def _decode(self, tc, K, weights, smp, t0, t1, state, return_logits):
+        """Steps [t0, t1) of the decode of B utterances from ``tc``, the (K*B, T, tc_dim) stack of K sources mixed by the
+        (B, K) device ``weights`` (None: K = 1, the plain decode).  ``smp``: (sampling, seed, keys), or None for greedy.
+        ``state`` None: the whole decode (t0 = 0, t1 = T) on the shared workspace; otherwise a range against that (B, T+1)
+        code state, on a private workspace since a captured range pins it.  The enqueues are device-only, so the call
+        replays as a CUDA graph from the second time on; ranges keep their graphs in a cache of their own, so streaming
+        never evicts the whole decodes'.  -> codes (B, t1 - t0) int64 [, logits (B, t1 - t0, V), or (K, B, t1 - t0, V)
+        when mixed]."""
+        B, T, V = tc.shape[0] // K, tc.shape[1], self.vq_bins
+        mix, ranged = weights is not None, state is not None
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
-        if sampling is not None:
-            return self._infer_sampled(pl, tc, return_logits, sampling, S.row_keys(keys, B, tc.device))
+        m = C.byref(pl.struct)
+        if mix:        # the mix entries take the sampling as a nullable argument
+            entry = lib.mtts_plm_infer_mix_range_f32 if ranged else lib.mtts_plm_infer_mix_f32
+        elif smp is None:
+            entry = lib.mtts_plm_infer_range_f32 if ranged else lib.mtts_plm_infer_f32
+        else:
+            entry = lib.mtts_plm_infer_range_sample_f32 if ranged else lib.mtts_plm_infer_sample_f32
 
-        def run(tc_):
+        def run(tc_, *rest):
+            state_, rest = (rest[0], rest[1:]) if ranged else (None, rest)
+            w_, rest = (rest[0], rest[1:]) if mix else (None, rest)
             codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
-            logits = torch.empty(B, T, self.vq_bins, dtype=torch.float32, device=tc_.device) if return_logits else None
-            ws = ops.workspace(lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T), tc_.device)
-            L.check(lib.mtts_plm_infer_f32(C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
-                                           codes.data_ptr(), logits.data_ptr() if return_logits else None,
-                                           ws.data_ptr(), ws.numel(), ops._stream()))
-            return (codes, logits) if return_logits else (codes,)
+            logits = torch.empty(K * B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
+            nbytes = (lib.mtts_plm_infer_mix_workspace_bytes(m, K, B, T) if mix else
+                      lib.mtts_plm_infer_workspace_bytes(m, B, T))
+            if ranged:
+                ws, ws_bytes = torch.empty(nbytes + 256, dtype=torch.uint8, device=tc_.device), nbytes
+            else:
+                ws = ops.workspace(nbytes, tc_.device)
+                ws_bytes = ws.numel()
+            lat = (tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T)
+            steps = (t0, t1, state_.data_ptr()) if ranged else ()
+            outs = (codes.data_ptr(), logits.data_ptr() if return_logits else None)
+            s = C.byref(smp[0].struct(*rest)) if smp is not None else None
+            if mix:
+                args = (m, K) + lat + (w_.data_ptr(),) + steps + outs + (s,)
+            else:
+                args = (m,) + lat + steps + outs + ((s,) if s is not None else ())
+            L.check(entry(*args, ws.data_ptr(), ws_bytes, ops._stream()))
+            return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
 
-        # the whole decode is one device-side enqueue sequence: replayed as a CUDA graph from the second call on
-        out = self._graphs().run(("plm", pl.serial, B, T, bool(return_logits), tc.stride(0), tc.stride(1),
-                                  ops.launch_policy_now()), (tc,), run)
-        codes = out[0]
-        logits = out[1] if return_logits else None
-        return (codes, logits) if return_logits else codes
-
-    def _infer_sampled(self, pl, tc, return_logits, sampling, keys):
-        B, T, _ = tc.shape
-        lib = L.lib()
-
-        def run(tc_, seed_, keys_):
-            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
-            logits = torch.empty(B, T, self.vq_bins, dtype=torch.float32, device=tc_.device) if return_logits else None
-            ws = ops.workspace(lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T), tc_.device)
-            s = sampling.struct(seed_, keys_)
-            L.check(lib.mtts_plm_infer_sample_f32(C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
-                                                  codes.data_ptr(), logits.data_ptr() if return_logits else None,
-                                                  C.byref(s), ws.data_ptr(), ws.numel(), ops._stream()))
-            return (codes, logits) if return_logits else (codes,)
-
-        out = self._graphs().run(("plm_sample", pl.serial, B, T, bool(return_logits), tc.stride(0), tc.stride(1),
-                                  ops.launch_policy_now(), sampling.graph_key()),
-                                 (tc, sampling.seed_tensor(tc.device), keys), run)
-        return (out[0], out[1]) if return_logits else out[0]
+        inputs = (tc,) + ((state,) if ranged else ()) + ((weights,) if mix else ()) + (smp[1:] if smp is not None else ())
+        key = (pl.serial, K, mix, B, T, t0, t1, bool(return_logits), tc.stride(0), tc.stride(1), ops.launch_policy_now(),
+               None if smp is None else smp[0].graph_key())
+        out = self._graphs("range" if ranged else "main").run(key, inputs, run)
+        if not return_logits:
+            return out[0]
+        return out[0], (out[1].reshape(K, B, t1 - t0, V) if mix else out[1])
 
     def _mix_sources(self, tc_latents, weights):
         """K source latents, each (B, T, tc_dim), and their weights -> (the (K*B, T, tc_dim) stack, (B, K) device weights)."""
@@ -217,26 +250,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         _eval_only(self)
         tc, w = self._mix_sources(tc_latents, weights)
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
-        V = self.vq_bins
-        pl = self._plan_get(tc.device, T)
-        lib = L.lib()
-
-        def run(tc_, w_, *smp):
-            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
-            logits = torch.empty(K * B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
-            ws = ops.workspace(lib.mtts_plm_infer_mix_workspace_bytes(C.byref(pl.struct), K, B, T), tc_.device)
-            s = C.byref(sampling.struct(*smp)) if smp else None
-            L.check(lib.mtts_plm_infer_mix_f32(C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
-                                               w_.data_ptr(), codes.data_ptr(),
-                                               logits.data_ptr() if return_logits else None, s, ws.data_ptr(), ws.numel(),
-                                               ops._stream()))
-            return (codes, logits) if return_logits else (codes,)
-
-        inputs = (tc, w) if sampling is None else (tc, w, sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device))
-        out = self._graphs().run(("plm_mix", pl.serial, K, B, T, bool(return_logits), tc.stride(0), tc.stride(1),
-                                  ops.launch_policy_now(), None if sampling is None else sampling.graph_key()),
-                                 inputs, run)
-        return (out[0], out[1].view(K, B, T, V)) if return_logits else out[0]
+        return self._decode(tc, K, w, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits)
 
     def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None) -> "PLMDecode":
         """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
@@ -248,80 +262,32 @@ class MegaPLM(pack.PlanMixin, nn.Module):
             K = len(tc_latent)
             tc, w = self._mix_sources(tc_latent, weights)
         else:
-            tc = ops._dev(tc_latent, name="tc_latent")
-            if tc.stride(2) != 1:
-                tc = tc.contiguous()
+            tc = _dev_rows(tc_latent, "tc_latent")
         B, T = tc.shape[0] // K, tc.shape[1]
         state = torch.full((B, T + 1), self.vq_bins, dtype=torch.int64, device=tc.device)   # column 0 = BOS
-        if sampling is None:
-            return PLMDecode(tc, state, None, None, None, w)
-        return PLMDecode(tc, state, sampling, sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device), w)
+        smp = _sampling_inputs(sampling, keys, B, tc.device) or (None, None, None)
+        return PLMDecode(tc, state, *smp, w)
 
     def decode_until(self, dec: "PLMDecode", t1: int, return_logits: bool = False):
         """Run steps [dec.t, t1) of the decode begun by ``begin_decode`` -> the new codes (B, t1 - dec.t) int64 [, their
         logits (B, t1 - dec.t, vq_bins)].  Each range replays as a CUDA graph keyed by (B, T, t0, t1), from a cache of its
-        own (``_range_graphs``), so streaming never evicts ``infer``'s graphs; a captured range pins a private workspace of
-        ``mtts_plm_infer_workspace_bytes(B, T)`` bytes.  A mixed decode (``begin_decode(..., weights=...)``) returns the
+        own (``_graphs("range")``), so streaming never evicts ``infer``'s graphs; a captured range pins a private workspace
+        of ``mtts_plm_infer_workspace_bytes(B, T)`` bytes.  A mixed decode (``begin_decode(..., weights=...)``) returns the
         logits as (K, B, t1 - dec.t, vq_bins) and replays with the weights as a graph input."""
         _eval_only(self)
-        tc, B, T, t0 = dec.tc, dec.B, dec.T, dec.t
-        t1 = int(t1)
+        B, T, t0, t1 = dec.B, dec.T, dec.t, int(t1)
         if not t0 <= t1 <= T:
             raise L.MttsError(f"decode_until: t1 = {t1} outside [{t0}, {T}]")
-        V = self.vq_bins
-        K, mix = dec.K, dec.weights is not None
         if t1 == t0:
-            codes = torch.empty(B, 0, dtype=torch.int64, device=tc.device)
-            lg_shape = (K, B, 0, V) if mix else (B, 0, V)
-            return (codes, torch.empty(*lg_shape, device=tc.device)) if return_logits else codes
-        pl = self._plan_get(tc.device, T)
-        lib = L.lib()
-        nbytes = (lib.mtts_plm_infer_mix_workspace_bytes(C.byref(pl.struct), K, B, T) if mix else
-                  lib.mtts_plm_infer_workspace_bytes(C.byref(pl.struct), B, T))
-
-        def run(tc_, state_, *rest):
-            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
-            logits = torch.empty(K * B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
-            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=tc_.device)   # private: a captured range pins it
-            lg = logits.data_ptr() if return_logits else None
-            if mix:
-                w_, smp = rest[0], rest[1:]
-                s = C.byref(dec.sampling.struct(*smp)) if smp else None
-                L.check(lib.mtts_plm_infer_mix_range_f32(C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0),
-                                                         tc_.stride(1), B, T, w_.data_ptr(), t0, t1, state_.data_ptr(),
-                                                         codes.data_ptr(), lg, s, ws.data_ptr(), nbytes, ops._stream()))
-                return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
-            args = (C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T, t0, t1, state_.data_ptr(),
-                    codes.data_ptr(), lg)
-            if rest:
-                s = dec.sampling.struct(*rest)
-                L.check(lib.mtts_plm_infer_range_sample_f32(*args, C.byref(s), ws.data_ptr(), nbytes, ops._stream()))
-            else:
-                L.check(lib.mtts_plm_infer_range_f32(*args, ws.data_ptr(), nbytes, ops._stream()))
-            return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
-
-        smp_key = None if dec.sampling is None else dec.sampling.graph_key()
-        inputs = (tc, dec.state) + ((dec.weights,) if mix else ()) + (() if dec.sampling is None else (dec.seed, dec.keys))
-        key = ("plm_range", pl.serial, B, T, t0, t1, bool(return_logits), tc.stride(0), tc.stride(1),
-               ops.launch_policy_now(), smp_key)
-        out = self._range_graphs().run(key + (("mix", K),) if mix else key, inputs, run)
-        dec.state[:, t0 + 1:t1 + 1].copy_(out[0])     # a replay advanced the graph's copy of the state, not dec.state
+            codes = torch.empty(B, 0, dtype=torch.int64, device=dec.tc.device)
+            lg_shape = (B, 0, self.vq_bins) if dec.weights is None else (dec.K, B, 0, self.vq_bins)
+            return (codes, torch.empty(*lg_shape, device=dec.tc.device)) if return_logits else codes
+        smp = None if dec.sampling is None else (dec.sampling, dec.seed, dec.keys)
+        out = self._decode(dec.tc, dec.K, dec.weights, smp, t0, t1, dec.state, return_logits)
+        # a replay advanced the graph's copy of the state, not dec.state
+        dec.state[:, t0 + 1:t1 + 1].copy_(out[0] if return_logits else out)
         dec.t = t1
-        if not return_logits:
-            return out[0]
-        return (out[0], out[1].reshape(K, B, t1 - t0, V)) if mix else (out[0], out[1])
-
-    def _range_graphs(self):
-        g = self.__dict__.get("_range_graph_cache")
-        if g is None:
-            from .. import graphs
-            g = self.__dict__["_range_graph_cache"] = graphs.GraphedCall()
-        return g
-
-    def __getstate__(self):
-        d = super().__getstate__()
-        d.pop("_range_graph_cache", None)
-        return d
+        return out
 
     def infer_causal(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None,
                      keys=None):
@@ -333,25 +299,18 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         logits equal the teacher-forced ``forward`` logits evaluated on its own output.  Same I/O as ``infer``,
         ``sampling`` and ``keys`` included (the same noise as ``infer`` for a given seed, key and step)."""
         _eval_only(self)
-        tc = ops._dev(tc_latent, name="tc_latent")
-        if tc.stride(2) != 1:
-            tc = tc.contiguous()
+        tc = _dev_rows(tc_latent, "tc_latent")
         B, T, _ = tc.shape
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
         codes = torch.empty(B, T, dtype=torch.int64, device=tc.device)
         logits = torch.empty(B, T, self.vq_bins, dtype=torch.float32, device=tc.device) if return_logits else None
         ws = ops.workspace(lib.mtts_plm_decode_causal_workspace_bytes(C.byref(pl.struct), B, T), tc.device)
-        if sampling is None:
-            L.check(lib.mtts_plm_decode_causal_f32(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B, T,
-                                                   codes.data_ptr(), logits.data_ptr() if return_logits else None,
-                                                   ws.data_ptr(), ws.numel(), ops._stream()))
-        else:
-            seed, keys = sampling.seed_tensor(tc.device), S.row_keys(keys, B, tc.device)
-            s = sampling.struct(seed, keys)
-            L.check(lib.mtts_plm_decode_causal_sample_f32(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B,
-                                                          T, codes.data_ptr(), logits.data_ptr() if return_logits else None,
-                                                          C.byref(s), ws.data_ptr(), ws.numel(), ops._stream()))
+        smp = _sampling_inputs(sampling, keys, B, tc.device)     # held until the call: the struct points into it
+        entry = lib.mtts_plm_decode_causal_f32 if smp is None else lib.mtts_plm_decode_causal_sample_f32
+        s = () if smp is None else (C.byref(sampling.struct(*smp[1:])),)
+        L.check(entry(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B, T, codes.data_ptr(),
+                      logits.data_ptr() if return_logits else None, *s, ws.data_ptr(), ws.numel(), ops._stream()))
         return (codes, logits) if return_logits else codes
 
     @classmethod
@@ -399,25 +358,12 @@ class MegaADM(pack.PlanMixin, nn.Module):
         self._plan = None
 
     def _plan_get(self, device, T):
-        sig = pack.signature(list(self.parameters())) + (getattr(self.adm, "engine", None), pack.default_engine())
-        if self._plan is None or self._plan.sig != sig or self._plan.pe_rows < T:
-            pl = pack.Plan()
-            pl.sig = sig
-            enc_pl = encoder_plan(self.adm, list(self.adm.layers))
-            pl.hold(enc_pl)
-            s = L.ADM()
-            s.enc = enc_pl.enc
+        def fill(pl, s):
             s.w_dt = pl.p(self.dt_linear_emb.weight.detach()[:, 0].contiguous())
             s.w_tc = pl.p(pack.pack_linear(self.tc_linear_emb.weight))
             s.w_predict = pl.p(self.predict_layer.weight.detach()[0].contiguous())
-            pe = self.pos_emb.table(device, max(T, 4000))
-            pl.pe_rows = pe.shape[0]
-            s.pe = pl.p(pe)
-            s.pe_alpha = self.pos_emb.alpha_host()
             s.emb_dim, s.tc_dim, s.tc_emb_dim = self.emb_dim, self.tc_latent_dim, self.tc_emb_dim
-            pl.struct = s
-            self._plan = pl
-        return self._plan
+        return _ar_plan(self, self.adm, self.pos_emb, L.ADM, device, T, fill)
 
     def forward(self, tc_latents: torch.Tensor, duration_tokens: torch.Tensor, lens: torch.Tensor):
         """Teacher-forced duration regression (models/megatts2.py:233-255); training mode runs on autograd Functions."""
@@ -443,9 +389,7 @@ class MegaADM(pack.PlanMixin, nn.Module):
         (p + 0.5) -> int32 -> clamp(1, 128)  (models/megatts2.py:257-275).
         tc_latents (B,T,512) -> (B,T,1) int32 [, raw (B,T) fp32]."""
         _eval_only(self)
-        tc = ops._dev(tc_latents, name="tc_latents")
-        if tc.stride(2) != 1:
-            tc = tc.contiguous()
+        tc = _dev_rows(tc_latents, "tc_latents")
         B, T, _ = tc.shape
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
@@ -471,9 +415,7 @@ class MegaADM(pack.PlanMixin, nn.Module):
         the training semantics of ``forward`` (causal=True, models/megatts2.py:244) with ``infer``'s raw-float
         feedback and final rounding; one row per utterance per step against K/V caches.  Same I/O as ``infer``."""
         _eval_only(self)
-        tc = ops._dev(tc_latents, name="tc_latents")
-        if tc.stride(2) != 1:
-            tc = tc.contiguous()
+        tc = _dev_rows(tc_latents, "tc_latents")
         B, T, _ = tc.shape
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
@@ -600,9 +542,7 @@ class HifiganGenerator(pack.PlanMixin, nn.Module):
 
     def inference_cl(self, mel_cl: torch.Tensor) -> torch.Tensor:
         """mel (B, T, 80) channels-last -> wav (B, 1, 256*(T+10))."""
-        mel = ops._dev(mel_cl, name="mel")
-        if mel.stride(2) != 1:
-            mel = mel.contiguous()
+        mel = _dev_rows(mel_cl, "mel")
         B, T, _ = mel.shape
         pl = self._plan_get()
         lib = L.lib()
@@ -700,6 +640,17 @@ class _RangeRestart(Exception):
     """An fp16 range flag raised before a stream yielded its first synthesized chunk."""
 
 
+def _fp16_operands():
+    """Whether the default engine feeds the tensor cores fp16 operands (f16x2 or f16), whose range the flag read by
+    ``ops.tc_overflow`` guards."""
+    return pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16)
+
+
+def _warn_fp16_range(then):
+    import warnings
+    warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; " + then, stacklevel=2)
+
+
 class Megatts(nn.Module):
     """Inference orchestrator (models/megatts2.py:295-375).  ``synthesize`` is the tensor-level
     body of the reference's ``forward`` for a batch; ``forward(wavs_dir, text)`` keeps the
@@ -762,10 +713,8 @@ class Megatts(nn.Module):
         args = (phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt, sampling, keys,
                 prosody_mels, prosody_weights)
         out = self._synthesize(*args)
-        if check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16) and ops.tc_overflow(dev):
-            import warnings
-            warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
-                          "re-running this batch on the bf16x3 engine")
+        if check_range and _fp16_operands() and ops.tc_overflow(dev):
+            _warn_fp16_range("re-running this batch on the bf16x3 engine")
             with pack.engine_scope(pack.ENGINE_BF16X3):
                 out = self._synthesize(*args)
         if return_intermediates:
@@ -839,14 +788,13 @@ class Megatts(nn.Module):
         else:
             tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
             dt = adm_decode(tc_latent)[..., 0]
-        d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
-        tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
-        tc8 = ops.maxpool_time(tc_expand, 8)
+        tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels)
         if prosody_mels is not None:
-            srcs = [tc8] + self._prosody_sources(phone_tokens, prosody_mels, d_used, tc_expand.shape[1])
-            p_codes = self.plm.infer_mix(srcs, prosody_weights, sampling=sampling, keys=keys)
+            tc8 = src[0]
+            p_codes = self.plm.infer_mix(src, prosody_weights, sampling=sampling, keys=keys)
         else:
-            p_codes = plm_decode(tc8) if sampling is None else plm_decode(tc8, sampling=sampling, keys=keys)
+            tc8 = src
+            p_codes = plm_decode(src, sampling=sampling, keys=keys)
         B, Lmax = tc_expand.shape[0], tc_expand.shape[1]
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]
@@ -878,12 +826,21 @@ class Megatts(nn.Module):
         return dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
                     mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
 
-    def _prosody_sources(self, phone_tokens, prosody_mels, d_used, Lmax):
-        """The PLM latent of each prosody prompt: MRTE on (phone_tokens, prompt), length-regulated with the target's
+    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels):
+        """The synthesis front end between the ADM and the PLM: the durations (``forced_durations`` if given, else
+        ``dt``) expand ``tc_latent`` to frames -> (tc_expand (B, Lmax, tc_dim), the per-utterance frame totals on the host
+        (one host sync), the PLM's source).  The source is tc8, tc_expand max-pooled by 8, or with ``prosody_mels`` the
+        list [tc8, *one latent per prosody prompt]: MRTE on (phone_tokens, prompt), length-regulated with the same
         durations to Lmax frames, max-pooled by 8."""
-        mrte = self.generator.mrte
-        return [ops.maxpool_time(ops.length_regulate(mrte.tc_latent(phone_tokens, m), d_used, l_out=Lmax)[0], 8)
-                for m in prosody_mels]
+        d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
+        tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
+        tc8 = ops.maxpool_time(tc_expand, 8)
+        if prosody_mels is None:
+            return tc_expand, totals, tc8
+        mrte, Lmax = self.generator.mrte, tc_expand.shape[1]
+        return tc_expand, totals, [tc8] + [
+            ops.maxpool_time(ops.length_regulate(mrte.tc_latent(phone_tokens, m), d_used, l_out=Lmax)[0], 8)
+            for m in prosody_mels]
 
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
@@ -912,7 +869,7 @@ class Megatts(nn.Module):
         if int(chunk_frames) < 1:
             raise L.MttsError(f"synthesize_stream: chunk_frames must be >= 1, got {chunk_frames}")
         self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False)
-        guard = check_range and pack.default_engine() in (pack.ENGINE_F16X2, pack.ENGINE_F16)
+        guard = check_range and _fp16_operands()
         return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
                                   int(chunk_frames), (prosody_mels, prosody_weights))
 
@@ -922,9 +879,7 @@ class Megatts(nn.Module):
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
                                     prosody)
         except _RangeRestart:
-            import warnings
-            warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; "
-                          "restarting this stream on the bf16x3 engine")
+            _warn_fp16_range("restarting this stream on the bf16x3 engine")
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, False, chunk_frames,
                                     prosody, engine=pack.ENGINE_BF16X3)
 
@@ -945,17 +900,11 @@ class Megatts(nn.Module):
         with torch.no_grad(), scope():
             tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
             dt = self.adm.infer(tc_latent)[..., 0]
-            d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
-            tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
-            tc8 = ops.maxpool_time(tc_expand, 8)
             prosody_mels, prosody_weights = prosody
-            if prosody_mels is not None:
-                srcs = [tc8] + self._prosody_sources(phone_tokens, prosody_mels, d_used, tc_expand.shape[1])
-                dec = self.plm.begin_decode(srcs, sampling=sampling, keys=keys, weights=prosody_weights)
-            else:
-                dec = self.plm.begin_decode(tc8, sampling=sampling, keys=keys)
+            tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels)
+            dec = self.plm.begin_decode(src, sampling=sampling, keys=keys, weights=prosody_weights)
             pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
-        B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], tc8.shape[1]
+        B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], dec.T
         if Lmax < 1:
             raise L.MttsError("synthesize_stream: every utterance has zero frames")
         mel = torch.zeros(B, Lmax, gen.mrte.mel_bins, dtype=torch.float32, device=dev)
@@ -971,9 +920,7 @@ class Megatts(nn.Module):
                 return False
             if not emitted:
                 raise _RangeRestart()
-            import warnings
-            warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; finishing this "
-                          "stream on the bf16x3 engine (its chunks can differ from synthesize's rerun)")
+            _warn_fp16_range("finishing this stream on the bf16x3 engine (its chunks can differ from synthesize's rerun)")
             guard, engine = False, pack.ENGINE_BF16X3
             return True
 

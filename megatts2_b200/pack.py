@@ -254,16 +254,17 @@ class PlanMixin:
     def __getstate__(self):
         d = self.__dict__.copy()
         d["_plan"] = None
-        d.pop("_graph_cache", None)
+        d.pop("_graph_caches", None)
         return d
 
-    def _graphs(self):
-        """CUDA-graph cache of this module's device-only drivers (megatts2_b200/graphs.py)."""
-        g = self.__dict__.get("_graph_cache")
-        if g is None:
+    def _graphs(self, name="main"):
+        """CUDA-graph cache ``name`` of this module's device-only drivers (megatts2_b200/graphs.py).  Each name is a cache
+        of its own, so one kind of call never evicts another's graphs."""
+        caches = self.__dict__.setdefault("_graph_caches", {})
+        if name not in caches:
             from . import graphs
-            g = self.__dict__["_graph_cache"] = graphs.GraphedCall()
-        return g
+            caches[name] = graphs.GraphedCall()
+        return caches[name]
 
 
 class Plan:
