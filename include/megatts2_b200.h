@@ -211,6 +211,13 @@ int mtts_attention_tc_f32(const mtts_attn_params* p, void* stream);
  * `min_len` rows runs on the tensor-core kernel (one 64-row tile per head) instead of the fp32 kernel; min_len <= 0 switches it off (the default: it is slower
  * inside the synthesis step, see csrc/ops.cu).  Returns the previous setting. */
 int mtts_set_attention_pair_min(int32_t min_len);
+/* Diagnostics (host only, no CUDA call; only the alignment of the pointers in *p is read): the kernel mtts_attention_f32
+ * (allow_f16_operands = 0) or mtts_attention_tc_f32 (1) launches for *p when mtts_set_attention_pair_min is set to
+ * pair_min.  out6 = {kernel (MTTS_ATTN_*), dh, then for MTTS_ATTN_FP32 its instantiation: query rows per warp RW, warps
+ * per CTA NW, keys per lane and tile KPL (0 otherwise), 16-byte loads (1) or scalar ones (0)}.  The argument checks and
+ * error codes are those of the launches. */
+enum { MTTS_ATTN_NONE = -1, MTTS_ATTN_FP32 = 0, MTTS_ATTN_TC = 1, MTTS_ATTN_TC_PAIR = 2 };
+int mtts_attention_plan_query(const mtts_attn_params* p, int32_t allow_f16_operands, int32_t pair_min, int32_t* out6);
 
 /* EuclideanCodebook.quantize (modules/quantization/core_vq.py:175-183): first index of
  * max_k -(|x|^2 - 2 x.e_k + |e_k|^2).  x (N, D) ld = ldx, embed (K, D) -> idx (N) int64 */

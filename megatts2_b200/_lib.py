@@ -129,6 +129,7 @@ SIGNATURES = {
     "mtts_tc_plan_query": (C.c_int, [i32, i32, i32, i32, i32, i32, i32, i32, i64, i32, C.POINTER(i32)]),
     "mtts_tc_plan_query_ex": (C.c_int, [i32, i32, i32, i32, i32, i32, i32, i32, i64, i32, i32, C.POINTER(i32)]),
     "mtts_set_attention_pair_min": (C.c_int, [i32]),
+    "mtts_attention_plan_query": (C.c_int, [C.POINTER(AttnParams), i32, i32, C.POINTER(i32)]),
     "mtts_mask_tail_f32": (C.c_int, [vp, i32, i32, i32, vp, vp]),
     "mtts_resample_f32": (C.c_int, [vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, vp, i64, i32, vp, vp]),
     "mtts_peak_normalize_f32": (C.c_int, [vp, i64, i32, i32, vp, vp, vp]),

@@ -937,6 +937,9 @@ int mtts_split_planes_f32(const float* x, int32_t ldx, int64_t rows, int32_t C, 
 }
 int mtts_tc_overflow_bind(int32_t* flag_dev) { return tc_overflow_bind(flag_dev); }
 int mtts_set_attention_pair_min(int32_t min_len) { return set_attention_pair_min(min_len); }
+int mtts_attention_plan_query(const mtts_attn_params* p, int32_t allow_f16_operands, int32_t pair_min, int32_t* out6) {
+  return attention_plan_query(p, allow_f16_operands, pair_min, out6);
+}
 int mtts_set_sm_limit(int32_t n_sms) { return set_sm_limit(n_sms); }
 int mtts_set_launch_policy(int32_t sm_limit, int32_t allow_pairs, int32_t allow_pdl) {
   return set_launch_policy(sm_limit, allow_pairs, allow_pdl);

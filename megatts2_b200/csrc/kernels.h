@@ -135,6 +135,15 @@ int layernorm(const float* x, int ldx, const float* gamma, const float* beta, co
               int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, cudaStream_t st);
 // allow_f16_operands: the caller's engine accepts fp16-range operands, so long sequences may use attn_tc.cu (f16x2 planes)
 int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t st);
+// attention()'s routing as a pure host function: attn_check holds the argument checks, attn_plan picks the kernel
+// (MTTS_ATTN_*, or ATTN_UNSUPPORTED for a head dim without one), and for the fp32 kernel its attn_kernel<dh / 32, RW, NW,
+// KPL> instantiation and whether it takes the 16-byte load path (vec); pair_min: shortest AR step routed to the tensor
+// cores (1 << 30: off)
+constexpr int ATTN_UNSUPPORTED = -2;
+struct AttnPlan { int kernel, dh, rw, nw, kpl, vec; };
+int attn_check(const mtts_attn_params& p);
+AttnPlan attn_plan(const mtts_attn_params& p, bool allow_f16_operands, int pair_min);
+int attention_plan_query(const mtts_attn_params* p, int allow_f16_operands, int pair_min, int32_t* out6);
 bool attention_tc_eligible(const mtts_attn_params& p);
 int attention_tc(const mtts_attn_params& p, cudaStream_t st);
 bool attention_tc_pair_eligible(const mtts_attn_params& p);

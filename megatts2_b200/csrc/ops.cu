@@ -366,7 +366,7 @@ __global__ void __launch_bounds__(NW * 32, (NI == 2 ? 3 : 2)) attn_kernel(const 
 }
 
 template <int NI, int RW, int NW, int KPL = 1>
-static int attn_launch(const mtts_attn_params& p, cudaStream_t st) {
+static int attn_launch(const mtts_attn_params& p, int vec, cudaStream_t st) {
   constexpr int DH = 32 * NI;
   constexpr int BQ = RW * NW, BKV = 32 * KPL;
   const size_t smem = sizeof(float) * (BQ * DH + BKV * (DH + 4) + BKV * DH + NW * RW * BKV);
@@ -378,9 +378,6 @@ static int attn_launch(const mtts_attn_params& p, cudaStream_t st) {
     if (e != cudaSuccess) return fail(MTTS_ERR_CUDA, "%s: cudaFuncSetAttribute failed: %lld", "attention", (long long)e);
     configured.fetch_or(1ull << dev, std::memory_order_relaxed);
   }
-  auto al = [](const void* q) { return (((uintptr_t)q) & 15) == 0; };
-  const int vec = al(p.q) && al(p.k) && al(p.v) && p.q_st % 4 == 0 && p.k_st % 4 == 0 && p.v_st % 4 == 0 &&
-                  p.q_sb % 4 == 0 && p.k_sb % 4 == 0 && p.v_sb % 4 == 0;
   dim3 grid((unsigned)cdiv64(p.Tq, BQ), (unsigned)p.H, (unsigned)p.B);
   launch_k(attn_kernel<NI, RW, NW, KPL>, grid, NW * 32, smem, st, p, vec, p.o_planes ? tc_ovf_ptr() : nullptr);
   MTTS_CHECK_LAUNCH();
@@ -393,12 +390,19 @@ static std::atomic<int> g_attn_pair_min{[] {
 }()};
 int set_attention_pair_min(int n) { return g_attn_pair_min.exchange(n > 0 ? n : (1 << 30), std::memory_order_relaxed); }
 
-int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t st) {
+int attn_check(const mtts_attn_params& p) {
   MTTS_REQUIRE(p.q && p.k && p.v && (p.o || p.o_planes), "null pointer");
   MTTS_REQUIRE(!p.o_planes || (p.o_planes_ld % 4 == 0 && p.o_plane_stride % 4 == 0), "plane output alignment");
   MTTS_REQUIRE(p.B >= 0 && p.H > 0 && p.Tq >= 0 && p.Tk > 0, "bad dims");
   MTTS_REQUIRE(p.H <= 65535 && p.B <= 65535, "grid too large");
-  if (p.B == 0 || p.Tq == 0) return 0;
+  return 0;
+}
+
+AttnPlan attn_plan(const mtts_attn_params& p, bool allow_f16_operands, int pair_min) {
+  AttnPlan pl{MTTS_ATTN_NONE, (int)p.dh, 0, 0, 0, 0};
+  if (p.B == 0 || p.Tq == 0) return pl;
+  pl.vec = al16(p.q) && al16(p.k) && al16(p.v) && p.q_st % 4 == 0 && p.k_st % 4 == 0 && p.v_st % 4 == 0 && p.q_sb % 4 == 0 &&
+           p.k_sb % 4 == 0 && p.v_sb % 4 == 0;
   // tensor-core path (attn_tc.cu): the head dims of the AR stacks once a sequence has more than 64 queries.  At the C4 step
   // shapes (Tq = Tk <= 64) a head is a 64 x 64 x 64 problem, all latency, so the AR steps of the benchmark stay on this fp32
   // kernel; longer sequences (teacher-forced forwards, config C3) go to the tensor cores.
@@ -406,40 +410,77 @@ int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t s
   // FFMA engines keep the full fp32 range here.
   if (allow_f16_operands) {
     constexpr int tc_min = 65;
-    if (p.Tq >= tc_min && attention_tc_eligible(p)) return attention_tc(p, st);
+    if (p.Tq >= tc_min && attention_tc_eligible(p)) { pl.kernel = MTTS_ATTN_TC; return pl; }
     // AR steps (Tq == Tk <= 64) on the tensor cores: one 64-row tile per head.  The operand conversions, not the MMAs, are
     // what a 64 x 64 x 64 head costs, so it is opt-in (mtts_set_attention_pair_min / MEGATTS2_ATTN_PAIR_MIN: shortest
     // sequence that takes it), off by default.
-    const int pair_min = g_attn_pair_min.load(std::memory_order_relaxed);
-    if (p.Tq >= pair_min && attention_tc_pair_eligible(p)) return attention_tc_pair(p, st);
+    if (p.Tq >= pair_min && attention_tc_pair_eligible(p)) { pl.kernel = MTTS_ATTN_TC_PAIR; return pl; }
   }
   // dh <= 128: one CTA of 8 warps covers a whole AR-step sequence (Tq <= 64), so K and V are read once per (b, h);
   // the rows are dealt evenly to the warps (RW = ceil(Tq / 8) rows each) - with a fixed 8 rows per warp a 35-row
   // step left three of the eight warps idle.  Row results do not depend on RW (each row's sums keep their order).
+  // KPL = 2 (Tk > 32): two keys per lane, one 64-key tile instead of two 32-key tiles.
   if (p.dh == 64 || p.dh == 96 || p.dh == 128) {
-    const int rw = p.Tq >= 64 ? 8 : (p.Tq + 7) / 8;
-    const bool two = p.Tk > 32;          // two keys per lane: one 64-key tile instead of two 32-key tiles
-#define MTTS_ATTN_RW(NI)                                                                    \
-    switch (rw) {                                                                             \
-      case 1: return two ? attn_launch<NI, 1, 8, 2>(p, st) : attn_launch<NI, 1, 8>(p, st);    \
-      case 2: return two ? attn_launch<NI, 2, 8, 2>(p, st) : attn_launch<NI, 2, 8>(p, st);    \
-      case 3: return two ? attn_launch<NI, 3, 8, 2>(p, st) : attn_launch<NI, 3, 8>(p, st);    \
-      case 4: return two ? attn_launch<NI, 4, 8, 2>(p, st) : attn_launch<NI, 4, 8>(p, st);    \
-      case 5: return two ? attn_launch<NI, 5, 8, 2>(p, st) : attn_launch<NI, 5, 8>(p, st);    \
-      case 6: return two ? attn_launch<NI, 6, 8, 2>(p, st) : attn_launch<NI, 6, 8>(p, st);    \
-      case 7: return two ? attn_launch<NI, 7, 8, 2>(p, st) : attn_launch<NI, 7, 8>(p, st);    \
-      default: return two ? attn_launch<NI, 8, 8, 2>(p, st) : attn_launch<NI, 8, 8>(p, st);   \
-    }
-    if (p.dh == 64) { MTTS_ATTN_RW(2) }
-    if (p.dh == 96) { MTTS_ATTN_RW(3) }
-    MTTS_ATTN_RW(4)
-#undef MTTS_ATTN_RW
+    pl.kernel = MTTS_ATTN_FP32;
+    pl.rw = p.Tq >= 64 ? 8 : (p.Tq + 7) / 8;
+    pl.nw = 8;
+    pl.kpl = p.Tk > 32 ? 2 : 1;
+  } else if (p.dh == 256 || p.dh == 512) {
+    pl.kernel = MTTS_ATTN_FP32;
+    pl.rw = 4;
+    pl.nw = 4;
+    pl.kpl = 1;
+  } else {
+    pl.kernel = ATTN_UNSUPPORTED;
   }
-  switch (p.dh) {
-    case 256: return attn_launch<8, 4, 4>(p, st);
-    case 512: return attn_launch<16, 4, 4>(p, st);
-    default: return fail(MTTS_ERR_UNSUPPORTED, "%s: head dim %lld not in {64,96,128,256,512}", "attention", p.dh);
+  return pl;
+}
+
+template <int NI>
+static int attn_launch_rw(const mtts_attn_params& p, const AttnPlan& pl, cudaStream_t st) {
+  const bool two = pl.kpl == 2;
+  const int vec = pl.vec;
+  switch (pl.rw) {
+    case 1: return two ? attn_launch<NI, 1, 8, 2>(p, vec, st) : attn_launch<NI, 1, 8>(p, vec, st);
+    case 2: return two ? attn_launch<NI, 2, 8, 2>(p, vec, st) : attn_launch<NI, 2, 8>(p, vec, st);
+    case 3: return two ? attn_launch<NI, 3, 8, 2>(p, vec, st) : attn_launch<NI, 3, 8>(p, vec, st);
+    case 4: return two ? attn_launch<NI, 4, 8, 2>(p, vec, st) : attn_launch<NI, 4, 8>(p, vec, st);
+    case 5: return two ? attn_launch<NI, 5, 8, 2>(p, vec, st) : attn_launch<NI, 5, 8>(p, vec, st);
+    case 6: return two ? attn_launch<NI, 6, 8, 2>(p, vec, st) : attn_launch<NI, 6, 8>(p, vec, st);
+    case 7: return two ? attn_launch<NI, 7, 8, 2>(p, vec, st) : attn_launch<NI, 7, 8>(p, vec, st);
+    default: return two ? attn_launch<NI, 8, 8, 2>(p, vec, st) : attn_launch<NI, 8, 8>(p, vec, st);
   }
+}
+
+int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t st) {
+  MTTS_TRY(attn_check(p));
+  const AttnPlan pl = attn_plan(p, allow_f16_operands, g_attn_pair_min.load(std::memory_order_relaxed));
+  switch (pl.kernel) {
+    case MTTS_ATTN_NONE: return 0;
+    case MTTS_ATTN_TC: return attention_tc(p, st);
+    case MTTS_ATTN_TC_PAIR: return attention_tc_pair(p, st);
+    case MTTS_ATTN_FP32: break;
+    default: return fail(MTTS_ERR_UNSUPPORTED, "%s: head dim %lld not in {64,96,128,256,512}", "attention", (long long)p.dh);
+  }
+  switch (pl.dh) {
+    case 64: return attn_launch_rw<2>(p, pl, st);
+    case 96: return attn_launch_rw<3>(p, pl, st);
+    case 128: return attn_launch_rw<4>(p, pl, st);
+    case 256: return attn_launch<8, 4, 4>(p, pl.vec, st);
+    default: return attn_launch<16, 4, 4>(p, pl.vec, st);
+  }
+}
+
+// diagnostics: the plan attention() would launch for these parameters with `pair_min` as the AR-step routing threshold
+// (<= 0: off); out6 = {kernel (MTTS_ATTN_*), dh, RW, NW, KPL, vec}
+int attention_plan_query(const mtts_attn_params* p, int allow_f16_operands, int pair_min, int32_t* out6) {
+  MTTS_REQUIRE(p && out6, "null params");
+  MTTS_TRY(attn_check(*p));
+  const AttnPlan pl = attn_plan(*p, allow_f16_operands != 0, pair_min > 0 ? pair_min : (1 << 30));
+  if (pl.kernel == ATTN_UNSUPPORTED)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: head dim %lld not in {64,96,128,256,512}", "attention", (long long)p->dh);
+  out6[0] = pl.kernel; out6[1] = pl.dh; out6[2] = pl.rw; out6[3] = pl.nw; out6[4] = pl.kpl; out6[5] = pl.vec;
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------

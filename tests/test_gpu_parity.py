@@ -173,7 +173,7 @@ def test_conv_linearity_property_full_size():
     assert (ops.conv1d(x1, w, None, k=1)[0, rows].double() - ref).abs().max().item() < 5e-5
 
 
-# ------------------------------------------------------------------------------ LN / attention
+# ------------------------------------------------------------------------------ LN
 @pytest.mark.parametrize("C_", [384, 512, 768, 1024, 100])
 def test_layernorm(C_):
     from megatts2_b200 import ops
@@ -191,56 +191,6 @@ def test_layernorm(C_):
     xi = x.clone().to(DEV)                  # in place
     ops.layernorm(xi, ga.to(DEV), be.to(DEV), out=xi)
     assert maxerr(xi, ref) < 1e-5
-
-
-@pytest.mark.parametrize("H,dh,Tq,Tk", [(16, 64, 70, 70), (8, 96, 33, 33), (2, 256, 12, 12), (1, 512, 64, 31),
-                                        (16, 64, 1, 200), (4, 128, 17, 65),
-                                        # tensor-core path (attn_tc.cu): one / several query tiles and key tiles, ragged edges
-                                        (16, 64, 64, 64), (16, 64, 130, 300), (8, 96, 200, 200), (8, 96, 16, 16), (2, 128, 129, 64),
-                                        # two heads per CTA (AR steps, Tq == Tk <= 64)
-                                        (16, 64, 24, 24), (16, 64, 47, 47), (8, 96, 64, 64), (2, 64, 40, 40)])
-def test_attention(H, dh, Tq, Tk):
-    from megatts2_b200 import ops
-    prev = ops.set_attention_pair_min(16)     # the opt-in two-heads-per-CTA kernel takes the eligible cases
-    try:
-        _attention_cases(ops, H, dh, Tq, Tk)
-    finally:
-        ops.set_attention_pair_min(0 if prev >= (1 << 30) else prev)
-    if Tq == Tk and Tk <= 64 and H % 2 == 0 and dh in (64, 96):
-        _attention_cases(ops, H, dh, Tq, Tk)  # and the default (fp32) kernel
-
-
-def _attention_cases(ops, H, dh, Tq, Tk):
-    g = gen(H * 1000 + dh + Tq)
-    B, D = 2, H * dh
-    q, k, v = (torch.randn(B, t, D, generator=g) for t in (Tq, Tk, Tk))
-
-    def ref_attn(mask):
-        qh = q.view(B, Tq, H, dh).transpose(1, 2).double()
-        kh = k.view(B, Tk, H, dh).transpose(1, 2).double()
-        vh = v.view(B, Tk, H, dh).transpose(1, 2).double()
-        s = qh @ kh.transpose(-1, -2) / math.sqrt(dh)
-        if mask is not None:
-            s = s + mask.double()
-        return (torch.softmax(s, -1) @ vh).transpose(1, 2).reshape(B, Tq, D)
-    y = ops.attention(q.to(DEV), k.to(DEV), v.to(DEV), H)
-    assert maxerr(y, ref_attn(None)) < 2e-5
-    if Tq == Tk:
-        m = R.attn_mask(torch.tensor([Tq, Tq], dtype=torch.int32), H, True)
-        y = ops.attention(q.to(DEV), k.to(DEV), v.to(DEV), H, m.to(DEV))
-        assert maxerr(y, ref_attn(m)) < 2e-5
-    pad = torch.zeros(B, 1, 1, Tk)
-    pad[1, ..., Tk // 2:] = float("-inf")
-    y = ops.attention(q.to(DEV), k.to(DEV), v.to(DEV), H, pad.to(DEV))
-    assert maxerr(y, ref_attn(pad)) < 2e-5
-    # strided (packed qkv) inputs
-    qkv = torch.cat([q, q, q], -1).to(DEV) if Tq == Tk else None
-    if qkv is not None:
-        y2 = ops.attention(qkv[..., :D], qkv[..., D:2 * D], qkv[..., 2 * D:], H)
-        qq = q
-        s = (qq.view(B, Tq, H, dh).transpose(1, 2).double() @ qq.view(B, Tq, H, dh).transpose(1, 2).double().transpose(-1, -2)) / math.sqrt(dh)
-        r2 = (torch.softmax(s, -1) @ qq.view(B, Tq, H, dh).transpose(1, 2).double()).transpose(1, 2).reshape(B, Tq, D)
-        assert maxerr(y2, r2) < 2e-5
 
 
 # ------------------------------------------------------------------------------ VQ
