@@ -522,6 +522,43 @@ int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_l
                                  int64_t* codes_out, float* logits_out, const mtts_sampling* s,
                                  void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Duration interpolation: the ADM decoded from a weighted mean of K prompts' duration predictions, the rhythm half of
+ * Mega-TTS 2's prosody (the PLM mix above is the pitch and energy half).  Utterance b has K >= 1 sources; source k is a
+ * latent tc^(k)[b] (T, tc_dim), source 0 conventionally the target prompt's, all with the same T, and b has a weight row
+ * w[b, 0..K) (fp32, every weight >= 0 and finite, row sum > 0; the host never reads it, callers validate it).  All K
+ * sources share one raw-duration history p[b, 0..T], p[b, 0] = 0.  At step t:
+ *   1. each source runs the reference-faithful step (mtts_adm_infer_f32's non-causal full recompute over t+1 positions,
+ *      the last layer pruned to the last row) over its own latent and the shared history -> readout y^(k);
+ *   2. w^_k = w_k / sum_k w_k, the sum in fp32 in k order; sources with w_k = 0 are skipped, even when y^(k) is not finite;
+ *   3. r = w^_k0 * y^(k0) for the first positive weight k0, then r = fmaf(w^_k, y^(k), r) for the later positive weights in
+ *      k order, all in fp32.  With exactly one positive weight w^ = w / w = 1, so r is that source's y bit for bit
+ *      (-0 included: starting from fmaf(1, y, 0) would turn -0 into +0), and a one-hot row decodes exactly what
+ *      mtts_adm_infer_f32 decodes from that source alone.  A row without a positive weight gives r = 0, the empty sum;
+ *   4. p[b, t+1] = r: the mixed value is what the next step reads back, as the single-source decode feeds back its own raw
+ *      prediction.
+ * The durations are mtts_adm_infer_f32's, from the mixed raw values: (r + 0.5) -> int32 -> clamp(1, 128).
+ * Why the mean: the ADM is trained with an MSE loss, so each y^(k) estimates the conditional mean of the next duration
+ * given source k; the weighted mean of the sources' means is the mean of their mixture.  K <= 8 (MTTS_ERR_UNSUPPORTED
+ * above). */
+
+/* The mix readout of one step: xl (K*B, D) contiguous, row k*B + b = the last encoder row of source k of utterance b;
+ * w_predict (D); weights (B, K) contiguous, device (NULL only when K = 1: weight 1).  out[b * ld_out] = r_b; y_out
+ * optional, y_out[(k*B + b) * ld_y] = y^(k)_b for every source, weighted or not.  y is the dot product of
+ * mtts_adm_infer_f32's readout, computed the same way, so y_out equals what that readout writes for the same row. */
+int mtts_adm_readout_mix_f32(const float* xl, int32_t D, const float* w_predict, int32_t K, int32_t B, const float* weights,
+                             float* out, int64_t ld_out, float* y_out, int64_t ld_y, void* stream);
+/* The mixed decode.  tc_latent is the (K*B, T, tc_dim) stack of the sources, row k*B + b = source k of utterance b (batch
+ * stride tc_sb, row stride tc_ld); weights (B, K) device (NULL only when K = 1); dur_out (B, T) int32; raw_out optional
+ * (B, T), the mixed raw values; raw_src_out optional (K, B, T), every source's readout y^(k) at every step.  Each step
+ * runs the encoder once over the K*B rows, then the mix readout.  The weights are read from device memory at every step,
+ * so a replayed CUDA graph picks up new values.  With K = 1 and weights NULL the launch sequence is mtts_adm_infer_f32's
+ * (raw_src_out NULL) and the outputs equal it bit for bit. */
+int64_t mtts_adm_infer_mix_workspace_bytes(const mtts_adm* m, int32_t K, int32_t B, int32_t T);
+int mtts_adm_infer_mix_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                           int32_t B, int32_t T, const float* weights, int32_t* dur_out, float* raw_out,
+                           float* raw_src_out, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ConvNet family (modules/convnet.py).  One ConvBlock = ReLU -> Conv1d(C,C,k,same) -> LN(C). */
 typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv_block;   /* w packed (k,C,C); w_tc (3,k,C,C) bf16 or NULL */
 

@@ -168,6 +168,9 @@ SIGNATURES = {
     "mtts_plm_infer_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
     "mtts_adm_infer_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32]),
     "mtts_adm_infer_f32": (C.c_int, [C.POINTER(ADM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
+    "mtts_adm_readout_mix_f32": (C.c_int, [vp, i32, vp, i32, i32, vp, vp, i64, vp, i64, vp]),
+    "mtts_adm_infer_mix_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32, i32]),
+    "mtts_adm_infer_mix_f32": (C.c_int, [C.POINTER(ADM), i32, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp]),
     "mtts_plm_decode_causal_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32]),
     "mtts_plm_decode_causal_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
     "mtts_adm_decode_causal_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32]),

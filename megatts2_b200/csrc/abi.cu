@@ -118,6 +118,11 @@ int mtts_attention_tc_f32(const mtts_attn_params* p, void* stream) {
   return attention(*p, true, (cudaStream_t)stream);
 }
 
+int mtts_adm_readout_mix_f32(const float* xl, int32_t D, const float* w_predict, int32_t K, int32_t B, const float* weights,
+                             float* out, int64_t ld_out, float* y_out, int64_t ld_y, void* stream) {
+  return adm_readout_mix(xl, D, w_predict, K, B, weights, out, ld_out, y_out, ld_y, (cudaStream_t)stream);
+}
+
 int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t rows, int32_t step, const mtts_sampling* s,
                          int64_t* out, int64_t ld_out, void* stream) {
   MTTS_REQUIRE(s, "null sampling parameters");

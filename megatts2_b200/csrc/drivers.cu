@@ -342,23 +342,32 @@ static int64_t adm_ws_floats(const mtts_adm* m, int B, int T) {
          (int64_t)B * (T + 1) + 6 * 64;
 }
 
+// Duration mix (weights or raw_src_out given): tc holds K sources stacked as K*B rows (row k*B + b = source k of utterance
+// b), all reading the shared (B, T+1) raw history.  tc_linear_emb and each step's encoder run once over the K*B rows, then
+// adm_readout_mix writes the mixed value into the history (and, with raw_src_out (K, B, T), every source's readout).
+// K = 1 without weights or raw_src_out is the plain decode.
 static int adm_infer(const mtts_adm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int32_t* dur_out,
-                     float* raw_out, void* ws, int64_t ws_bytes, cudaStream_t st) {
+                     float* raw_out, void* ws, int64_t ws_bytes, cudaStream_t st, int K = 1, const float* weights = nullptr,
+                     float* raw_src_out = nullptr) {
   const int D = m->enc.d_model;
   MTTS_REQUIRE(D == m->emb_dim + m->tc_emb_dim, "d_model != emb_dim + tc_emb_dim");
   MTTS_REQUIRE(tc && dur_out && m->w_dt && m->w_tc && m->w_predict && m->pe, "null pointer");
+  MTTS_TRY(adm_mix_check(K));
+  MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
   if (B <= 0 || T <= 0) return 0;
+  const bool mix = weights || raw_src_out;
+  const int R = K * B;                                       // latent rows: the K sources of the B utterances
   Arena top(ws, ws_bytes);
-  float* X = top.take<float>((int64_t)B * T * D);
-  float* xl = top.take<float>((int64_t)B * D);
-  float* tc_emb = top.take<float>((int64_t)B * T * m->tc_emb_dim);
+  float* X = top.take<float>((int64_t)R * T * D);
+  float* xl = top.take<float>((int64_t)R * D);
+  float* tc_emb = top.take<float>((int64_t)R * T * m->tc_emb_dim);
   float* praw = top.take<float>((int64_t)B * (T + 1));
-  TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, (int64_t)B * T), (int64_t)B * T, tc_fmt_of_engine(m->enc.engine)};
+  TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, (int64_t)R * T), (int64_t)R * T, tc_fmt_of_engine(m->enc.engine)};
   if (tcs.bytes) tcs.p = top.take<char>(tcs.bytes);
   const int64_t enc_off = align_up(top.off, 256);
-  if (enc_off + encoder_ws_floats(&m->enc, B, T) * 4 > ws_bytes)
+  if (enc_off + encoder_ws_floats(&m->enc, R, T) * 4 > ws_bytes)
     return fail(MTTS_ERR_WORKSPACE, "%s: workspace too small (need %lld bytes)", "adm_infer",
-                enc_off + encoder_ws_floats(&m->enc, B, T) * 4);
+                enc_off + encoder_ws_floats(&m->enc, R, T) * 4);
   // tc_linear_emb(tc_latents[:, :t+1]) is step-invariant row by row: computed once (exact)
   {
     mtts_conv_params p;
@@ -366,18 +375,22 @@ static int adm_infer(const mtts_adm* m, const float* tc, int64_t tc_sb, int tc_l
     p.x = tc; p.ldx = tc_ld; p.x_batch_stride = tc_sb;
     p.w = m->w_tc;
     p.y = tc_emb; p.ldy = m->tc_emb_dim; p.y_batch_stride = (int64_t)T * m->tc_emb_dim;
-    p.B = B; p.Tin = T; p.Tout = T; p.Cin = m->tc_dim; p.Cout = m->tc_emb_dim; p.k = 1; p.stride = 1; p.dil = 1;
+    p.B = R; p.Tin = T; p.Tout = T; p.Cin = m->tc_dim; p.Cout = m->tc_emb_dim; p.k = 1; p.stride = 1; p.dil = 1;
     p.out_scale = 1.0f;
     MTTS_TRY(conv1d(p, st));
   }
   MTTS_TRY(fill_f32(praw, T + 1, B, 0.0f, st));   // p_code = [[0]] (megatts2.py:262-263)
   for (int t = 0; t < T; ++t) {
     const int S = t + 1;
-    MTTS_TRY(adm_build_input(tc_emb, (int64_t)T * m->tc_emb_dim, m->tc_emb_dim, m->tc_emb_dim, praw, T + 1, m->w_dt,
-                             m->emb_dim, m->pe, m->pe_alpha, B, S, X, st));
+    MTTS_TRY(adm_build_input(tc_emb, (int64_t)T * m->tc_emb_dim, m->tc_emb_dim, m->tc_emb_dim, praw, T + 1, B, m->w_dt,
+                             m->emb_dim, m->pe, m->pe_alpha, R, S, X, st));
     Arena ar((char*)ws + enc_off, ws_bytes - enc_off);
-    MTTS_TRY(encoder_forward(&m->enc, X, xl, B, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
-    MTTS_TRY(adm_readout(xl, D, m->w_predict, B, praw, T + 1, t + 1, st));
+    MTTS_TRY(encoder_forward(&m->enc, X, xl, R, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
+    if (mix)
+      MTTS_TRY(adm_readout_mix(xl, D, m->w_predict, K, B, weights, praw + (t + 1), T + 1,
+                               raw_src_out ? raw_src_out + t : nullptr, T, st));
+    else
+      MTTS_TRY(adm_readout(xl, D, m->w_predict, B, praw, T + 1, t + 1, st));
   }
   MTTS_TRY(adm_finalize(praw, T + 1, B, T, dur_out, raw_out, st));
   return 0;
@@ -518,7 +531,7 @@ static int adm_decode_causal(const mtts_adm* m, const float* tc, int64_t tc_sb, 
   MTTS_TRY(fill_f32(praw, T + 1, B, 0.0f, st));   // p_code = [[0]] (megatts2.py:262-263)
   for (int t = 0; t < T; ++t) {
     MTTS_TRY(adm_build_input(tc_emb + (int64_t)t * m->tc_emb_dim, (int64_t)T * m->tc_emb_dim, m->tc_emb_dim, m->tc_emb_dim,
-                             praw + t, T + 1, m->w_dt, m->emb_dim, m->pe + (int64_t)t * D, m->pe_alpha, B, 1, cb.x, st));
+                             praw + t, T + 1, B, m->w_dt, m->emb_dim, m->pe + (int64_t)t * D, m->pe_alpha, B, 1, cb.x, st));
     MTTS_TRY(causal_step(&m->enc, B, T, t, cb, st));
     MTTS_TRY(adm_readout(cb.x, D, m->w_predict, B, praw, T + 1, t + 1, st));
   }
@@ -1011,6 +1024,16 @@ int mtts_adm_infer_f32(const mtts_adm* m, const float* tc_latent, int64_t tc_sb,
                        int32_t* dur_out, float* raw_out, void* workspace, int64_t workspace_bytes, void* stream) {
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
   return adm_infer(m, tc_latent, tc_sb, tc_ld, B, T, dur_out, raw_out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int64_t mtts_adm_infer_mix_workspace_bytes(const mtts_adm* m, int32_t K, int32_t B, int32_t T) {
+  return adm_ws_floats(m, K * B, T) * 4 + 8192;
+}
+int mtts_adm_infer_mix_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                           int32_t T, const float* weights, int32_t* dur_out, float* raw_out, float* raw_src_out,
+                           void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
+  return adm_infer(m, tc_latent, tc_sb, tc_ld, B, T, dur_out, raw_out, workspace, workspace_bytes, (cudaStream_t)stream,
+                   K, weights, raw_src_out);
 }
 
 int64_t mtts_plm_decode_causal_workspace_bytes(const mtts_plm* m, int32_t B, int32_t T) {

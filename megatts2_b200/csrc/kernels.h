@@ -185,10 +185,16 @@ int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const flo
                      cudaStream_t st);
 int fill_i64(int64_t* p, int64_t stride, int n, int64_t v, cudaStream_t st);
 int fill_f32(float* p, int64_t stride, int n, float v, cudaStream_t st);
+// latent row r reads history row r % B_hist (B_hist = B: one history per latent row; fewer: sources sharing a history)
 int adm_build_input(const float* tc_emb, int64_t te_sb, int te_ld, int tc_emb_dim, const float* praw, int p_ld,
-                    const float* w_dt, int emb_dim, const float* pe, float alpha, int B, int S, float* X,
+                    int B_hist, const float* w_dt, int emb_dim, const float* pe, float alpha, int B, int S, float* X,
                     cudaStream_t st);
 int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st);
+// duration mix: r_b from the K rows k*B + b of xl and the (B, K) weights into out[b * ld_out]; y_out (optional) gets every
+// source's readout.  adm_mix_check validates K before a driver enqueues anything.
+int adm_mix_check(int K);
+int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, float* out, int64_t ld_out,
+                    float* y_out, int64_t ld_y, cudaStream_t st);
 int adm_finalize(const float* praw, int p_ld, int B, int T, int32_t* dur, float* raw_out, cudaStream_t st);
 
 // convenience: dense linear layer  Y[M,N] = act(X[M,K] W + b) (+ res)

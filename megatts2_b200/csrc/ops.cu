@@ -882,9 +882,9 @@ int fill_f32(float* p, int64_t stride, int n, float v, cudaStream_t st) {
 
 // ADM step input (models/megatts2.py:265-269): X[b,s,:] = cat(tc_emb[b,s,:], p[b,s]*w_dt[:]) + alpha*pe[s]
 __global__ void adm_build_input_kernel(const float* __restrict__ tc_emb, int64_t te_sb, int te_ld, int tc_emb_dim,
-                                       const float* __restrict__ praw, int p_ld, const float* __restrict__ w_dt,
-                                       int emb_dim, const float* __restrict__ pe, float alpha, int S,
-                                       float* __restrict__ X, int64_t total) {
+                                       const float* __restrict__ praw, int p_ld, int B_hist,
+                                       const float* __restrict__ w_dt, int emb_dim, const float* __restrict__ pe,
+                                       float alpha, int S, float* __restrict__ X, int64_t total) {
   pdl_entry();
   const int D = tc_emb_dim + emb_dim;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -895,18 +895,29 @@ __global__ void adm_build_input_kernel(const float* __restrict__ tc_emb, int64_t
   const int b = (int)(bs / S);
   float v;
   if (d < tc_emb_dim) v = tc_emb[(int64_t)b * te_sb + (int64_t)s * te_ld + d];
-  else v = praw[(int64_t)b * p_ld + s] * __ldg(w_dt + (d - tc_emb_dim));
+  else v = praw[(int64_t)(b % B_hist) * p_ld + s] * __ldg(w_dt + (d - tc_emb_dim));
   X[i] = v * 1.0f + alpha * __ldg(pe + (int64_t)s * D + d);
 }
 
 int adm_build_input(const float* tc_emb, int64_t te_sb, int te_ld, int tc_emb_dim, const float* praw, int p_ld,
-                    const float* w_dt, int emb_dim, const float* pe, float alpha, int B, int S, float* X,
+                    int B_hist, const float* w_dt, int emb_dim, const float* pe, float alpha, int B, int S, float* X,
                     cudaStream_t st) {
   const int64_t total = (int64_t)B * S * (tc_emb_dim + emb_dim);
   if (total <= 0) return 0;
-  launch_k(adm_build_input_kernel, (unsigned)cdiv64(total, 256), 256, 0, st, tc_emb, te_sb, te_ld, tc_emb_dim, praw, p_ld, w_dt, emb_dim, pe, alpha, S, X, total);
+  MTTS_REQUIRE(B_hist >= 1, "B_hist must be >= 1");
+  launch_k(adm_build_input_kernel, (unsigned)cdiv64(total, 256), 256, 0, st, tc_emb, te_sb, te_ld, tc_emb_dim, praw, p_ld,
+           B_hist, w_dt, emb_dim, pe, alpha, S, X, total);
   MTTS_CHECK_LAUNCH();
   return 0;
+}
+
+// x_last . w_predict of one row (models/megatts2.py:272-273), by one warp; every lane returns the sum.  Both readouts
+// call it, so a mixed row with one weighted source reproduces the plain readout bit for bit.
+__device__ __forceinline__ float adm_readout_dot(const float* __restrict__ xl, int64_t row, int D,
+                                                 const float* __restrict__ w, int lane) {
+  float s = 0.f;
+  for (int d = lane; d < D; d += 32) s = fmaf(xl[row * D + d], __ldg(w + d), s);
+  return warp_sum(s);
 }
 
 // ADM readout (models/megatts2.py:272-273): p[b, s_next] = x_last[b,:] . w_predict ; one warp per b
@@ -916,14 +927,67 @@ __global__ void adm_readout_kernel(const float* __restrict__ xl, int D, const fl
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (b >= B) return;
-  float s = 0.f;
-  for (int d = lane; d < D; d += 32) s = fmaf(xl[(int64_t)b * D + d], __ldg(w + d), s);
-  s = warp_sum(s);
+  const float s = adm_readout_dot(xl, b, D, w, lane);
   if (lane == 0) praw[(int64_t)b * p_ld + s_next] = s;
 }
 int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st) {
   if (B <= 0) return 0;
   launch_k(adm_readout_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, B, praw, p_ld, s_next);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
+// Duration mix readout (the contract is stated with mtts_adm_readout_mix_f32 in include/megatts2_b200.h): one warp per
+// utterance b.  The warp computes y of each weighted source (of every source when y_out is given) and folds the weighted
+// ones into r in k order: the first term is w^ y, the later ones fmaf(w^, y, r).
+constexpr int ADM_MIX_MAX_K = 8;
+__global__ void adm_readout_mix_kernel(const float* __restrict__ xl, int D, const float* __restrict__ w, int K, int B,
+                                       const float* __restrict__ weights, float* __restrict__ out, int64_t ld_out,
+                                       float* __restrict__ y_out, int64_t ld_y) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;
+  float wk[ADM_MIX_MAX_K];
+  float wsum = 0.f;
+#pragma unroll
+  for (int k = 0; k < ADM_MIX_MAX_K; ++k) {
+    wk[k] = k < K ? (weights ? weights[(int64_t)b * K + k] : 1.f) : 0.f;
+    if (wk[k] > 0.f) wsum += wk[k];             // zero weights add nothing; NaN or negative ones are skipped throughout
+  }
+  float r = 0.f;
+  bool first = true;
+#pragma unroll
+  for (int k = 0; k < ADM_MIX_MAX_K; ++k) {
+    if (k >= K) break;
+    const bool on = wk[k] > 0.f;
+    if (!on && !y_out) continue;
+    const int64_t row = (int64_t)k * B + b;
+    const float y = adm_readout_dot(xl, row, D, w, lane);
+    if (y_out && lane == 0) y_out[row * ld_y] = y;
+    if (!on) continue;
+    const float wn = wk[k] / wsum;
+    r = first ? wn * y : fmaf(wn, y, r);
+    first = false;
+  }
+  if (lane == 0) out[(int64_t)b * ld_out] = r;
+}
+
+int adm_mix_check(int K) {
+  MTTS_REQUIRE(K >= 1, "K must be >= 1");
+  if (K > ADM_MIX_MAX_K)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: K = %lld sources is above the bound of %lld", "adm_readout_mix", K, ADM_MIX_MAX_K);
+  return 0;
+}
+
+int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, float* out, int64_t ld_out,
+                    float* y_out, int64_t ld_y, cudaStream_t st) {
+  MTTS_TRY(adm_mix_check(K));
+  MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
+  MTTS_REQUIRE(D >= 1 && ld_out >= 0 && ld_y >= 0, "D must be >= 1 and ld >= 0");
+  if (B <= 0) return 0;
+  MTTS_REQUIRE(xl && w && out, "null pointer");
+  launch_k(adm_readout_mix_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, K, B, weights, out, ld_out, y_out, ld_y);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

@@ -64,6 +64,9 @@ class GraphedCall:
                 self.cache[key] = ("eager",)      # capture not possible here (e.g. an allocator or driver restriction)
                 torch.cuda.synchronize()
                 return fn(*inputs)
+            # the captured kernels address the scratch buffers ops.workspace handed out: the graph keeps them alive, since
+            # a later, larger call replaces them there and the allocator would otherwise reuse their memory
+            g.workspaces = ops.workspace_buffers()
             e = (g, static_in, static_out, ops._lib_launch_count() - n0)
             self.cache[key] = e
         elif e[0] == "eager":

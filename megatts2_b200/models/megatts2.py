@@ -47,6 +47,22 @@ def _sampling_inputs(sampling, keys, rows, device):
     return sampling, sampling.seed_tensor(device), S.row_keys(keys, rows, device)
 
 
+def _mix_sources(tc_latents, weights, dim, what):
+    """K source latents, each (B, T, dim), and their weights -> (the (K*B, T, dim) stack, (B, K) device weights).  ``what``
+    names the mix in the error messages."""
+    if isinstance(tc_latents, torch.Tensor) or not len(tc_latents):
+        raise L.MttsError(f"{what}: tc_latents must be a non-empty list of (B, T, tc_dim) tensors")
+    tcs = [ops._dev(t, name=f"tc_latents[{k}]") for k, t in enumerate(tc_latents)]
+    shape = tuple(tcs[0].shape)
+    if len(shape) != 3 or shape[2] != dim or any(tuple(t.shape) != shape for t in tcs):
+        raise L.MttsError(f"{what}: every source must be (B, T, {dim}) with the same B and T, got "
+                          f"{[tuple(t.shape) for t in tcs]}")
+    if any(t.device != tcs[0].device for t in tcs):
+        raise L.MttsError(f"{what}: the sources must be on one device")
+    w = S.mix_weights(weights, len(tcs), shape[0], what).to(tcs[0].device)
+    return torch.cat(tcs, 0), w
+
+
 def _ar_plan(model, enc, pos, struct, device, T, fill):
     """The weight plan of an AR model (MegaPLM / MegaADM), rebuilt when its weights or engine changed or when its
     positional table has fewer than T rows: the encoder ``enc``, then ``fill(plan, s)`` for the model's own fields of the
@@ -224,20 +240,6 @@ class MegaPLM(pack.PlanMixin, nn.Module):
             return out[0]
         return out[0], (out[1].reshape(K, B, t1 - t0, V) if mix else out[1])
 
-    def _mix_sources(self, tc_latents, weights):
-        """K source latents, each (B, T, tc_dim), and their weights -> (the (K*B, T, tc_dim) stack, (B, K) device weights)."""
-        if isinstance(tc_latents, torch.Tensor) or not len(tc_latents):
-            raise L.MttsError("prosody mix: tc_latents must be a non-empty list of (B, T, tc_dim) tensors")
-        tcs = [ops._dev(t, name=f"tc_latents[{k}]") for k, t in enumerate(tc_latents)]
-        shape = tuple(tcs[0].shape)
-        if len(shape) != 3 or shape[2] != self.tc_latent_dim or any(tuple(t.shape) != shape for t in tcs):
-            raise L.MttsError(f"prosody mix: every source must be (B, T, {self.tc_latent_dim}) with the same B and T, got "
-                              f"{[tuple(t.shape) for t in tcs]}")
-        if any(t.device != tcs[0].device for t in tcs):
-            raise L.MttsError("prosody mix: the sources must be on one device")
-        w = S.mix_weights(weights, len(tcs), shape[0]).to(tcs[0].device)
-        return torch.cat(tcs, 0), w
-
     def infer_mix(self, tc_latents, weights, return_logits: bool = False, sampling: S.Sampling = None, keys=None):
         """Prosody interpolation (Mega-TTS 2): the ``infer`` decode of B utterances from a weighted mixture of K sources'
         code distributions.  ``tc_latents``: K tensors (B, T, tc_dim), one per source (e.g. ``tc_latent`` from different
@@ -248,7 +250,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         raw per-source logits].  Replays as a CUDA graph whose inputs are the latents, the weights, the seed and the keys,
         so new weight values need no new capture."""
         _eval_only(self)
-        tc, w = self._mix_sources(tc_latents, weights)
+        tc, w = _mix_sources(tc_latents, weights, self.tc_latent_dim, "prosody mix")
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
         return self._decode(tc, K, w, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits)
 
@@ -260,7 +262,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         K, w = 1, None
         if weights is not None:
             K = len(tc_latent)
-            tc, w = self._mix_sources(tc_latent, weights)
+            tc, w = _mix_sources(tc_latent, weights, self.tc_latent_dim, "prosody mix")
         else:
             tc = _dev_rows(tc_latent, "tc_latent")
         B, T = tc.shape[0] // K, tc.shape[1]
@@ -409,6 +411,37 @@ class MegaADM(pack.PlanMixin, nn.Module):
         raw = out[1] if return_raw else None
         dur = dur.unsqueeze(-1)
         return (dur, raw) if return_raw else dur
+
+    def infer_mix(self, tc_latents, weights, return_raw: bool = False):
+        """Duration interpolation: the ``infer`` decode of B utterances from a weighted mean of K sources' duration
+        predictions.  ``tc_latents``: K tensors (B, T, tc_dim), one per source (e.g. ``tc_latent`` of different prompts);
+        ``weights``: (K,) or (B, K), >= 0, each row with a positive sum (normalised per utterance).  All sources share one
+        raw-duration history; step t runs every source's ``infer`` step and feeds back r = sum_k w^_k y_k, the weighted
+        mean of their readouts; with exactly one positive weight in a row, r is that source's readout bit for bit
+        (include/megatts2_b200.h states the contract).  -> durations (B, T, 1) int32 [, raw (B, T) fp32 (the mixed values),
+        raw_src (K, B, T) fp32 (every source's readout)].  Replays as a CUDA graph whose inputs are the latents and the
+        weights, so new weight values need no new capture."""
+        _eval_only(self)
+        tc, w = _mix_sources(tc_latents, weights, self.tc_latent_dim, "duration mix")
+        K, (B, T, _) = len(tc_latents), tc_latents[0].shape
+        pl = self._plan_get(tc.device, T)
+        lib = L.lib()
+
+        def run(tc_, w_):
+            dur = torch.empty(B, T, dtype=torch.int32, device=tc_.device)
+            raw = torch.empty(B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
+            raw_src = torch.empty(K, B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
+            ws = ops.workspace(lib.mtts_adm_infer_mix_workspace_bytes(C.byref(pl.struct), K, B, T), tc_.device)
+            L.check(lib.mtts_adm_infer_mix_f32(C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
+                                               w_.data_ptr(), dur.data_ptr(), raw.data_ptr() if return_raw else None,
+                                               raw_src.data_ptr() if return_raw else None, ws.data_ptr(), ws.numel(),
+                                               ops._stream()))
+            return (dur, raw, raw_src) if return_raw else (dur,)
+
+        out = self._graphs().run(("adm_mix", pl.serial, K, B, T, bool(return_raw), tc.stride(0), tc.stride(1),
+                                  ops.launch_policy_now()), (tc, w), run)
+        dur = out[0].unsqueeze(-1)
+        return (dur, out[1], out[2]) if return_raw else dur
 
     def infer_causal(self, tc_latents: torch.Tensor, return_raw: bool = False):
         """OPT-IN causal KV-cache duration decode (SURVEY.md 8f-1) - NOT what the reference's ``infer`` computes:
@@ -676,7 +709,8 @@ class Megatts(nn.Module):
     def synthesize(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                    return_intermediates: bool = False, causal_decode: bool = False, prompt_mels: torch.Tensor = None,
                    return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None,
-                   sampling: S.Sampling = None, keys=None, prosody_mels=None, prosody_weights=None):
+                   sampling: S.Sampling = None, keys=None, prosody_mels=None, prosody_weights=None,
+                   duration_weights=None):
         """phone_tokens (B,Tp) int64, mels (B,Tm,80) prompt mel (frames-major) -> wav (B,1,256*(max sum d + 10)).
         Steps = models/megatts2.py:354-373; every utterance's result equals the reference's batch-1 run on it
         (utterances are independent; the only cross-utterance coupling would be the zero rows the LengthRegulator
@@ -706,12 +740,17 @@ class Megatts(nn.Module):
         ``prosody_mels`` (opt-in prosody interpolation): a list of (B, Tm_k, 80) prosody prompts, with ``prosody_weights``
         (K,) or (B, K), K = 1 + len(prosody_mels); weight 0 belongs to ``mels``.  Each prompt gives a source latent
         ``mrte.tc_latent(phone_tokens, prompt)``, length-regulated and max-pooled with the target's durations, and the
-        codes come from ``MegaPLM.infer_mix`` over the K sources.  The durations, the mel decoder and the vocoder keep
-        the target's (``mels``) latent, so the timbre stays the target's.  Not with ``causal_decode``."""
+        codes come from ``MegaPLM.infer_mix`` over the K sources.  The durations (unless ``duration_weights`` is given),
+        the mel decoder and the vocoder keep the target's (``mels``) latent, so the timbre stays the target's.  Not with
+        ``causal_decode``.
+        ``duration_weights`` (opt-in duration interpolation, with ``prosody_mels``): (K,) or (B, K), the same K; weight 0
+        belongs to ``mels``.  The durations then come from ``MegaADM.infer_mix`` over [the target's latent, *the prompts'
+        latents] instead of ``MegaADM.infer`` on the target's alone, so the rhythm moves toward the prompts as well; each
+        prompt's latent is computed once and serves both mixes.  ``forced_durations`` still override them."""
         dev = phone_tokens.device
-        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode)
+        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights)
         args = (phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt, sampling, keys,
-                prosody_mels, prosody_weights)
+                prosody_mels, prosody_weights, duration_weights)
         out = self._synthesize(*args)
         if check_range and _fp16_operands() and ops.tc_overflow(dev):
             _warn_fp16_range("re-running this batch on the bf16x3 engine")
@@ -731,10 +770,12 @@ class Megatts(nn.Module):
                 float(os.environ.get("MEGATTS2_REVOCODE_FRAC", str(REVOCODE_FRAC_DEFAULT))),
                 os.environ.get("MEGATTS2_REVOCODE_FROM", REVOCODE_FROM_DEFAULT))
 
-    def _check_prosody(self, phone_tokens, prosody_mels, prosody_weights, causal_decode):
+    def _check_prosody(self, phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights=None):
         if prosody_mels is None:
             if prosody_weights is not None:
                 raise L.MttsError("prosody_weights without prosody_mels")
+            if duration_weights is not None:
+                raise L.MttsError("duration_weights without prosody_mels")
             return
         if causal_decode:
             raise L.MttsError("prosody interpolation runs on the reference-faithful decode, not with causal_decode=True")
@@ -748,9 +789,11 @@ class Megatts(nn.Module):
             if m.dim() != 3 or m.shape[0] != B or m.shape[2] != nb or m.shape[1] < 1:
                 raise L.MttsError(f"prosody_mels[{k}]: expected ({B}, Tm, {nb}), got {tuple(m.shape)}")
         S.mix_weights(prosody_weights, 1 + len(prosody_mels), B)
+        if duration_weights is not None:
+            S.mix_weights(duration_weights, 1 + len(prosody_mels), B, "duration mix")
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
-                    sampling=None, keys=None, prosody_mels=None, prosody_weights=None):
+                    sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None):
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -782,13 +825,13 @@ class Megatts(nn.Module):
             with ops.launch_policy(nsm - V, pairs=False, pdl=True):
                 if start != "adm":
                     tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
-                dt = adm_decode(tc_latent)[..., 0]
+                dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights)
             main.wait_stream(side)
             pw_side.record_stream(main)
         else:
             tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
-            dt = adm_decode(tc_latent)[..., 0]
-        tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels)
+            dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights)
+        tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats)
         if prosody_mels is not None:
             tc8 = src[0]
             p_codes = self.plm.infer_mix(src, prosody_weights, sampling=sampling, keys=keys)
@@ -826,25 +869,35 @@ class Megatts(nn.Module):
         return dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
                     mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
 
-    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels):
+    def _durations(self, adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights):
+        """-> (dt (B, Tp) int32, the prompts' MRTE latents or None).  Without ``duration_weights``: ``adm_decode`` on
+        ``tc_latent``, and the prompts' latents are left to ``_plm_source``.  With them: MRTE on (phone_tokens, prompt) for
+        each prosody prompt, then ``MegaADM.infer_mix`` over [tc_latent, *those latents]."""
+        if duration_weights is None:
+            return adm_decode(tc_latent)[..., 0], None
+        lats = [self.generator.mrte.tc_latent(phone_tokens, m) for m in prosody_mels]
+        return self.adm.infer_mix([tc_latent] + lats, duration_weights)[..., 0], lats
+
+    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels, prosody_latents=None):
         """The synthesis front end between the ADM and the PLM: the durations (``forced_durations`` if given, else
         ``dt``) expand ``tc_latent`` to frames -> (tc_expand (B, Lmax, tc_dim), the per-utterance frame totals on the host
         (one host sync), the PLM's source).  The source is tc8, tc_expand max-pooled by 8, or with ``prosody_mels`` the
-        list [tc8, *one latent per prosody prompt]: MRTE on (phone_tokens, prompt), length-regulated with the same
-        durations to Lmax frames, max-pooled by 8."""
+        list [tc8, *one latent per prosody prompt]: MRTE on (phone_tokens, prompt) (or its ``prosody_latents`` entry when
+        the duration mix already computed it), length-regulated with the same durations to Lmax frames, max-pooled by 8."""
         d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
         tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
         tc8 = ops.maxpool_time(tc_expand, 8)
         if prosody_mels is None:
             return tc_expand, totals, tc8
         mrte, Lmax = self.generator.mrte, tc_expand.shape[1]
-        return tc_expand, totals, [tc8] + [
-            ops.maxpool_time(ops.length_regulate(mrte.tc_latent(phone_tokens, m), d_used, l_out=Lmax)[0], 8)
-            for m in prosody_mels]
+        lats = prosody_latents if prosody_latents is not None else (mrte.tc_latent(phone_tokens, m) for m in prosody_mels)
+        return tc_expand, totals, [tc8] + [ops.maxpool_time(ops.length_regulate(lat, d_used, l_out=Lmax)[0], 8)
+                                       for lat in lats]
 
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
-                          chunk_frames: int = 64, prosody_mels=None, prosody_weights=None, **unsupported):
+                          chunk_frames: int = 64, prosody_mels=None, prosody_weights=None, duration_weights=None,
+                          **unsupported):
         """``synthesize`` as a generator of waveform chunks, each yielded as soon as the prosody LM has decoded the codes
         its samples depend on.  Arguments as in ``synthesize``; ``chunk_frames`` mel frames (hop = 256 samples each) per
         chunk.  Each chunk is a dict: ``wav`` (B, 1, n) device tensor, ``offset`` (its first sample's index in the waveform
@@ -868,10 +921,10 @@ class Megatts(nn.Module):
                               "(the causal decode and the overlapped prompt re-vocode are not streamed)")
         if int(chunk_frames) < 1:
             raise L.MttsError(f"synthesize_stream: chunk_frames must be >= 1, got {chunk_frames}")
-        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False)
+        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False, duration_weights)
         guard = check_range and _fp16_operands()
         return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
-                                  int(chunk_frames), (prosody_mels, prosody_weights))
+                                  int(chunk_frames), (prosody_mels, prosody_weights, duration_weights))
 
     def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
                       prosody):
@@ -899,9 +952,9 @@ class Megatts(nn.Module):
         hd, hv = gen.decoder.receptive_field(), voc.receptive_field()
         with torch.no_grad(), scope():
             tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
-            dt = self.adm.infer(tc_latent)[..., 0]
-            prosody_mels, prosody_weights = prosody
-            tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels)
+            prosody_mels, prosody_weights, duration_weights = prosody
+            dt, lats = self._durations(self.adm.infer, tc_latent, phone_tokens, prosody_mels, duration_weights)
+            tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats)
             dec = self.plm.begin_decode(src, sampling=sampling, keys=keys, weights=prosody_weights)
             pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
         B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], dec.T

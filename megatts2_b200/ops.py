@@ -246,6 +246,26 @@ def mix_logprob_rows(logits, weights):
     return out
 
 
+def adm_readout_mix(xl, w_predict, weights):
+    """The duration mix of one ADM step: xl (K, B, D) fp32 (the last encoder row of source k of utterance b), w_predict
+    (D,) and weights (K,) or (B, K) -> (r (B,), y (K, B)): r_b = sum_k w^_k y_kb with y_kb = xl[k, b] . w_predict
+    (include/megatts2_b200.h, mtts_adm_readout_mix_f32)."""
+    from . import sampling as S
+    xl = _dev(xl, name="xl")
+    if xl.dim() != 3:
+        raise L.MttsError(f"xl: expected (K, B, D), got shape {tuple(xl.shape)}")
+    K, B, D = xl.shape
+    x = xl.contiguous()
+    w = _dev(w_predict, name="w_predict").contiguous()
+    if tuple(w.shape) != (D,):
+        raise L.MttsError(f"w_predict: expected ({D},), got shape {tuple(w.shape)}")
+    wt = S.mix_weights(weights, K, B, "duration mix").to(xl.device)
+    r = torch.empty(B, dtype=_F32, device=xl.device)
+    y = torch.empty(K, B, dtype=_F32, device=xl.device)
+    L.check(L.lib().mtts_adm_readout_mix_f32(_ptr(x), D, _ptr(w), K, B, _ptr(wt), _ptr(r), 1, _ptr(y), 1, _stream()))
+    return r, y
+
+
 def philox4x32_10(ctr, key):
     """The sampler's generator: ctr (n, 4) and key (n, 2) uint32 words, as int64 tensors holding values < 2**32, ->
     (n, 4) words (int64, values < 2**32)."""
@@ -426,6 +446,12 @@ def workspace(nbytes, device):
         assert buf.data_ptr() % 256 == 0
         _ws_cache[key] = buf
     return buf
+
+
+def workspace_buffers():
+    """The scratch buffers ``workspace`` hands out now.  A CUDA graph captured on one of them holds this tuple: it replays
+    on that address, so the buffer must outlive the graph even after ``workspace`` has grown past it."""
+    return tuple(_ws_cache.values())
 
 
 # ------------------------------------------------------------------------------ launch policy

@@ -69,29 +69,30 @@ class Sampling:
 MIX_MAX_SOURCES = 8
 
 
-def mix_weights(weights, K, B):
-    """The prosody-mix weights of ``MegaPLM.infer_mix`` as a validated (B, K) fp32 CPU tensor: ``weights`` is (K,) (the
-    same row for every utterance) or (B, K); every weight finite and >= 0, every row with a positive fp32 sum."""
+def mix_weights(weights, K, B, what="prosody mix"):
+    """The mix weights of ``MegaPLM.infer_mix`` and ``MegaADM.infer_mix`` as a validated (B, K) fp32 CPU tensor:
+    ``weights`` is (K,) (the same row for every utterance) or (B, K); every weight finite and >= 0, every row with a
+    positive fp32 sum.  ``what`` names the mix in the error messages."""
     if not 1 <= K <= MIX_MAX_SOURCES:
-        raise L.MttsError(f"prosody mix: K = {K} sources, expected 1 to {MIX_MAX_SOURCES}")
+        raise L.MttsError(f"{what}: K = {K} sources, expected 1 to {MIX_MAX_SOURCES}")
     try:
         w = torch.as_tensor(weights).detach()
     except (TypeError, ValueError, RuntimeError) as e:
-        raise L.MttsError(f"prosody mix: weights must be a (K,) or (B, K) array of real numbers ({e})") from None
+        raise L.MttsError(f"{what}: weights must be a (K,) or (B, K) array of real numbers ({e})") from None
     if w.dtype == torch.bool or w.is_complex() or not (w.is_floating_point() or w.dtype in (
             torch.int64, torch.int32, torch.int16, torch.int8, torch.uint8)):
-        raise L.MttsError(f"prosody mix: weights must be real numbers, got {w.dtype}")
+        raise L.MttsError(f"{what}: weights must be real numbers, got {w.dtype}")
     w64 = w.to(device="cpu", dtype=torch.float64)
     if w64.dim() == 1:
         w64 = w64.unsqueeze(0).expand(B, -1)
     if tuple(w64.shape) != (B, K):
-        raise L.MttsError(f"prosody mix: weights of shape {tuple(w.shape)}, expected ({K},) or ({B}, {K})")
+        raise L.MttsError(f"{what}: weights of shape {tuple(w.shape)}, expected ({K},) or ({B}, {K})")
     if not bool(torch.isfinite(w64).all()) or bool((w64 < 0).any()):
-        raise L.MttsError("prosody mix: every weight must be finite and >= 0")
+        raise L.MttsError(f"{what}: every weight must be finite and >= 0")
     w32 = w64.to(torch.float32).contiguous()
     s = w32.sum(1)
     if not bool(torch.isfinite(s).all()) or bool((s <= 0).any()):
-        raise L.MttsError("prosody mix: every weight row needs a positive, finite sum")
+        raise L.MttsError(f"{what}: every weight row needs a positive, finite sum")
     return w32
 
 
