@@ -523,6 +523,43 @@ int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_l
                                  void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * In-context prompting: the PLM decodes the target's codes as the continuation of prompt utterances' latents and codes,
+ * the sequences it is trained on (the reference's MegaPLMDataset prepends up to ten same-speaker cuts to every target).
+ * A context is P >= 0 rows: latents ctx_tc (Bc, P, tc_dim) and codes ctx_codes (Bc, P) int64 in [0, vq_bins), with Bc = 1
+ * (one context for every utterance: batch strides ctx_sb = ctx_codes_sb = 0) or B.  P is the same for every utterance of a
+ * call: there is no padding, since the encoder is unmasked and padding rows would change the result.  Target step j
+ * (0 <= j < T) is the reference loop's step P + j over the concatenated sequence:
+ *   latents [ctx_tc; tc[:, :j+1]] at positions 0 .. P+j of the sinusoidal table, codes [BOS, ctx_codes, c_0 .. c_{j-1}],
+ *   and the logits of the last row.
+ * That is MegaPLM.infer on cat(ctx_tc, tc) with the first P codes teacher-forced and only the last T steps decoded; P = 0
+ * is mtts_plm_infer_f32.  The causal form is the same under the causal mask: the teacher-forced MegaPLM.forward over the
+ * concatenation evaluated on its own output, which is what training optimises.  A sampled draw at target step j is keyed by
+ * (seed, keys[b], j), not P + j, so the same seed and key give the same noise with and without a context.  codes_out (B, T)
+ * and logits_out (optional, (B, T, vq_bins)) hold the target steps only.  The context latents and codes are read from
+ * device memory at every call, so a replayed CUDA graph picks up a new context of the same (Bc, P). */
+int64_t mtts_plm_infer_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T);
+/* The non-causal decode with a context (s NULL = greedy).  The pe table of m must have >= P + T rows. */
+int mtts_plm_infer_ctx_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
+                           const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes, int64_t ctx_codes_sb,
+                           int32_t P, int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
+                           int64_t workspace_bytes, void* stream);
+/* Target steps [j0, j1) of it against a caller-owned code state (B, P + T + 1) int64: column 0 holds BOS, columns 1..P the
+ * context codes (written by this call when j0 = 0), column P + 1 + j the code of target step j.  Any split of [0, T) into
+ * consecutive ranges yields the codes and logits of one mtts_plm_infer_ctx_f32 call.  Same workspace size. */
+int mtts_plm_infer_ctx_range_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                                 int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
+                                 int64_t ctx_codes_sb, int32_t P, int32_t j0, int32_t j1, int64_t* code_state,
+                                 int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
+                                 int64_t workspace_bytes, void* stream);
+/* The causal decode with a context.  The P context rows run through the stack once, as one teacher-forced causal pass of
+ * B*P rows per layer that fills the K/V caches of positions 0..P-1; T single-row steps from position P follow. */
+int64_t mtts_plm_decode_causal_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T);
+int mtts_plm_decode_causal_ctx_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                                   int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
+                                   int64_t ctx_codes_sb, int32_t P, int64_t* codes_out, float* logits_out,
+                                   const mtts_sampling* s, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Duration interpolation: the ADM decoded from a weighted mean of K prompts' duration predictions, the rhythm half of
  * Mega-TTS 2's prosody (the PLM mix above is the pitch and energy half).  Utterance b has K >= 1 sources; source k is a
  * latent tc^(k)[b] (T, tc_dim), source 0 conventionally the target prompt's, all with the same T, and b has a weight row

@@ -190,6 +190,14 @@ SIGNATURES = {
                                          i64, vp]),
     "mtts_plm_infer_mix_range_f32": (C.c_int, [C.POINTER(PLM), i32, vp, i64, i32, i32, i32, vp, i32, i32, vp, vp, vp,
                                                C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_plm_infer_ctx_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32, i32]),
+    "mtts_plm_infer_ctx_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, vp, vp,
+                                         C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_plm_infer_ctx_range_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, i32, i32,
+                                               vp, vp, vp, C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_plm_decode_causal_ctx_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32, i32]),
+    "mtts_plm_decode_causal_ctx_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, vp, vp,
+                                                 C.POINTER(Sampling), vp, i64, vp]),
     "mtts_convnet_workspace_bytes": (i64, [C.POINTER(ConvNet), i32, i32]),
     "mtts_convnet_forward_f32": (C.c_int, [C.POINTER(ConvNet), vp, i64, i32, vp, i64, i32, i32, i32, vp, i64, vp]),
     "mtts_convnet_double_out_len": (i32, [C.POINTER(ConvNetDouble), i32]),

@@ -116,9 +116,11 @@ static int64_t encoder_ws_floats(const mtts_encoder* e, int B, int T) {
   return M * (D + D + 3 * D + D + F) + 5 * 64;
 }
 
+// kv (optional): every layer's [k | v] rows are also written to kv + l * B * kv_T * 2D, a (B, kv_T, 2D) cache per layer
+// (rows 0..T-1), as the causal decode's prefill needs them.  With kv null the encoder enqueues nothing extra.
 static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int B, int T, const float* mask,
                            int64_t mask_sb, int64_t mask_sh, int64_t mask_sq, int last_row_only, Arena& ar,
-                           const TcScratch* tc, cudaStream_t st) {
+                           const TcScratch* tc, cudaStream_t st, float* kv = nullptr, int kv_T = 0) {
   const int D = e->d_model, H = e->n_heads, F = e->ff_dim, dh = D / H;
   MTTS_REQUIRE(D % H == 0, "d_model not divisible by n_heads");
   MTTS_REQUIRE(!(last_row_only && e->conv_ff), "last_row_only needs a linear feed-forward");
@@ -163,6 +165,9 @@ static int encoder_forward(const mtts_encoder* e, const float* x, float* y, int 
       MTTS_TRY(layernorm(xin, D, L.ln1_g, L.ln1_b, nullptr, 0, h, D, M, D, 1e-5f, 0, 0, st));
       MTTS_TRY(lin(e, tc, h, D, M, D, 3 * D, L.w_qkv, L.w_qkv_tc, L.b_qkv, nullptr, 0, qkv, 3 * D, 0, st));
     }
+    if (kv)
+      MTTS_TRY(copy_strided(qkv + D, (int64_t)T * 3 * D, 3 * D, 1, kv + (int64_t)l * B * kv_T * 2 * D, (int64_t)kv_T * 2 * D,
+                            2 * D, 1, B, T, 2 * D, 0, st));
     mtts_attn_params ap;
     memset(&ap, 0, sizeof(ap));
     ap.B = B; ap.H = H; ap.Tk = T; ap.dh = dh; ap.scale = scale;
@@ -276,38 +281,50 @@ static int64_t plm_ws_floats(const mtts_plm* m, int B, int T) {
 // reading the shared (B, T+1) code state.  Each step runs the encoder and the predict layer once over the K*B rows, then
 // mix_logprob_rows turns each utterance's K logits rows and its row of the (B, K) weights into l (B, V), and the pick
 // reads l.  logits_out, when given, is (K*B, T, V): the raw per-source logits.  K = 1 without weights is the plain decode.
+// Prompt context (ctx != nullptr, K = 1): the decode runs over N = P + T positions, the first P latent rows from ctx->tc
+// and the codes of columns 1..P of the (B, N+1) code state from ctx->codes (written here when t0 = 0).  t0, t1, codes_out,
+// logits_out and the sampler's step key stay in target steps: target step j is position P + j.  P = 0 is the plain decode.
+struct PlmCtx {
+  const float* tc; int64_t tc_sb; int tc_ld;           // (Bc, P, tc_dim); tc_sb = 0: one context for every utterance
+  const int64_t* codes; int64_t codes_sb;              // (Bc, P); codes_sb = 0 likewise
+  int P;
+};
 static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int t0, int t1,
                            int64_t* state, int64_t* codes_out, float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
-                           const mtts_sampling* smp, int K = 1, const float* weights = nullptr) {
+                           const mtts_sampling* smp, int K = 1, const float* weights = nullptr,
+                           const PlmCtx* ctx = nullptr) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
   MTTS_REQUIRE(0 <= t0 && t0 <= t1 && t1 <= (T > 0 ? T : 0), "step range outside [0, T]");
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
+  MTTS_REQUIRE(!ctx || (K == 1 && ctx->P >= 0 && (ctx->P == 0 || (ctx->tc && ctx->codes))), "bad context");
   if (weights) MTTS_TRY(mix_logprob_check(V, K));
   if (B <= 0 || T <= 0 || t0 == t1) return 0;
   const int R = K * B;                                       // latent rows: the K sources of the B utterances
+  const int P = ctx ? ctx->P : 0, N = P + T;                 // positions: the context rows, then the target's
   Arena top(ws, ws_bytes);
-  float* X = top.take<float>((int64_t)R * T * D);
+  float* X = top.take<float>((int64_t)R * N * D);
   float* xl = top.take<float>((int64_t)R * D);
   float* logits = top.take<float>((int64_t)R * V);
-  int64_t* codes = top.take<int64_t>((int64_t)R * (T + 1));
-  TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, (int64_t)R * T), (int64_t)R * T, tc_fmt_of_engine(m->enc.engine)};
+  int64_t* codes = top.take<int64_t>((int64_t)R * (N + 1));
+  TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, (int64_t)R * N), (int64_t)R * N, tc_fmt_of_engine(m->enc.engine)};
   if (tcs.bytes) tcs.p = top.take<char>(tcs.bytes);
   float* mixed = weights ? top.take<float>((int64_t)B * V) : nullptr;
   const int64_t enc_off = align_up(top.off, 256);
-  if (enc_off + encoder_ws_floats(&m->enc, R, T) * 4 > ws_bytes)
+  if (enc_off + encoder_ws_floats(&m->enc, R, N) * 4 > ws_bytes)
     return fail(MTTS_ERR_WORKSPACE, "%s: workspace too small (need %lld bytes)", "plm_infer",
-                enc_off + encoder_ws_floats(&m->enc, R, T) * 4);
+                enc_off + encoder_ws_floats(&m->enc, R, N) * 4);
   if (state) codes = state;
-  else MTTS_TRY(fill_i64(codes, T + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
-  for (int t = t0; t < t1; ++t) {
-    const int S = t + 1;
-    MTTS_TRY(plm_build_input(tc, tc_sb, tc_ld, m->tc_dim, codes, T + 1, B, m->pc_embedding, m->vq_dim, V + 2, m->pe,
-                             m->pe_alpha, R, S, X, st));
+  else MTTS_TRY(fill_i64(codes, N + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
+  if (P > 0 && t0 == 0) MTTS_TRY(copy_codes(ctx->codes, ctx->codes_sb, codes + 1, N + 1, B, P, st));
+  for (int j = t0; j < t1; ++j) {
+    const int t = P + j, S = t + 1;
+    MTTS_TRY(plm_build_input(tc, tc_sb, tc_ld, m->tc_dim, codes, N + 1, B, m->pc_embedding, m->vq_dim, V + 2, m->pe,
+                             m->pe_alpha, R, S, X, st, P ? ctx->tc : nullptr, P ? ctx->tc_sb : 0, P ? ctx->tc_ld : 0, P));
     Arena ar((char*)ws + enc_off, ws_bytes - enc_off);
     MTTS_TRY(encoder_forward(&m->enc, X, xl, R, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
-    float* lg = logits_out ? logits_out + (int64_t)t * V : logits;
+    float* lg = logits_out ? logits_out + (int64_t)j * V : logits;
     const int64_t lg_sb = logits_out ? (int64_t)T * V : V;
     mtts_conv_params p;
     memset(&p, 0, sizeof(p));
@@ -323,8 +340,8 @@ static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, in
       MTTS_TRY(mix_logprob_rows(lg, lg_sb, V, K, B, weights, mixed, V, st));
       pick_from = mixed; pick_ld = V;
     }
-    if (smp) MTTS_TRY(sample_rows(pick_from, pick_ld, V, B, t, *smp, codes + (t + 1), T + 1, codes_out + t, T, st));
-    else MTTS_TRY(argmax_rows(pick_from, pick_ld, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
+    if (smp) MTTS_TRY(sample_rows(pick_from, pick_ld, V, B, j, *smp, codes + (t + 1), N + 1, codes_out + j, T, st));
+    else MTTS_TRY(argmax_rows(pick_from, pick_ld, V, B, codes + (t + 1), N + 1, codes_out + j, T, st));
   }
   return 0;
 }
@@ -466,38 +483,72 @@ static int causal_step(const mtts_encoder* e, int B, int T, int t, const CausalB
   return 0;
 }
 
-static int64_t plm_causal_ws_floats(const mtts_plm* m, int B, int T) {
-  return causal_ws_floats(&m->enc, B, T) + (int64_t)B * m->vq_bins + 2 * ((int64_t)B * (T + 1) + 64) + 4 * 64;
+// the prefill of a P-row context: input rows, the causal mask, the pruned last layer's output, the encoder's own buffers
+// and the tensor-core scratch of B*P rows
+static int64_t plm_prefill_ws_floats(const mtts_plm* m, int B, int P) {
+  if (P <= 0) return 0;
+  const int64_t D = m->enc.d_model, M = (int64_t)B * P;
+  return M * D + (int64_t)P * P + (int64_t)B * D + encoder_ws_floats(&m->enc, B, P) + tc_scratch_bytes(&m->enc, M) / 4 +
+         6 * 64 + 1024;
 }
 
+static int64_t plm_causal_ws_floats(const mtts_plm* m, int B, int T, int P = 0) {
+  return causal_ws_floats(&m->enc, B, P + T) + (int64_t)B * m->vq_bins + 2 * ((int64_t)B * (P + T + 1) + 64) + 4 * 64 +
+         plm_prefill_ws_floats(m, B, P);
+}
+
+// Context (ctx != nullptr, P = ctx->P > 0): the P context rows go through the stack ONCE, as one teacher-forced causal pass
+// of B*P rows per layer (the full-sequence encoder with a causal mask: tensor-core GEMMs and the masked attention kernel),
+// which writes every layer's [k | v] for positions 0..P-1 into the caches; then T single-row steps from position P.
+// codes_out / logits_out and the sampler's step key are in target steps.
 static int plm_decode_causal(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int64_t* codes_out,
                              float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
-                             const mtts_sampling* smp = nullptr) {
+                             const mtts_sampling* smp = nullptr, const PlmCtx* ctx = nullptr) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
   MTTS_REQUIRE(!m->enc.conv_ff && D % m->enc.n_heads == 0, "needs a linear feed-forward encoder");
+  MTTS_REQUIRE(!ctx || (ctx->P >= 0 && (ctx->P == 0 || (ctx->tc && ctx->codes))), "bad context");
   if (B <= 0 || T <= 0) return 0;
+  const int P = ctx ? ctx->P : 0, N = P + T;
   Arena ar(ws, ws_bytes);
   float* logits = ar.take<float>((int64_t)B * V);
-  int64_t* codes = ar.take<int64_t>((int64_t)B * (T + 1));
+  int64_t* codes = ar.take<int64_t>((int64_t)B * (N + 1));
   CausalBufs cb;
-  MTTS_TRY(causal_take(&m->enc, B, T, ar, cb));
-  MTTS_TRY(fill_i64(codes, T + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
-  for (int t = 0; t < T; ++t) {
-    // row t of the input: cat(tc[:, t], emb[codes[:, t]]) + alpha * pe[t]   (megatts2.py:154-157)
-    MTTS_TRY(plm_build_input(tc + (int64_t)t * tc_ld, tc_sb, tc_ld, m->tc_dim, codes + t, T + 1, B, m->pc_embedding,
+  MTTS_TRY(causal_take(&m->enc, B, N, ar, cb));
+  MTTS_TRY(fill_i64(codes, N + 1, B, (int64_t)V, st));   // BOS = vq_bins (megatts2.py:170-171)
+  if (P > 0) {
+    MTTS_TRY(copy_codes(ctx->codes, ctx->codes_sb, codes + 1, N + 1, B, P, st));
+    const int64_t M = (int64_t)B * P;
+    float* X = ar.take<float>(M * D);
+    float* mask = ar.take<float>((int64_t)P * P);
+    float* yl = ar.take<float>((int64_t)B * D);
+    TcScratch tcs{nullptr, tc_scratch_bytes(&m->enc, M), M, tc_fmt_of_engine(m->enc.engine)};
+    if (tcs.bytes) tcs.p = ar.take<char>(tcs.bytes);
+    if (!ar.ok()) return fail(MTTS_ERR_WORKSPACE, "%s: workspace too small (need %lld bytes)", "causal prefill", ar.off);
+    Arena enc_ar((char*)ws + align_up(ar.off, 256), ws_bytes - align_up(ar.off, 256));
+    // rows 0..P-1: cat(ctx[:, s], emb[codes[:, s]]) + alpha * pe[s], codes = BOS, ctx codes 0..P-2
+    MTTS_TRY(plm_build_input(ctx->tc, ctx->tc_sb, ctx->tc_ld, m->tc_dim, codes, N + 1, B, m->pc_embedding, m->vq_dim, V + 2,
+                             m->pe, m->pe_alpha, B, P, X, st));
+    MTTS_TRY(causal_mask(mask, P, st));
+    // the last layer is pruned to the last row: the caches take every layer's k and v before its attention
+    MTTS_TRY(encoder_forward(&m->enc, X, yl, B, P, mask, 0, 0, P, 1, enc_ar, &tcs, st, cb.kv, N));
+  }
+  for (int j = 0; j < T; ++j) {
+    const int t = P + j;
+    // row t of the input: cat(tc[:, j], emb[codes[:, t]]) + alpha * pe[t]   (megatts2.py:154-157)
+    MTTS_TRY(plm_build_input(tc + (int64_t)j * tc_ld, tc_sb, tc_ld, m->tc_dim, codes + t, N + 1, B, m->pc_embedding,
                              m->vq_dim, V + 2, m->pe + (int64_t)t * D, m->pe_alpha, B, 1, cb.x, st));
-    MTTS_TRY(causal_step(&m->enc, B, T, t, cb, st));
-    float* lg = logits_out ? logits_out + (int64_t)t * V : logits;
+    MTTS_TRY(causal_step(&m->enc, B, N, t, cb, st));
+    float* lg = logits_out ? logits_out + (int64_t)j * V : logits;
     const int64_t lg_sb = logits_out ? (int64_t)T * V : V;
     mtts_conv_params p = linear_params(cb.x, D, m->w_predict, nullptr, lg, V, B, D, V);
     p.y_batch_stride = lg_sb;
     p.B = B; p.Tin = 1; p.Tout = 1; p.x_batch_stride = D;
     p.tc_scratch = cb.scratch; p.tc_scratch_bytes = cb.scratch_bytes;
     MTTS_TRY(conv1d(p, st));
-    if (smp) MTTS_TRY(sample_rows(lg, lg_sb, V, B, t, *smp, codes + (t + 1), T + 1, codes_out + t, T, st));
-    else MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), T + 1, codes_out + t, T, st));
+    if (smp) MTTS_TRY(sample_rows(lg, lg_sb, V, B, j, *smp, codes + (t + 1), N + 1, codes_out + j, T, st));
+    else MTTS_TRY(argmax_rows(lg, lg_sb, V, B, codes + (t + 1), N + 1, codes_out + j, T, st));
   }
   return 0;
 }
@@ -1017,6 +1068,44 @@ int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_l
   if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
                          workspace_bytes, (cudaStream_t)stream, s, K, weights);
+}
+
+int64_t mtts_plm_infer_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T) {
+  return plm_infer_ws_bytes(m, 1, B, P + T, false);
+}
+int mtts_plm_infer_ctx_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B, int32_t T,
+                           const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes, int64_t ctx_codes_sb,
+                           int32_t P, int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, &c);
+}
+int mtts_plm_infer_ctx_range_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                                 int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
+                                 int64_t ctx_codes_sb, int32_t P, int32_t j0, int32_t j1, int64_t* code_state,
+                                 int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
+                                 int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && code_state, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, j0, j1, code_state, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, &c);
+}
+int64_t mtts_plm_decode_causal_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T) {
+  return plm_causal_ws_floats(m, B, T, P > 0 ? P : 0) * 4 + 8192;
+}
+int mtts_plm_decode_causal_ctx_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                                   int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
+                                   int64_t ctx_codes_sb, int32_t P, int64_t* codes_out, float* logits_out,
+                                   const mtts_sampling* s, void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
+  return plm_decode_causal(m, tc_latent, tc_sb, tc_ld, B, T, codes_out, logits_out, workspace, workspace_bytes,
+                           (cudaStream_t)stream, s, &c);
 }
 
 int64_t mtts_adm_infer_workspace_bytes(const mtts_adm* m, int32_t B, int32_t T) { return adm_ws_floats(m, B, T) * 4 + 8192; }

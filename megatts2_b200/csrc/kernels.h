@@ -166,10 +166,16 @@ int mel_spectrogram(const float* wav, int64_t wav_sb, int B, int L, const int32_
                     const float* fb_w, const int32_t* fb_off, const int32_t* fb_start, int n_mels, float clamp_min,
                     float* out, int64_t out_sb, int64_t out_sm, int64_t out_sf, cudaStream_t st);
 // AR-loop helpers
-// latent row r reads code row r % B_codes (B_codes = B: one code row per latent row; fewer: sources sharing a history)
+// latent row r reads code row r % B_codes (B_codes = B: one code row per latent row; fewer: sources sharing a history).
+// With a context (P > 0), positions s < P read their latent from ctx (batch stride ctx_sb, 0 = one context for every row,
+// row stride ctx_ld) and positions s >= P read tc row s - P.
 int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const int64_t* codes, int codes_ld,
                     int B_codes, const float* emb, int vq_dim, int vocab, const float* pe, float alpha, int B, int S,
-                    float* X, cudaStream_t st);
+                    float* X, cudaStream_t st, const float* ctx = nullptr, int64_t ctx_sb = 0, int ctx_ld = 0, int P = 0);
+// y[b * ldy + p] = x[b * x_sb + p], p < n (int64 codes; x_sb = 0 broadcasts one row)
+int copy_codes(const int64_t* x, int64_t x_sb, int64_t* y, int64_t ldy, int B, int n, cudaStream_t st);
+// additive causal mask (T, T): 0 where key <= query, -inf above the diagonal
+int causal_mask(float* m, int T, cudaStream_t st);
 int argmax_rows(const float* x, int64_t ldx, int V, int rows, int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb,
                 cudaStream_t st);
 // opt-in sampler (sample.cu): validates s against V, then draws one code per row (argmax_rows when temperature == 0 or

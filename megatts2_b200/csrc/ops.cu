@@ -784,12 +784,13 @@ int mask_tail(float* x, int B, int rows, int L, const int32_t* keep, cudaStream_
 // ------------------------------------------------------------------------------------------
 // Autoregressive-loop helpers (device-resident state: no host sync inside the loops).
 
-// PLM step input (models/megatts2.py:173-175): X[b,s,:] = cat(tc[b,s,:], emb[codes[b,s]]) + alpha*pe[s]
+// PLM step input (models/megatts2.py:173-175): X[b,s,:] = cat(lat[b,s,:], emb[codes[b,s]]) + alpha*pe[s], where the latent
+// row lat[b,s] is ctx[b,s] for s < P (a prompt context) and tc[b,s-P] after it
 __global__ void plm_build_input_kernel(const float* __restrict__ tc, int64_t tc_sb, int tc_ld, int tc_dim,
                                        const int64_t* __restrict__ codes, int codes_ld, int B_codes,
                                        const float* __restrict__ emb, int vq_dim, int vocab,
                                        const float* __restrict__ pe, float alpha, int S, float* __restrict__ X,
-                                       int64_t total) {
+                                       int64_t total, const float* __restrict__ ctx, int64_t ctx_sb, int ctx_ld, int P) {
   pdl_entry();
   const int D = tc_dim + vq_dim;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -800,7 +801,7 @@ __global__ void plm_build_input_kernel(const float* __restrict__ tc, int64_t tc_
   const int b = (int)(bs / S);
   float v;
   if (d < tc_dim) {
-    v = tc[(int64_t)b * tc_sb + (int64_t)s * tc_ld + d];
+    v = s < P ? ctx[(int64_t)b * ctx_sb + (int64_t)s * ctx_ld + d] : tc[(int64_t)b * tc_sb + (int64_t)(s - P) * tc_ld + d];
   } else {
     int64_t id = codes[(int64_t)(b % B_codes) * codes_ld + s];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
@@ -811,12 +812,13 @@ __global__ void plm_build_input_kernel(const float* __restrict__ tc, int64_t tc_
 
 int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const int64_t* codes, int codes_ld,
                     int B_codes, const float* emb, int vq_dim, int vocab, const float* pe, float alpha, int B, int S,
-                    float* X, cudaStream_t st) {
+                    float* X, cudaStream_t st, const float* ctx, int64_t ctx_sb, int ctx_ld, int P) {
   const int64_t total = (int64_t)B * S * (tc_dim + vq_dim);
   if (total <= 0) return 0;
   MTTS_REQUIRE(B_codes >= 1, "B_codes must be >= 1");
+  MTTS_REQUIRE(P >= 0 && (P == 0 || ctx), "context rows without a context latent");
   launch_k(plm_build_input_kernel, (unsigned)cdiv64(total, 256), 256, 0, st, tc, tc_sb, tc_ld, tc_dim, codes, codes_ld,
-           B_codes, emb, vq_dim, vocab, pe, alpha, S, X, total);
+           B_codes, emb, vq_dim, vocab, pe, alpha, S, X, total, ctx, ctx_sb, ctx_ld, P);
   MTTS_CHECK_LAUNCH();
   return 0;
 }
@@ -853,6 +855,36 @@ int argmax_rows(const float* x, int64_t ldx, int V, int rows, int64_t* out_a, in
                 cudaStream_t st) {
   if (rows <= 0) return 0;
   launch_k(argmax_rows_kernel, (unsigned)cdiv64(rows, 4), 128, 0, st, x, ldx, V, rows, out_a, lda, out_b, ldb);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
+// y[b * ldy + p] = x[b * x_sb + p] for p < n: the context codes into a code state (x_sb = 0: one row for every b)
+__global__ void copy_codes_kernel(const int64_t* __restrict__ x, int64_t x_sb, int64_t* __restrict__ y, int64_t ldy, int B,
+                                  int n) {
+  pdl_entry();
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)B * n) return;
+  const int b = (int)(i / n), p = (int)(i % n);
+  y[(int64_t)b * ldy + p] = x[(int64_t)b * x_sb + p];
+}
+int copy_codes(const int64_t* x, int64_t x_sb, int64_t* y, int64_t ldy, int B, int n, cudaStream_t st) {
+  if (B <= 0 || n <= 0) return 0;
+  launch_k(copy_codes_kernel, (unsigned)cdiv64((int64_t)B * n, 256), 256, 0, st, x, x_sb, y, ldy, B, n);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
+// m (T, T): 0 on and below the diagonal, -inf above it (make_attn_mask's causal part, utils/utils.py:21-39)
+__global__ void causal_mask_kernel(float* m, int T) {
+  pdl_entry();
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)T * T) return;
+  m[i] = (int)(i % T) > (int)(i / T) ? -INFINITY : 0.0f;
+}
+int causal_mask(float* m, int T, cudaStream_t st) {
+  if (T <= 0) return 0;
+  launch_k(causal_mask_kernel, (unsigned)cdiv64((int64_t)T * T, 256), 256, 0, st, m, T);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

@@ -63,6 +63,76 @@ def _mix_sources(tc_latents, weights, dim, what):
     return torch.cat(tcs, 0), w
 
 
+class PLMContext:
+    """A prompt context for the prosody LM's in-context decode (include/megatts2_b200.h states the contract): P rows of
+    latents ``tc8`` (Bc, P, tc_dim) fp32 and their codes ``codes`` (Bc, P) int64 >= 0, on one CUDA device.  Bc is 1 (one
+    context for every utterance of a call) or the call's batch size.  This is what the reference's MegaPLMDataset prepends
+    to a target: a same-speaker cut's max-pooled MRTE latent and its VQ codes (``MegaG.plm_context`` makes one).  A list of
+    contexts, wherever one is taken, is joined along P in the order given (``PLMContext.cat``).  The codes are read to the
+    host once, here; the decode checks that they are below its ``vq_bins`` and that Bc fits its batch."""
+
+    def __init__(self, tc8, codes):
+        if not (isinstance(tc8, torch.Tensor) and tc8.dtype == torch.float32 and isinstance(codes, torch.Tensor)
+                and codes.dtype == torch.int64):
+            raise L.MttsError("PLMContext: tc8 must be a float32 tensor and codes an int64 tensor")
+        if tc8.dim() != 3 or codes.dim() != 2 or codes.shape != tc8.shape[:2] or tc8.shape[0] < 1:
+            raise L.MttsError(f"PLMContext: tc8 (Bc, P, tc_dim) and codes (Bc, P) with equal Bc >= 1 and P, got "
+                              f"{tuple(tc8.shape)} and {tuple(codes.shape)}")
+        if codes.device != tc8.device:
+            raise L.MttsError("PLMContext: tc8 and codes must be on one device")
+        lo, hi = torch.stack([codes.min(), codes.max()]).tolist() if codes.numel() else (0, -1)   # the one host read
+        if lo < 0:
+            raise L.MttsError(f"PLMContext: codes must be >= 0, got {lo}")
+        ops._dev(tc8, name="PLMContext.tc8")
+        self.tc8, self.codes, self.max_code = tc8.contiguous(), codes.contiguous(), hi
+
+    @property
+    def P(self):
+        return self.tc8.shape[1]
+
+    @staticmethod
+    def cat(contexts) -> "PLMContext":
+        """Contexts joined along P in the order given (their Bc all equal, or 1 and one other value)."""
+        cs = list(contexts)
+        if not cs or not all(isinstance(c, PLMContext) for c in cs):
+            raise L.MttsError("PLMContext.cat: expected a non-empty list of PLMContext")
+        if len(cs) == 1:
+            return cs[0]
+        Bc = max(c.tc8.shape[0] for c in cs)
+        if any(c.tc8.shape[0] not in (1, Bc) for c in cs) or len({c.tc8.shape[2] for c in cs}) != 1:
+            raise L.MttsError(f"PLMContext.cat: every Bc must be 1 or {Bc}, with one tc_dim")
+        if len({c.tc8.device for c in cs}) != 1:
+            raise L.MttsError("PLMContext.cat: the contexts must be on one device")
+        out = PLMContext.__new__(PLMContext)
+        out.tc8 = torch.cat([c.tc8.expand(Bc, -1, -1) for c in cs], 1).contiguous()
+        out.codes = torch.cat([c.codes.expand(Bc, -1) for c in cs], 1).contiguous()
+        out.max_code = max(c.max_code for c in cs)
+        return out
+
+
+def _context_inputs(context, B, tc_dim, vq_bins, device):
+    """``context`` (a PLMContext, a list of them, or None) checked against a decode of B utterances -> (tc8 (Bc, P, tc_dim),
+    codes (Bc, P)), or None."""
+    if context is None:
+        return None
+    c = PLMContext.cat(context if isinstance(context, (list, tuple)) else [context])
+    if c.tc8.shape[0] not in (1, B):
+        raise L.MttsError(f"context: Bc = {c.tc8.shape[0]}, expected 1 or B = {B}")
+    if c.tc8.shape[2] != tc_dim or c.tc8.device != device:
+        raise L.MttsError(f"context: latents (Bc, P, {tc_dim}) on {device}, got {tuple(c.tc8.shape)} on {c.tc8.device}")
+    if c.max_code >= vq_bins:
+        raise L.MttsError(f"context: codes must be in [0, {vq_bins}), got {c.max_code}")
+    return c.tc8, c.codes
+
+
+def _ctx_args(ctx):
+    """The context arguments of the mtts_plm_*_ctx_* entries; a batch stride of 0 broadcasts a Bc = 1 context."""
+    tc8, codes = ctx
+    one = tc8.shape[0] == 1
+    return (tc8.data_ptr(), 0 if one else tc8.stride(0), tc8.stride(1), codes.data_ptr(), 0 if one else codes.stride(0),
+            tc8.shape[1])
+
+
 def _ar_plan(model, enc, pos, struct, device, T, fill):
     """The weight plan of an AR model (MegaPLM / MegaADM), rebuilt when its weights or engine changed or when its
     positional table has fewer than T rows: the encoder ``enc``, then ``fill(plan, s)`` for the model's own fields of the
@@ -108,6 +178,28 @@ class MegaG(nn.Module):
         """(models/megatts2.py:76-84)"""
         _, _, _, codes = self.vqpe(mel_vqpe)
         return self.mrte.tc_latent(phone, phone_lens, mel_mrte), codes
+
+    def plm_context(self, phone, durations, mel_prompt, mel_timbre) -> PLMContext:
+        """The prosody LM context of prompt utterances: the reference dataset's ``read_latent`` (modules/datamodule.py:
+        163-178) applied to ``s2_latent``'s output, on the device.  phone (B, Tp) int64, durations (B, Tp) int, the
+        utterances' mel ``mel_prompt`` (B, Tm, mel_bins) and the timbre mel ``mel_timbre`` (B, Tt, mel_bins).  The latent
+        is ``mrte.tc_latent(phone, mel_timbre)`` length-regulated by ``durations`` and max-pooled by 8 (ceil); the codes are
+        the VQ prosody encoder's codes of ``mel_prompt[:, :sum(d)]``; both have ceil(sum(d) / 8) rows.  Every utterance
+        must have the same sum(d) (one host read), and mel_prompt at least that many frames."""
+        _eval_only(self)
+        d = torch.as_tensor(durations).to(phone.device, torch.int32)
+        tc = self.mrte.tc_latent(phone, mel_timbre)
+        tce, totals = ops.length_regulate(tc, d, return_host_totals=True)
+        if len(set(totals)) > 1:
+            raise L.MttsError(f"plm_context: every utterance needs the same sum(durations), got {totals}")
+        n = totals[0] if totals else 0
+        if mel_prompt.dim() != 3 or mel_prompt.shape[0] != phone.shape[0] or mel_prompt.shape[1] < n:
+            raise L.MttsError(f"plm_context: mel_prompt ({phone.shape[0]}, >= {n}, mel_bins) needed, got "
+                              f"{tuple(mel_prompt.shape)}")
+        if n == 0:
+            raise L.MttsError("plm_context: the durations sum to zero frames")
+        _, _, _, codes = self.vqpe(mel_prompt[:, :n].contiguous())
+        return PLMContext(ops.maxpool_time(tce, 8), codes[0])
 
     def decode_mel_cl(self, tc_latent_expand: torch.Tensor, p_codes: torch.Tensor) -> torch.Tensor:
         """Glue of Megatts.forward (models/megatts2.py:361-368): codes -> codebook rows repeated x8,
@@ -177,32 +269,44 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         logits = ops.linear(h, pack.pack_linear(self.predict_layer.weight))
         return logits, p_codes[:, 1:]
 
-    def infer(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None, keys=None):
+    def infer(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None, keys=None,
+              context=None):
         """Greedy AR decode, BOS = vq_bins, exactly T steps, NON-causal full recompute per step
         (models/megatts2.py:165-181).  tc_latent (B,T,tc_dim) -> (B,T) int64 [, (B,T,vq_bins) logits].
 
         ``sampling`` (opt-in, megatts2_b200.sampling.Sampling): each step's code is drawn on the device instead of the
         argmax, row b keyed by ``keys[b]`` (B 64-bit integers, default arange(B)); the returned logits stay the raw ones.
-        The seed and the keys are inputs of the replayed CUDA graph, so a new seed needs no new capture."""
+        The seed and the keys are inputs of the replayed CUDA graph, so a new seed needs no new capture.
+
+        ``context`` (opt-in in-context prompting; a ``PLMContext`` or a list of them, joined in order): the target is
+        decoded as the continuation of the context's P rows, as the model was trained: step j sees the latents
+        [context; tc_latent[:, :j+1]] at positions 0..P+j and the codes [BOS, context codes, c_0 .. c_{j-1}].  The codes
+        and logits are the target's only; a sampled step j draws the noise of ``infer``'s step j.  The context is a graph
+        input, so a new context of the same shape needs no new capture."""
         _eval_only(self)
         tc = _dev_rows(tc_latent, "tc_latent")
         B, T, _ = tc.shape
-        return self._decode(tc, 1, None, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits)
+        ctx = _context_inputs(context, B, self.tc_latent_dim, self.vq_bins, tc.device)
+        return self._decode(tc, 1, None, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits, ctx)
 
-    def _decode(self, tc, K, weights, smp, t0, t1, state, return_logits):
+    def _decode(self, tc, K, weights, smp, t0, t1, state, return_logits, ctx=None):
         """Steps [t0, t1) of the decode of B utterances from ``tc``, the (K*B, T, tc_dim) stack of K sources mixed by the
         (B, K) device ``weights`` (None: K = 1, the plain decode).  ``smp``: (sampling, seed, keys), or None for greedy.
         ``state`` None: the whole decode (t0 = 0, t1 = T) on the shared workspace; otherwise a range against that (B, T+1)
-        code state, on a private workspace since a captured range pins it.  The enqueues are device-only, so the call
-        replays as a CUDA graph from the second time on; ranges keep their graphs in a cache of their own, so streaming
-        never evicts the whole decodes'.  -> codes (B, t1 - t0) int64 [, logits (B, t1 - t0, V), or (K, B, t1 - t0, V)
-        when mixed]."""
+        code state, on a private workspace since a captured range pins it.  ``ctx``: (tc8 (Bc, P, tc_dim), codes (Bc, P)) of
+        a prompt context, or None; the steps stay target steps and the state is then (B, P+T+1).  The enqueues are
+        device-only, so the call replays as a CUDA graph from the second time on; ranges keep their graphs in a cache of
+        their own, so streaming never evicts the whole decodes'.  -> codes (B, t1 - t0) int64 [, logits (B, t1 - t0, V),
+        or (K, B, t1 - t0, V) when mixed]."""
         B, T, V = tc.shape[0] // K, tc.shape[1], self.vq_bins
         mix, ranged = weights is not None, state is not None
-        pl = self._plan_get(tc.device, T)
+        P = 0 if ctx is None else ctx[0].shape[1]
+        pl = self._plan_get(tc.device, P + T)
         lib = L.lib()
         m = C.byref(pl.struct)
-        if mix:        # the mix entries take the sampling as a nullable argument
+        if ctx is not None:   # so do the context entries
+            entry = lib.mtts_plm_infer_ctx_range_f32 if ranged else lib.mtts_plm_infer_ctx_f32
+        elif mix:        # the mix entries take the sampling as a nullable argument
             entry = lib.mtts_plm_infer_mix_range_f32 if ranged else lib.mtts_plm_infer_mix_f32
         elif smp is None:
             entry = lib.mtts_plm_infer_range_f32 if ranged else lib.mtts_plm_infer_f32
@@ -212,9 +316,11 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         def run(tc_, *rest):
             state_, rest = (rest[0], rest[1:]) if ranged else (None, rest)
             w_, rest = (rest[0], rest[1:]) if mix else (None, rest)
+            ctx_, rest = (rest[:2], rest[2:]) if ctx is not None else (None, rest)
             codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
             logits = torch.empty(K * B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
             nbytes = (lib.mtts_plm_infer_mix_workspace_bytes(m, K, B, T) if mix else
+                      lib.mtts_plm_infer_ctx_workspace_bytes(m, B, P, T) if ctx is not None else
                       lib.mtts_plm_infer_workspace_bytes(m, B, T))
             if ranged:
                 ws, ws_bytes = torch.empty(nbytes + 256, dtype=torch.uint8, device=tc_.device), nbytes
@@ -225,16 +331,19 @@ class MegaPLM(pack.PlanMixin, nn.Module):
             steps = (t0, t1, state_.data_ptr()) if ranged else ()
             outs = (codes.data_ptr(), logits.data_ptr() if return_logits else None)
             s = C.byref(smp[0].struct(*rest)) if smp is not None else None
-            if mix:
+            if ctx is not None:
+                args = (m,) + lat + _ctx_args(ctx_) + steps + outs + (s,)
+            elif mix:
                 args = (m, K) + lat + (w_.data_ptr(),) + steps + outs + (s,)
             else:
                 args = (m,) + lat + steps + outs + ((s,) if s is not None else ())
             L.check(entry(*args, ws.data_ptr(), ws_bytes, ops._stream()))
             return (codes[:, t0:t1], logits[:, t0:t1]) if return_logits else (codes[:, t0:t1],)
 
-        inputs = (tc,) + ((state,) if ranged else ()) + ((weights,) if mix else ()) + (smp[1:] if smp is not None else ())
+        inputs = ((tc,) + ((state,) if ranged else ()) + ((weights,) if mix else ()) + (tuple(ctx) if ctx is not None else ())
+                  + (smp[1:] if smp is not None else ()))
         key = (pl.serial, K, mix, B, T, t0, t1, bool(return_logits), tc.stride(0), tc.stride(1), ops.launch_policy_now(),
-               None if smp is None else smp[0].graph_key())
+               None if smp is None else smp[0].graph_key(), None if ctx is None else (ctx[0].shape[0], P))
         out = self._graphs("range" if ranged else "main").run(key, inputs, run)
         if not return_logits:
             return out[0]
@@ -254,21 +363,28 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
         return self._decode(tc, K, w, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits)
 
-    def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None) -> "PLMDecode":
+    def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None, context=None) -> "PLMDecode":
         """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
-        any number of ranges gives ``infer``'s codes and logits (same ``sampling`` and ``keys``).  With ``weights``,
-        ``tc_latent`` is the list of K sources of ``infer_mix`` and the ranges give ``infer_mix``'s codes and logits."""
+        any number of ranges gives ``infer``'s codes and logits (same ``sampling``, ``keys`` and ``context``).  With
+        ``weights``, ``tc_latent`` is the list of K sources of ``infer_mix`` and the ranges give ``infer_mix``'s codes and
+        logits (not with a context)."""
         _eval_only(self)
         K, w = 1, None
         if weights is not None:
+            if context is not None:
+                raise L.MttsError("begin_decode: a context does not combine with prosody mix weights")
             K = len(tc_latent)
             tc, w = _mix_sources(tc_latent, weights, self.tc_latent_dim, "prosody mix")
         else:
             tc = _dev_rows(tc_latent, "tc_latent")
         B, T = tc.shape[0] // K, tc.shape[1]
-        state = torch.full((B, T + 1), self.vq_bins, dtype=torch.int64, device=tc.device)   # column 0 = BOS
+        ctx = _context_inputs(context, B, self.tc_latent_dim, self.vq_bins, tc.device)
+        P = 0 if ctx is None else ctx[0].shape[1]
+        state = torch.full((B, P + T + 1), self.vq_bins, dtype=torch.int64, device=tc.device)   # column 0 = BOS
+        if P:
+            state[:, 1:P + 1] = ctx[1]
         smp = _sampling_inputs(sampling, keys, B, tc.device) or (None, None, None)
-        return PLMDecode(tc, state, *smp, w)
+        return PLMDecode(tc, state, *smp, w, ctx)
 
     def decode_until(self, dec: "PLMDecode", t1: int, return_logits: bool = False):
         """Run steps [dec.t, t1) of the decode begun by ``begin_decode`` -> the new codes (B, t1 - dec.t) int64 [, their
@@ -285,34 +401,47 @@ class MegaPLM(pack.PlanMixin, nn.Module):
             lg_shape = (B, 0, self.vq_bins) if dec.weights is None else (dec.K, B, 0, self.vq_bins)
             return (codes, torch.empty(*lg_shape, device=dec.tc.device)) if return_logits else codes
         smp = None if dec.sampling is None else (dec.sampling, dec.seed, dec.keys)
-        out = self._decode(dec.tc, dec.K, dec.weights, smp, t0, t1, dec.state, return_logits)
+        out = self._decode(dec.tc, dec.K, dec.weights, smp, t0, t1, dec.state, return_logits, dec.ctx)
         # a replay advanced the graph's copy of the state, not dec.state
-        dec.state[:, t0 + 1:t1 + 1].copy_(out[0] if return_logits else out)
+        dec.target[:, t0:t1].copy_(out[0] if return_logits else out)
         dec.t = t1
         return out
 
     def infer_causal(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None,
-                     keys=None):
+                     keys=None, context=None):
         """OPT-IN causal KV-cache greedy decode (SURVEY.md 8f-1) - NOT what the reference's ``infer`` computes.
 
         ``infer`` re-runs the stack bidirectionally every step (models/megatts2.py:177); this decode follows the
         *training* semantics of ``forward`` (causal=True, models/megatts2.py:158): row t attends to rows <= t, so
         each step computes one row per utterance against per-layer K/V caches (O(T) instead of O(T^2)).  Its
         logits equal the teacher-forced ``forward`` logits evaluated on its own output.  Same I/O as ``infer``,
-        ``sampling`` and ``keys`` included (the same noise as ``infer`` for a given seed, key and step)."""
+        ``sampling`` and ``keys`` included (the same noise as ``infer`` for a given seed, key and step).
+
+        ``context`` (as in ``infer``): the causal form of the in-context decode.  The context's P rows run through the stack
+        once, as one teacher-forced causal pass that fills the K/V caches, then T single-row steps follow; the logits
+        equal the teacher-forced ``forward`` over [context; target] at the decoded codes."""
         _eval_only(self)
         tc = _dev_rows(tc_latent, "tc_latent")
         B, T, _ = tc.shape
-        pl = self._plan_get(tc.device, T)
+        ctx = _context_inputs(context, B, self.tc_latent_dim, self.vq_bins, tc.device)
+        P = 0 if ctx is None else ctx[0].shape[1]
+        pl = self._plan_get(tc.device, P + T)
         lib = L.lib()
+        m = C.byref(pl.struct)
         codes = torch.empty(B, T, dtype=torch.int64, device=tc.device)
         logits = torch.empty(B, T, self.vq_bins, dtype=torch.float32, device=tc.device) if return_logits else None
-        ws = ops.workspace(lib.mtts_plm_decode_causal_workspace_bytes(C.byref(pl.struct), B, T), tc.device)
         smp = _sampling_inputs(sampling, keys, B, tc.device)     # held until the call: the struct points into it
+        s = None if smp is None else C.byref(sampling.struct(*smp[1:]))
+        lat = (tc.data_ptr(), tc.stride(0), tc.stride(1), B, T)
+        outs = (codes.data_ptr(), logits.data_ptr() if return_logits else None)
+        if ctx is not None:
+            ws = ops.workspace(lib.mtts_plm_decode_causal_ctx_workspace_bytes(m, B, P, T), tc.device)
+            L.check(lib.mtts_plm_decode_causal_ctx_f32(m, *lat, *_ctx_args(ctx), *outs, s, ws.data_ptr(), ws.numel(),
+                                                       ops._stream()))
+            return (codes, logits) if return_logits else codes
+        ws = ops.workspace(lib.mtts_plm_decode_causal_workspace_bytes(m, B, T), tc.device)
         entry = lib.mtts_plm_decode_causal_f32 if smp is None else lib.mtts_plm_decode_causal_sample_f32
-        s = () if smp is None else (C.byref(sampling.struct(*smp[1:])),)
-        L.check(entry(C.byref(pl.struct), tc.data_ptr(), tc.stride(0), tc.stride(1), B, T, codes.data_ptr(),
-                      logits.data_ptr() if return_logits else None, *s, ws.data_ptr(), ws.numel(), ops._stream()))
+        L.check(entry(m, *lat, *outs, *(() if s is None else (s,)), ws.data_ptr(), ws.numel(), ops._stream()))
         return (codes, logits) if return_logits else codes
 
     @classmethod
@@ -326,21 +455,28 @@ class MegaPLM(pack.PlanMixin, nn.Module):
 
 class PLMDecode:
     """State of one resumable PLM decode (``MegaPLM.begin_decode``): the latent ``tc`` (B, T, tc_dim), the code state
-    (B, T+1) int64 (column 0 = BOS, column t+1 = the code of step t once decoded), the sampling parameters with the seed
-    and row keys as device tensors (None for greedy), and ``t``, the number of steps decoded.  A mixed decode also holds
-    the (B, K) device ``weights``, and ``tc`` is then the (K*B, T, tc_dim) stack of its K sources."""
+    (B, P+T+1) int64 (column 0 = BOS, columns 1..P the context's codes, column P+1+t the code of target step t once
+    decoded), the sampling parameters with the seed and row keys as device tensors (None for greedy), and ``t``, the number
+    of target steps decoded.  A mixed decode also holds the (B, K) device ``weights``, and ``tc`` is then the (K*B, T,
+    tc_dim) stack of its K sources; a decode with a context holds ``ctx`` = (tc8 (Bc, P, tc_dim), codes (Bc, P)) and P."""
 
-    def __init__(self, tc, state, sampling, seed, keys, weights=None):
+    def __init__(self, tc, state, sampling, seed, keys, weights=None, ctx=None):
         self.tc, self.state, self.sampling, self.seed, self.keys = tc, state, sampling, seed, keys
-        self.weights = weights
+        self.weights, self.ctx = weights, ctx
         self.K = 1 if weights is None else weights.shape[1]
+        self.P = 0 if ctx is None else ctx[0].shape[1]
         self.B, self.T = state.shape[0], tc.shape[1]
         self.t = 0
 
     @property
+    def target(self):
+        """The target's code columns of the state, (B, T) (a view; columns >= t are not decoded yet)."""
+        return self.state[:, self.P + 1:]
+
+    @property
     def codes(self):
         """The codes decoded so far, (B, t) (a view of the state)."""
-        return self.state[:, 1:self.t + 1]
+        return self.target[:, :self.t]
 
 
 class MegaADM(pack.PlanMixin, nn.Module):
@@ -710,7 +846,7 @@ class Megatts(nn.Module):
                    return_intermediates: bool = False, causal_decode: bool = False, prompt_mels: torch.Tensor = None,
                    return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None,
                    sampling: S.Sampling = None, keys=None, prosody_mels=None, prosody_weights=None,
-                   duration_weights=None):
+                   duration_weights=None, plm_context=None):
         """phone_tokens (B,Tp) int64, mels (B,Tm,80) prompt mel (frames-major) -> wav (B,1,256*(max sum d + 10)).
         Steps = models/megatts2.py:354-373; every utterance's result equals the reference's batch-1 run on it
         (utterances are independent; the only cross-utterance coupling would be the zero rows the LengthRegulator
@@ -746,11 +882,16 @@ class Megatts(nn.Module):
         ``duration_weights`` (opt-in duration interpolation, with ``prosody_mels``): (K,) or (B, K), the same K; weight 0
         belongs to ``mels``.  The durations then come from ``MegaADM.infer_mix`` over [the target's latent, *the prompts'
         latents] instead of ``MegaADM.infer`` on the target's alone, so the rhythm moves toward the prompts as well; each
-        prompt's latent is computed once and serves both mixes.  ``forced_durations`` still override them."""
+        prompt's latent is computed once and serves both mixes.  ``forced_durations`` still override them.
+        ``plm_context`` (opt-in in-context prompting): a ``PLMContext`` (or a list of them, joined in order), e.g. from
+        ``generator.plm_context`` on same-speaker prompt utterances; the prosody codes come from ``MegaPLM.infer`` (or
+        ``infer_causal`` with ``causal_decode``) with ``context=plm_context``, so the target continues the prompts'
+        prosody as in training.  The durations, the mel decoder and the vocoder see the target only.  Not with
+        ``prosody_mels``."""
         dev = phone_tokens.device
-        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights)
+        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights, plm_context)
         args = (phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt, sampling, keys,
-                prosody_mels, prosody_weights, duration_weights)
+                prosody_mels, prosody_weights, duration_weights, plm_context)
         out = self._synthesize(*args)
         if check_range and _fp16_operands() and ops.tc_overflow(dev):
             _warn_fp16_range("re-running this batch on the bf16x3 engine")
@@ -770,7 +911,11 @@ class Megatts(nn.Module):
                 float(os.environ.get("MEGATTS2_REVOCODE_FRAC", str(REVOCODE_FRAC_DEFAULT))),
                 os.environ.get("MEGATTS2_REVOCODE_FROM", REVOCODE_FROM_DEFAULT))
 
-    def _check_prosody(self, phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights=None):
+    def _check_prosody(self, phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights=None,
+                       plm_context=None):
+        if plm_context is not None and prosody_mels is not None:
+            raise L.MttsError("plm_context does not combine with prosody_mels: the mixed sources would need one code "
+                              "history with one context length")
         if prosody_mels is None:
             if prosody_weights is not None:
                 raise L.MttsError("prosody_weights without prosody_mels")
@@ -793,7 +938,8 @@ class Megatts(nn.Module):
             S.mix_weights(duration_weights, 1 + len(prosody_mels), B, "duration mix")
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
-                    sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None):
+                    sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None,
+                    plm_context=None):
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -837,7 +983,7 @@ class Megatts(nn.Module):
             p_codes = self.plm.infer_mix(src, prosody_weights, sampling=sampling, keys=keys)
         else:
             tc8 = src
-            p_codes = plm_decode(src, sampling=sampling, keys=keys)
+            p_codes = plm_decode(src, sampling=sampling, keys=keys, context=plm_context)
         B, Lmax = tc_expand.shape[0], tc_expand.shape[1]
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]
@@ -897,7 +1043,7 @@ class Megatts(nn.Module):
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
                           chunk_frames: int = 64, prosody_mels=None, prosody_weights=None, duration_weights=None,
-                          **unsupported):
+                          plm_context=None, **unsupported):
         """``synthesize`` as a generator of waveform chunks, each yielded as soon as the prosody LM has decoded the codes
         its samples depend on.  Arguments as in ``synthesize``; ``chunk_frames`` mel frames (hop = 256 samples each) per
         chunk.  Each chunk is a dict: ``wav`` (B, 1, n) device tensor, ``offset`` (its first sample's index in the waveform
@@ -921,10 +1067,10 @@ class Megatts(nn.Module):
                               "(the causal decode and the overlapped prompt re-vocode are not streamed)")
         if int(chunk_frames) < 1:
             raise L.MttsError(f"synthesize_stream: chunk_frames must be >= 1, got {chunk_frames}")
-        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False, duration_weights)
+        self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False, duration_weights, plm_context)
         guard = check_range and _fp16_operands()
         return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
-                                  int(chunk_frames), (prosody_mels, prosody_weights, duration_weights))
+                                  int(chunk_frames), (prosody_mels, prosody_weights, duration_weights, plm_context))
 
     def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
                       prosody):
@@ -952,10 +1098,10 @@ class Megatts(nn.Module):
         hd, hv = gen.decoder.receptive_field(), voc.receptive_field()
         with torch.no_grad(), scope():
             tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
-            prosody_mels, prosody_weights, duration_weights = prosody
+            prosody_mels, prosody_weights, duration_weights, plm_context = prosody
             dt, lats = self._durations(self.adm.infer, tc_latent, phone_tokens, prosody_mels, duration_weights)
             tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats)
-            dec = self.plm.begin_decode(src, sampling=sampling, keys=keys, weights=prosody_weights)
+            dec = self.plm.begin_decode(src, sampling=sampling, keys=keys, weights=prosody_weights, context=plm_context)
             pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
         B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], dec.T
         if Lmax < 1:
@@ -991,7 +1137,7 @@ class Megatts(nn.Module):
             wav = torch.zeros(B, 1, n, dtype=torch.float32, device=dev)
             for (rows, win), idx in groups(k, lambda c: (c.rows, c.dec) if c.dec is not None else None):
                 (r0, r1), (da, db) = rows, win
-                m = gen.decode_mel_cl(tc_expand[idx, da:db].contiguous(), dec.state[idx, 1 + da // 8:1 + -(-db // 8)])
+                m = gen.decode_mel_cl(tc_expand[idx, da:db].contiguous(), dec.target[idx, da // 8:-(-db // 8)])
                 mel[idx, r0:r1] = m[:, r0 - da:r1 - da]
             for (p0, p1, va, vb), idx in groups(k, lambda c: (c.p0, c.p1) + c.voc):
                 w = self.hifi_gan.decode_batch_cl(mel[idx, va:vb])
@@ -1018,7 +1164,7 @@ class Megatts(nn.Module):
             valid = [0 if pl[k] is None else hop * (pl[k].p1 - pl[k].p0) for pl in plans]
             chunk = dict(wav=wav, offset=off0 + hop * P[k], valid=valid, last=k == K - 1)
             if k == K - 1:
-                chunk.update(p_codes=dec.state[:, 1:].clone(), dt=dt, mel=mel,
+                chunk.update(p_codes=dec.target.clone(), dt=dt, mel=mel,
                              wav_lens=[hop * (t + 2 * pad) + off0 for t in totals])
             yield chunk
 
@@ -1030,8 +1176,8 @@ class Megatts(nn.Module):
         Returns a list of 1-D waveforms (valid samples only), in input order.  With ``sampling``, utterance i is keyed
         by its index i in ``items``, so the bucketing and ``max_batch`` do not change what it draws.  Prosody prompts
         (``prosody_mels``) are not taken here: call ``synthesize`` per batch."""
-        if "prosody_mels" in kw or "prosody_weights" in kw:
-            raise L.MttsError("synthesize_many does not take prosody prompts; call synthesize per batch")
+        if "prosody_mels" in kw or "prosody_weights" in kw or "plm_context" in kw:
+            raise L.MttsError("synthesize_many does not take prosody prompts or a PLM context; call synthesize per batch")
         if sampling is not None:
             kw["sampling"] = sampling
         buckets = {}
