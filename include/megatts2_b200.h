@@ -523,6 +523,42 @@ int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_l
                                  void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Prosody and duration schedules: mix weights that change along the utterance.  The weights are an array W (B, T, K) fp32
+ * on the device, row (b, t) at W + b*w_sb + t*w_st (K contiguous floats; w_sb, w_st >= 0).  Target step t of utterance b
+ * runs the mix above with row (b, t) in place of the utterance's one row: the PLM picks c_t from
+ * l = log sum_k w^_{b,t,k} softmax(z^(k)), the ADM feeds back r = sum_k w^_{b,t,k} y^(k), each row normalised, checked
+ * and applied exactly as the per-utterance row is (a row with one positive weight gives that source's raw logits row or
+ * readout, bit for bit).  w_st = 0 and w_sb = K is the (B, K) mix: the per-utterance entries are these with those
+ * strides, and their launch sequences are the same.  Same workspace sizes as the per-utterance entries.
+ *
+ * Per-phone weights (B, Tp, K) become PLM step weights by mtts_mix_step_weights_f32, with the phone durations that the
+ * length regulator uses (negative durations count as 0).  PLM step t covers the mel frames [8t, 8t+8) of [0, L_b),
+ * L_b = sum of b's durations, and takes the weight row of the phone that owns the most of those frames, the earlier
+ * phone on a tie; zero-duration phones own no frames.  A step at or past L_b (the steps of a shorter utterance in a batch
+ * of T = ceil(max L_b / 8) steps) takes the row of b's last phone with a positive duration, or phone 0 if none has one.
+ * So prosody changes are quantised to the PLM's 8-frame steps (128 ms at 16 kHz, hop 256).  The rule is integer-only and
+ * the rows are copied as bits, so the expansion is exact.  The ADM's steps are the phones themselves: per-phone duration
+ * weights go to mtts_adm_infer_mix_steps_f32 as they are, T = Tp. */
+
+/* mtts_plm_infer_mix_f32 / mtts_plm_infer_mix_range_f32 with weights (B, T, K) at strides (w_sb, w_st).  In a range,
+ * target step j reads row j, so any split of [0, T) into consecutive ranges yields the codes and logits of the whole
+ * decode.  K in 1..8 (MTTS_ERR_UNSUPPORTED above 8); weights must not be NULL. */
+int mtts_plm_infer_mix_steps_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                 int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st,
+                                 int64_t* codes_out, float* logits_out, const mtts_sampling* s,
+                                 void* workspace, int64_t workspace_bytes, void* stream);
+int mtts_plm_infer_mix_steps_range_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb,
+                                       int32_t tc_ld, int32_t B, int32_t T, const float* weights, int64_t w_sb,
+                                       int64_t w_st, int32_t t0, int32_t t1, int64_t* code_state, int64_t* codes_out,
+                                       float* logits_out, const mtts_sampling* s, void* workspace,
+                                       int64_t workspace_bytes, void* stream);
+/* The phone -> PLM step rule above: phone_w (B, Tp, K) device, utterance b at phone_w + b*pw_sb, phone rows K floats
+ * apart; durations (B, Tp) int32 device, utterance b at durations + b*dur_sb; out (B, T, K) contiguous.  One CTA per
+ * utterance.  1 <= K <= 8 and 1 <= Tp <= 8192 (MTTS_ERR_UNSUPPORTED above the bounds); B <= 0 or T <= 0 does nothing. */
+int mtts_mix_step_weights_f32(const float* phone_w, int64_t pw_sb, int32_t Tp, int32_t K, int32_t B,
+                              const int32_t* durations, int64_t dur_sb, int32_t T, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * In-context prompting: the PLM decodes the target's codes as the continuation of prompt utterances' latents and codes,
  * the sequences it is trained on (the reference's MegaPLMDataset prepends up to ten same-speaker cuts to every target).
  * A context is P >= 0 rows: latents ctx_tc (Bc, P, tc_dim) and codes ctx_codes (Bc, P) int64 in [0, vq_bins), with Bc = 1
@@ -595,6 +631,12 @@ int64_t mtts_adm_infer_mix_workspace_bytes(const mtts_adm* m, int32_t K, int32_t
 int mtts_adm_infer_mix_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
                            int32_t B, int32_t T, const float* weights, int32_t* dur_out, float* raw_out,
                            float* raw_src_out, void* workspace, int64_t workspace_bytes, void* stream);
+/* mtts_adm_infer_mix_f32 with weights (B, T, K) at strides (w_sb, w_st), T = Tp: step t, the duration of phone t, mixes
+ * by row t (the schedule section above states the rule).  weights must not be NULL. */
+int mtts_adm_infer_mix_steps_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                 int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st,
+                                 int32_t* dur_out, float* raw_out, float* raw_src_out, void* workspace,
+                                 int64_t workspace_bytes, void* stream);
 
 /* ConvNet family (modules/convnet.py).  One ConvBlock = ReLU -> Conv1d(C,C,k,same) -> LN(C). */
 typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv_block;   /* w packed (k,C,C); w_tc (3,k,C,C) bf16 or NULL */

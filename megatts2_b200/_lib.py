@@ -171,6 +171,8 @@ SIGNATURES = {
     "mtts_adm_readout_mix_f32": (C.c_int, [vp, i32, vp, i32, i32, vp, vp, i64, vp, i64, vp]),
     "mtts_adm_infer_mix_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32, i32]),
     "mtts_adm_infer_mix_f32": (C.c_int, [C.POINTER(ADM), i32, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp]),
+    "mtts_adm_infer_mix_steps_f32": (C.c_int, [C.POINTER(ADM), i32, vp, i64, i32, i32, i32, vp, i64, i64, vp, vp, vp, vp,
+                                               i64, vp]),
     "mtts_plm_decode_causal_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32]),
     "mtts_plm_decode_causal_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
     "mtts_adm_decode_causal_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32]),
@@ -190,6 +192,11 @@ SIGNATURES = {
                                          i64, vp]),
     "mtts_plm_infer_mix_range_f32": (C.c_int, [C.POINTER(PLM), i32, vp, i64, i32, i32, i32, vp, i32, i32, vp, vp, vp,
                                                C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_plm_infer_mix_steps_f32": (C.c_int, [C.POINTER(PLM), i32, vp, i64, i32, i32, i32, vp, i64, i64, vp, vp,
+                                               C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_plm_infer_mix_steps_range_f32": (C.c_int, [C.POINTER(PLM), i32, vp, i64, i32, i32, i32, vp, i64, i64, i32, i32,
+                                                     vp, vp, vp, C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_mix_step_weights_f32": (C.c_int, [vp, i64, i32, i32, i32, vp, i64, i32, vp, vp]),
     "mtts_plm_infer_ctx_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32, i32]),
     "mtts_plm_infer_ctx_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, vp, vp,
                                          C.POINTER(Sampling), vp, i64, vp]),

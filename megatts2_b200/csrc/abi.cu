@@ -120,7 +120,12 @@ int mtts_attention_tc_f32(const mtts_attn_params* p, void* stream) {
 
 int mtts_adm_readout_mix_f32(const float* xl, int32_t D, const float* w_predict, int32_t K, int32_t B, const float* weights,
                              float* out, int64_t ld_out, float* y_out, int64_t ld_y, void* stream) {
-  return adm_readout_mix(xl, D, w_predict, K, B, weights, out, ld_out, y_out, ld_y, (cudaStream_t)stream);
+  return adm_readout_mix(xl, D, w_predict, K, B, weights, K, out, ld_out, y_out, ld_y, (cudaStream_t)stream);
+}
+
+int mtts_mix_step_weights_f32(const float* phone_w, int64_t pw_sb, int32_t Tp, int32_t K, int32_t B,
+                              const int32_t* durations, int64_t dur_sb, int32_t T, float* out, void* stream) {
+  return mix_step_weights(phone_w, pw_sb, Tp, K, B, durations, dur_sb, T, out, (cudaStream_t)stream);
 }
 
 int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t rows, int32_t step, const mtts_sampling* s,
@@ -131,7 +136,7 @@ int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t row
 
 int mtts_mix_logprob_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t K, int32_t B, const float* weights,
                               float* out, int64_t ld_out, void* stream) {
-  return mix_logprob_rows(logits, ld, V, K, B, weights, out, ld_out, (cudaStream_t)stream);
+  return mix_logprob_rows(logits, ld, V, K, B, weights, K, out, ld_out, (cudaStream_t)stream);
 }
 
 int mtts_philox4x32_10_u32(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, void* stream) {

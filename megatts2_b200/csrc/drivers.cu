@@ -279,8 +279,9 @@ static int64_t plm_ws_floats(const mtts_plm* m, int B, int T) {
 // (sample.cu), keyed by the step index t, so the split does not change the draws either.
 // Prosody mix (weights != nullptr): tc holds K sources stacked as K*B rows (row k*B + b = source k of utterance b), all
 // reading the shared (B, T+1) code state.  Each step runs the encoder and the predict layer once over the K*B rows, then
-// mix_logprob_rows turns each utterance's K logits rows and its row of the (B, K) weights into l (B, V), and the pick
-// reads l.  logits_out, when given, is (K*B, T, V): the raw per-source logits.  K = 1 without weights is the plain decode.
+// mix_logprob_rows turns each utterance's K logits rows and its weight row into l (B, V), and the pick reads l.  Target
+// step j of utterance b reads the row weights + b w_sb + j w_st: w_st = 0 is one (B, K) row per utterance for every step.
+// logits_out, when given, is (K*B, T, V): the raw per-source logits.  K = 1 without weights is the plain decode.
 // Prompt context (ctx != nullptr, K = 1): the decode runs over N = P + T positions, the first P latent rows from ctx->tc
 // and the codes of columns 1..P of the (B, N+1) code state from ctx->codes (written here when t0 = 0).  t0, t1, codes_out,
 // logits_out and the sampler's step key stay in target steps: target step j is position P + j.  P = 0 is the plain decode.
@@ -291,13 +292,14 @@ struct PlmCtx {
 };
 static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int t0, int t1,
                            int64_t* state, int64_t* codes_out, float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
-                           const mtts_sampling* smp, int K = 1, const float* weights = nullptr,
-                           const PlmCtx* ctx = nullptr) {
+                           const mtts_sampling* smp, int K = 1, const float* weights = nullptr, int64_t w_sb = 0,
+                           int64_t w_st = 0, const PlmCtx* ctx = nullptr) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
   MTTS_REQUIRE(0 <= t0 && t0 <= t1 && t1 <= (T > 0 ? T : 0), "step range outside [0, T]");
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
+  MTTS_REQUIRE(w_sb >= 0 && w_st >= 0, "weight strides must be >= 0");
   MTTS_REQUIRE(!ctx || (K == 1 && ctx->P >= 0 && (ctx->P == 0 || (ctx->tc && ctx->codes))), "bad context");
   if (weights) MTTS_TRY(mix_logprob_check(V, K));
   if (B <= 0 || T <= 0 || t0 == t1) return 0;
@@ -337,7 +339,7 @@ static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, in
     const float* pick_from = lg;
     int64_t pick_ld = lg_sb;
     if (weights) {
-      MTTS_TRY(mix_logprob_rows(lg, lg_sb, V, K, B, weights, mixed, V, st));
+      MTTS_TRY(mix_logprob_rows(lg, lg_sb, V, K, B, weights + j * w_st, w_sb, mixed, V, st));
       pick_from = mixed; pick_ld = V;
     }
     if (smp) MTTS_TRY(sample_rows(pick_from, pick_ld, V, B, j, *smp, codes + (t + 1), N + 1, codes_out + j, T, st));
@@ -362,15 +364,17 @@ static int64_t adm_ws_floats(const mtts_adm* m, int B, int T) {
 // Duration mix (weights or raw_src_out given): tc holds K sources stacked as K*B rows (row k*B + b = source k of utterance
 // b), all reading the shared (B, T+1) raw history.  tc_linear_emb and each step's encoder run once over the K*B rows, then
 // adm_readout_mix writes the mixed value into the history (and, with raw_src_out (K, B, T), every source's readout).
+// Step t of utterance b reads the weight row weights + b w_sb + t w_st (w_st = 0: one row for every step).
 // K = 1 without weights or raw_src_out is the plain decode.
 static int adm_infer(const mtts_adm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int32_t* dur_out,
                      float* raw_out, void* ws, int64_t ws_bytes, cudaStream_t st, int K = 1, const float* weights = nullptr,
-                     float* raw_src_out = nullptr) {
+                     int64_t w_sb = 0, int64_t w_st = 0, float* raw_src_out = nullptr) {
   const int D = m->enc.d_model;
   MTTS_REQUIRE(D == m->emb_dim + m->tc_emb_dim, "d_model != emb_dim + tc_emb_dim");
   MTTS_REQUIRE(tc && dur_out && m->w_dt && m->w_tc && m->w_predict && m->pe, "null pointer");
   MTTS_TRY(adm_mix_check(K));
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
+  MTTS_REQUIRE(w_sb >= 0 && w_st >= 0, "weight strides must be >= 0");
   if (B <= 0 || T <= 0) return 0;
   const bool mix = weights || raw_src_out;
   const int R = K * B;                                       // latent rows: the K sources of the B utterances
@@ -404,8 +408,8 @@ static int adm_infer(const mtts_adm* m, const float* tc, int64_t tc_sb, int tc_l
     Arena ar((char*)ws + enc_off, ws_bytes - enc_off);
     MTTS_TRY(encoder_forward(&m->enc, X, xl, R, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
     if (mix)
-      MTTS_TRY(adm_readout_mix(xl, D, m->w_predict, K, B, weights, praw + (t + 1), T + 1,
-                               raw_src_out ? raw_src_out + t : nullptr, T, st));
+      MTTS_TRY(adm_readout_mix(xl, D, m->w_predict, K, B, weights ? weights + t * w_st : nullptr, w_sb, praw + (t + 1),
+                               T + 1, raw_src_out ? raw_src_out + t : nullptr, T, st));
     else
       MTTS_TRY(adm_readout(xl, D, m->w_predict, B, praw, T + 1, t + 1, st));
   }
@@ -1058,7 +1062,7 @@ int mtts_plm_infer_mix_f32(const mtts_plm* m, int32_t K, const float* tc_latent,
   MTTS_REQUIRE(m && m->enc.layers && workspace && weights, "null pointer");
   if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
-                         workspace_bytes, (cudaStream_t)stream, s, K, weights);
+                         workspace_bytes, (cudaStream_t)stream, s, K, weights, K, 0);
 }
 int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
                                  int32_t B, int32_t T, const float* weights, int32_t t0, int32_t t1, int64_t* code_state,
@@ -1067,7 +1071,25 @@ int mtts_plm_infer_mix_range_f32(const mtts_plm* m, int32_t K, const float* tc_l
   MTTS_REQUIRE(m && m->enc.layers && workspace && weights && code_state, "null pointer");
   if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
-                         workspace_bytes, (cudaStream_t)stream, s, K, weights);
+                         workspace_bytes, (cudaStream_t)stream, s, K, weights, K, 0);
+}
+int mtts_plm_infer_mix_steps_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                 int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st, int64_t* codes_out,
+                                 float* logits_out, const mtts_sampling* s, void* workspace, int64_t workspace_bytes,
+                                 void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && weights, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, K, weights, w_sb, w_st);
+}
+int mtts_plm_infer_mix_steps_range_f32(const mtts_plm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                       int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st, int32_t t0,
+                                       int32_t t1, int64_t* code_state, int64_t* codes_out, float* logits_out,
+                                       const mtts_sampling* s, void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && weights && code_state, "null pointer");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, t0, t1, code_state, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, K, weights, w_sb, w_st);
 }
 
 int64_t mtts_plm_infer_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T) {
@@ -1081,7 +1103,7 @@ int mtts_plm_infer_ctx_f32(const mtts_plm* m, const float* tc_latent, int64_t tc
   if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
   const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, 0, T > 0 ? T : 0, nullptr, codes_out, logits_out, workspace,
-                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, &c);
+                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, 0, 0, &c);
 }
 int mtts_plm_infer_ctx_range_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
                                  int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
@@ -1092,7 +1114,7 @@ int mtts_plm_infer_ctx_range_f32(const mtts_plm* m, const float* tc_latent, int6
   if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
   const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, j0, j1, code_state, codes_out, logits_out, workspace,
-                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, &c);
+                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, 0, 0, &c);
 }
 int64_t mtts_plm_decode_causal_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T) {
   return plm_causal_ws_floats(m, B, T, P > 0 ? P : 0) * 4 + 8192;
@@ -1122,7 +1144,14 @@ int mtts_adm_infer_mix_f32(const mtts_adm* m, int32_t K, const float* tc_latent,
                            void* workspace, int64_t workspace_bytes, void* stream) {
   MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
   return adm_infer(m, tc_latent, tc_sb, tc_ld, B, T, dur_out, raw_out, workspace, workspace_bytes, (cudaStream_t)stream,
-                   K, weights, raw_src_out);
+                   K, weights, K, 0, raw_src_out);
+}
+int mtts_adm_infer_mix_steps_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                                 int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st, int32_t* dur_out,
+                                 float* raw_out, float* raw_src_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && weights, "null pointer");
+  return adm_infer(m, tc_latent, tc_sb, tc_ld, B, T, dur_out, raw_out, workspace, workspace_bytes, (cudaStream_t)stream,
+                   K, weights, w_sb, w_st, raw_src_out);
 }
 
 int64_t mtts_plm_decode_causal_workspace_bytes(const mtts_plm* m, int32_t B, int32_t T) {

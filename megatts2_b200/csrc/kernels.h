@@ -184,11 +184,11 @@ int sampling_check(const mtts_sampling* s, int V);
 int sample_rows(const float* x, int64_t ldx, int V, int rows, int step, const mtts_sampling& s, int64_t* out_a,
                 int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st);
 int philox4x32_10_words(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, cudaStream_t st);
-// prosody mix (sample.cu): l (B, V) from K source rows per utterance and (B, K) weights; mix_logprob_check validates
-// (V, K) before a driver enqueues anything
+// prosody mix (sample.cu): l (B, V) from K source rows per utterance and the weight rows w + b ldw; mix_logprob_check
+// validates (V, K) before a driver enqueues anything
 int mix_logprob_check(int V, int K);
-int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const float* w, float* out, int64_t ldo,
-                     cudaStream_t st);
+int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const float* w, int64_t ldw, float* out,
+                     int64_t ldo, cudaStream_t st);
 int fill_i64(int64_t* p, int64_t stride, int n, int64_t v, cudaStream_t st);
 int fill_f32(float* p, int64_t stride, int n, float v, cudaStream_t st);
 // latent row r reads history row r % B_hist (B_hist = B: one history per latent row; fewer: sources sharing a history)
@@ -196,11 +196,14 @@ int adm_build_input(const float* tc_emb, int64_t te_sb, int te_ld, int tc_emb_di
                     int B_hist, const float* w_dt, int emb_dim, const float* pe, float alpha, int B, int S, float* X,
                     cudaStream_t st);
 int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st);
-// duration mix: r_b from the K rows k*B + b of xl and the (B, K) weights into out[b * ld_out]; y_out (optional) gets every
-// source's readout.  adm_mix_check validates K before a driver enqueues anything.
+// duration mix: r_b from the K rows k*B + b of xl and the weight rows weights + b ldw into out[b * ld_out]; y_out
+// (optional) gets every source's readout.  adm_mix_check validates K before a driver enqueues anything.
 int adm_mix_check(int K);
-int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, float* out, int64_t ld_out,
-                    float* y_out, int64_t ld_y, cudaStream_t st);
+int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, int64_t ldw, float* out,
+                    int64_t ld_out, float* y_out, int64_t ld_y, cudaStream_t st);
+// per-phone mix weights (B, Tp, K) -> per-PLM-step weights (B, T, K) by the durations (mtts_mix_step_weights_f32)
+int mix_step_weights(const float* pw, int64_t pw_sb, int Tp, int K, int B, const int32_t* dur, int64_t dur_sb, int T,
+                     float* out, cudaStream_t st);
 int adm_finalize(const float* praw, int p_ld, int B, int T, int32_t* dur, float* raw_out, cudaStream_t st);
 
 // convenience: dense linear layer  Y[M,N] = act(X[M,K] W + b) (+ res)

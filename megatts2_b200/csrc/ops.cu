@@ -970,12 +970,12 @@ int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int 
 }
 
 // Duration mix readout (the contract is stated with mtts_adm_readout_mix_f32 in include/megatts2_b200.h): one warp per
-// utterance b.  The warp computes y of each weighted source (of every source when y_out is given) and folds the weighted
+// utterance b, whose weight row is weights + b ldw.  The warp computes y of each weighted source (of every source when y_out is given) and folds the weighted
 // ones into r in k order: the first term is w^ y, the later ones fmaf(w^, y, r).
 constexpr int ADM_MIX_MAX_K = 8;
 __global__ void adm_readout_mix_kernel(const float* __restrict__ xl, int D, const float* __restrict__ w, int K, int B,
-                                       const float* __restrict__ weights, float* __restrict__ out, int64_t ld_out,
-                                       float* __restrict__ y_out, int64_t ld_y) {
+                                       const float* __restrict__ weights, int64_t ldw, float* __restrict__ out,
+                                       int64_t ld_out, float* __restrict__ y_out, int64_t ld_y) {
   pdl_entry();
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -984,7 +984,7 @@ __global__ void adm_readout_mix_kernel(const float* __restrict__ xl, int D, cons
   float wsum = 0.f;
 #pragma unroll
   for (int k = 0; k < ADM_MIX_MAX_K; ++k) {
-    wk[k] = k < K ? (weights ? weights[(int64_t)b * K + k] : 1.f) : 0.f;
+    wk[k] = k < K ? (weights ? weights[(int64_t)b * ldw + k] : 1.f) : 0.f;
     if (wk[k] > 0.f) wsum += wk[k];             // zero weights add nothing; NaN or negative ones are skipped throughout
   }
   float r = 0.f;
@@ -1012,14 +1012,104 @@ int adm_mix_check(int K) {
   return 0;
 }
 
-int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, float* out, int64_t ld_out,
-                    float* y_out, int64_t ld_y, cudaStream_t st) {
+int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, int64_t ldw, float* out,
+                    int64_t ld_out, float* y_out, int64_t ld_y, cudaStream_t st) {
   MTTS_TRY(adm_mix_check(K));
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
-  MTTS_REQUIRE(D >= 1 && ld_out >= 0 && ld_y >= 0, "D must be >= 1 and ld >= 0");
+  MTTS_REQUIRE(D >= 1 && ldw >= 0 && ld_out >= 0 && ld_y >= 0, "D must be >= 1 and ld >= 0");
   if (B <= 0) return 0;
   MTTS_REQUIRE(xl && w && out, "null pointer");
-  launch_k(adm_readout_mix_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, K, B, weights, out, ld_out, y_out, ld_y);
+  launch_k(adm_readout_mix_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, K, B, weights, ldw, out, ld_out, y_out,
+           ld_y);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
+// Phone -> PLM step weights (the contract is stated with mtts_mix_step_weights_f32 in include/megatts2_b200.h): one CTA
+// per utterance.  The CTA scans the durations into cum[0..Tp] (cum[i] = frames of the phones before i, negative durations
+// counted as 0, as length_regulate_kernel counts them); then each thread takes steps t: the phone owning frame 8t by
+// length_regulate_kernel's search, then the phones after it while they start before the step's end, keeping the first
+// with the most frames.  Integer arithmetic only, and the K weights are copied as bits.
+constexpr int STEPW_THREADS = 256;
+constexpr int STEPW_MAX_TP = 8192;
+__device__ __forceinline__ int stepw_owner(const int* cum, int Tp, int r) {   // largest i < Tp with cum[i] <= r
+  int lo = 0, hi = Tp;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (cum[mid] <= r) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+__global__ void __launch_bounds__(STEPW_THREADS)
+mix_step_weights_kernel(const float* __restrict__ pw, int64_t pw_sb, int Tp, int K, const int32_t* __restrict__ dur,
+                        int64_t dur_sb, int T, float* __restrict__ out) {
+  extern __shared__ int cum[];   // Tp + 1
+  __shared__ int s_warp[STEPW_THREADS / 32];
+  pdl_entry();
+  const int b = blockIdx.x, lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+  const int32_t* d = dur + (int64_t)b * dur_sb;
+  const int per = (Tp + STEPW_THREADS - 1) / STEPW_THREADS;
+  const int i0 = min((int)threadIdx.x * per, Tp), i1 = min(i0 + per, Tp);
+  int own = 0;
+  for (int i = i0; i < i1; ++i) own += max(d[i], 0);
+  int incl = own;                                            // block scan: warp shuffles, then the warp totals
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  if (lane == 31) s_warp[wp] = incl;
+  __syncthreads();
+  if (wp == 0) {
+    int v = lane < STEPW_THREADS / 32 ? s_warp[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += u;
+    }
+    if (lane < STEPW_THREADS / 32) s_warp[lane] = v;
+  }
+  __syncthreads();
+  int c = incl - own + (wp ? s_warp[wp - 1] : 0);
+  for (int i = i0; i < i1; ++i) {
+    cum[i] = c;
+    c += max(d[i], 0);
+  }
+  if (threadIdx.x == 0) cum[Tp] = s_warp[STEPW_THREADS / 32 - 1];
+  __syncthreads();
+  const int L = cum[Tp];
+  const int last = L > 0 ? stepw_owner(cum, Tp, L - 1) : 0;   // the last phone with a positive duration
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(pw + (int64_t)b * pw_sb);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(out + (int64_t)b * T * K);
+  for (int t = threadIdx.x; t < T; t += STEPW_THREADS) {
+    int p = last;
+    if ((int64_t)t * 8 < L) {
+      const int s0 = 8 * t, e = min(s0 + 8, L);
+      int best = 0;
+      for (int i = stepw_owner(cum, Tp, s0); i < Tp && cum[i] < e; ++i) {
+        const int n = min(cum[i + 1], e) - max(cum[i], s0);
+        if (n > best) { best = n; p = i; }
+      }
+    }
+    for (int k = 0; k < K; ++k) dst[(int64_t)t * K + k] = src[(int64_t)p * K + k];
+  }
+}
+
+int mix_step_weights(const float* pw, int64_t pw_sb, int Tp, int K, int B, const int32_t* dur, int64_t dur_sb, int T,
+                     float* out, cudaStream_t st) {
+  MTTS_REQUIRE(K >= 1, "K must be >= 1");
+  if (K > ADM_MIX_MAX_K)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: K = %lld sources is above the bound of %lld", "mix_step_weights", K,
+                ADM_MIX_MAX_K);
+  MTTS_REQUIRE(Tp >= 1, "Tp must be >= 1");
+  if (Tp > STEPW_MAX_TP)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: Tp = %lld phones is above the bound of %lld", "mix_step_weights", Tp,
+                STEPW_MAX_TP);
+  MTTS_REQUIRE(pw_sb >= 0 && dur_sb >= 0, "strides must be >= 0");
+  if (B <= 0 || T <= 0) return 0;
+  MTTS_REQUIRE(pw && dur && out, "null pointer");
+  launch_k(mix_step_weights_kernel, (unsigned)B, STEPW_THREADS, (size_t)(Tp + 1) * sizeof(int), st, pw, pw_sb, Tp, K,
+           dur, dur_sb, T, out);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

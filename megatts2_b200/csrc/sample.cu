@@ -195,19 +195,19 @@ __device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os
 }
 
 // One CTA per utterance b: l_i = log sum_k w^_k softmax(z_k)_i over the K rows z_k = x[(k B + b) ldx ..] (the contract is
-// stated with mtts_mix_logprob_rows_f32 in include/megatts2_b200.h).  Warp k reduces source k's (max, sum of exps) and its
+// stated with mtts_mix_logprob_rows_f32 in include/megatts2_b200.h), with the weight row w + b ldw.  Warp k reduces source k's (max, sum of exps) and its
 // lowest +inf index with shuffles; then every thread combines the sources for its tokens as a log-sum-exp in fp32.  The
 // rows were just written by the predict layer and are read from L2: each lane issues MIX_CHUNK loads before it uses one,
 // so a row costs V / (32 MIX_CHUNK) load latencies instead of V / 32.
 constexpr int MIX_CHUNK = 16;
 __global__ void __launch_bounds__(SAMPLE_THREADS)
 mix_logprob_rows_kernel(const float* __restrict__ x, int64_t ldx, int V, int K, int B, const float* __restrict__ w,
-                        float* __restrict__ out, int64_t ldo) {
+                        int64_t ldw, float* __restrict__ out, int64_t ldo) {
   __shared__ float s_lw[MIX_MAX_K], s_m[MIX_MAX_K];          // log w^_k - log sum_k, max_k
   __shared__ int s_inf[MIX_MAX_K], s_on[MIX_MAX_K];
   pdl_entry();
   const int b = blockIdx.x, lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
-  const float* wr = w + (int64_t)b * K;
+  const float* wr = w + (int64_t)b * ldw;
   float wk[MIX_MAX_K];
 #pragma unroll
   for (int k = 0; k < MIX_MAX_K; ++k) wk[k] = k < K ? wr[k] : 0.f;
@@ -331,13 +331,13 @@ int mix_logprob_check(int V, int K) {
   return 0;
 }
 
-int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const float* w, float* out, int64_t ldo,
-                     cudaStream_t st) {
+int mix_logprob_rows(const float* x, int64_t ldx, int V, int K, int B, const float* w, int64_t ldw, float* out,
+                     int64_t ldo, cudaStream_t st) {
   MTTS_TRY(mix_logprob_check(V, K));
-  MTTS_REQUIRE(ldx >= 0 && ldo >= 0, "ld must be >= 0");
+  MTTS_REQUIRE(ldx >= 0 && ldw >= 0 && ldo >= 0, "ld must be >= 0");
   if (B <= 0) return 0;
   MTTS_REQUIRE(x && w && out, "null pointer");
-  launch_k(mix_logprob_rows_kernel, (unsigned)B, SAMPLE_THREADS, 0, st, x, ldx, V, K, B, w, out, ldo);
+  launch_k(mix_logprob_rows_kernel, (unsigned)B, SAMPLE_THREADS, 0, st, x, ldx, V, K, B, w, ldw, out, ldo);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

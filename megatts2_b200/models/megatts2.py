@@ -48,8 +48,8 @@ def _sampling_inputs(sampling, keys, rows, device):
 
 
 def _mix_sources(tc_latents, weights, dim, what):
-    """K source latents, each (B, T, dim), and their weights -> (the (K*B, T, dim) stack, (B, K) device weights).  ``what``
-    names the mix in the error messages."""
+    """K source latents, each (B, T, dim), and their weights -> (the (K*B, T, dim) stack, (B, K) device weights, or
+    (B, T, K) when ``weights`` is a schedule with one row per step).  ``what`` names the mix in the error messages."""
     if isinstance(tc_latents, torch.Tensor) or not len(tc_latents):
         raise L.MttsError(f"{what}: tc_latents must be a non-empty list of (B, T, tc_dim) tensors")
     tcs = [ops._dev(t, name=f"tc_latents[{k}]") for k, t in enumerate(tc_latents)]
@@ -59,8 +59,11 @@ def _mix_sources(tc_latents, weights, dim, what):
                           f"{[tuple(t.shape) for t in tcs]}")
     if any(t.device != tcs[0].device for t in tcs):
         raise L.MttsError(f"{what}: the sources must be on one device")
-    w = S.mix_weights(weights, len(tcs), shape[0], what).to(tcs[0].device)
-    return torch.cat(tcs, 0), w
+    if S.per_step(weights):
+        w = S.mix_step_weights(weights, len(tcs), shape[0], shape[1], what)
+    else:
+        w = S.mix_weights(weights, len(tcs), shape[0], what)
+    return torch.cat(tcs, 0), w.to(tcs[0].device)
 
 
 class PLMContext:
@@ -291,7 +294,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
 
     def _decode(self, tc, K, weights, smp, t0, t1, state, return_logits, ctx=None):
         """Steps [t0, t1) of the decode of B utterances from ``tc``, the (K*B, T, tc_dim) stack of K sources mixed by the
-        (B, K) device ``weights`` (None: K = 1, the plain decode).  ``smp``: (sampling, seed, keys), or None for greedy.
+        (B, K) device ``weights``, or by the (B, T, K) schedule with one row per step (None: K = 1, the plain decode).  ``smp``: (sampling, seed, keys), or None for greedy.
         ``state`` None: the whole decode (t0 = 0, t1 = T) on the shared workspace; otherwise a range against that (B, T+1)
         code state, on a private workspace since a captured range pins it.  ``ctx``: (tc8 (Bc, P, tc_dim), codes (Bc, P)) of
         a prompt context, or None; the steps stay target steps and the state is then (B, P+T+1).  The enqueues are
@@ -300,13 +303,16 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         or (K, B, t1 - t0, V) when mixed]."""
         B, T, V = tc.shape[0] // K, tc.shape[1], self.vq_bins
         mix, ranged = weights is not None, state is not None
+        sched = mix and weights.dim() == 3
         P = 0 if ctx is None else ctx[0].shape[1]
         pl = self._plan_get(tc.device, P + T)
         lib = L.lib()
         m = C.byref(pl.struct)
         if ctx is not None:   # so do the context entries
             entry = lib.mtts_plm_infer_ctx_range_f32 if ranged else lib.mtts_plm_infer_ctx_f32
-        elif mix:        # the mix entries take the sampling as a nullable argument
+        elif sched:      # the mix entries take the sampling as a nullable argument
+            entry = lib.mtts_plm_infer_mix_steps_range_f32 if ranged else lib.mtts_plm_infer_mix_steps_f32
+        elif mix:
             entry = lib.mtts_plm_infer_mix_range_f32 if ranged else lib.mtts_plm_infer_mix_f32
         elif smp is None:
             entry = lib.mtts_plm_infer_range_f32 if ranged else lib.mtts_plm_infer_f32
@@ -334,7 +340,8 @@ class MegaPLM(pack.PlanMixin, nn.Module):
             if ctx is not None:
                 args = (m,) + lat + _ctx_args(ctx_) + steps + outs + (s,)
             elif mix:
-                args = (m, K) + lat + (w_.data_ptr(),) + steps + outs + (s,)
+                w_args = (w_.data_ptr(), T * K, K) if sched else (w_.data_ptr(),)
+                args = (m, K) + lat + w_args + steps + outs + (s,)
             else:
                 args = (m,) + lat + steps + outs + ((s,) if s is not None else ())
             L.check(entry(*args, ws.data_ptr(), ws_bytes, ops._stream()))
@@ -343,7 +350,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         inputs = ((tc,) + ((state,) if ranged else ()) + ((weights,) if mix else ()) + (tuple(ctx) if ctx is not None else ())
                   + (smp[1:] if smp is not None else ()))
         key = (pl.serial, K, mix, B, T, t0, t1, bool(return_logits), tc.stride(0), tc.stride(1), ops.launch_policy_now(),
-               None if smp is None else smp[0].graph_key(), None if ctx is None else (ctx[0].shape[0], P))
+               None if smp is None else smp[0].graph_key(), None if ctx is None else (ctx[0].shape[0], P), sched)
         out = self._graphs("range" if ranged else "main").run(key, inputs, run)
         if not return_logits:
             return out[0]
@@ -357,7 +364,11 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         by ``sampling`` / ``keys`` as in ``infer``; with exactly one positive weight in a row, l is that source's raw
         logits row (include/megatts2_b200.h states the contract).  -> codes (B, T) int64 [, logits (K, B, T, vq_bins), the
         raw per-source logits].  Replays as a CUDA graph whose inputs are the latents, the weights, the seed and the keys,
-        so new weight values need no new capture."""
+        so new weight values need no new capture.
+
+        ``weights`` may also be a schedule (B, T, K): step t of utterance b then mixes by row (b, t), under the same rules
+        per row, so the prosody can follow one prompt in one part of the utterance and another elsewhere
+        (``ops.mix_step_weights`` makes such a schedule from per-phone weights)."""
         _eval_only(self)
         tc, w = _mix_sources(tc_latents, weights, self.tc_latent_dim, "prosody mix")
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
@@ -366,8 +377,8 @@ class MegaPLM(pack.PlanMixin, nn.Module):
     def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None, context=None) -> "PLMDecode":
         """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
         any number of ranges gives ``infer``'s codes and logits (same ``sampling``, ``keys`` and ``context``).  With
-        ``weights``, ``tc_latent`` is the list of K sources of ``infer_mix`` and the ranges give ``infer_mix``'s codes and
-        logits (not with a context)."""
+        ``weights`` ((K,), (B, K) or a (B, T, K) schedule), ``tc_latent`` is the list of K sources of ``infer_mix`` and the
+        ranges give ``infer_mix``'s codes and logits (not with a context)."""
         _eval_only(self)
         K, w = 1, None
         if weights is not None:
@@ -458,12 +469,12 @@ class PLMDecode:
     (B, P+T+1) int64 (column 0 = BOS, columns 1..P the context's codes, column P+1+t the code of target step t once
     decoded), the sampling parameters with the seed and row keys as device tensors (None for greedy), and ``t``, the number
     of target steps decoded.  A mixed decode also holds the (B, K) device ``weights``, and ``tc`` is then the (K*B, T,
-    tc_dim) stack of its K sources; a decode with a context holds ``ctx`` = (tc8 (Bc, P, tc_dim), codes (Bc, P)) and P."""
+    tc_dim) stack of its K sources (or the (B, T, K) schedule); a decode with a context holds ``ctx`` = (tc8 (Bc, P, tc_dim), codes (Bc, P)) and P."""
 
     def __init__(self, tc, state, sampling, seed, keys, weights=None, ctx=None):
         self.tc, self.state, self.sampling, self.seed, self.keys = tc, state, sampling, seed, keys
         self.weights, self.ctx = weights, ctx
-        self.K = 1 if weights is None else weights.shape[1]
+        self.K = 1 if weights is None else weights.shape[-1]
         self.P = 0 if ctx is None else ctx[0].shape[1]
         self.B, self.T = state.shape[0], tc.shape[1]
         self.t = 0
@@ -556,10 +567,14 @@ class MegaADM(pack.PlanMixin, nn.Module):
         mean of their readouts; with exactly one positive weight in a row, r is that source's readout bit for bit
         (include/megatts2_b200.h states the contract).  -> durations (B, T, 1) int32 [, raw (B, T) fp32 (the mixed values),
         raw_src (K, B, T) fp32 (every source's readout)].  Replays as a CUDA graph whose inputs are the latents and the
-        weights, so new weight values need no new capture."""
+        weights, so new weight values need no new capture.
+
+        ``weights`` may also be a schedule (B, T, K), one row per phone: step t, the duration of phone t, mixes by row
+        (b, t)."""
         _eval_only(self)
         tc, w = _mix_sources(tc_latents, weights, self.tc_latent_dim, "duration mix")
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
+        sched = w.dim() == 3
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
 
@@ -568,14 +583,17 @@ class MegaADM(pack.PlanMixin, nn.Module):
             raw = torch.empty(B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
             raw_src = torch.empty(K, B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
             ws = ops.workspace(lib.mtts_adm_infer_mix_workspace_bytes(C.byref(pl.struct), K, B, T), tc_.device)
-            L.check(lib.mtts_adm_infer_mix_f32(C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
-                                               w_.data_ptr(), dur.data_ptr(), raw.data_ptr() if return_raw else None,
-                                               raw_src.data_ptr() if return_raw else None, ws.data_ptr(), ws.numel(),
-                                               ops._stream()))
+            lat = (C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T)
+            outs = (dur.data_ptr(), raw.data_ptr() if return_raw else None, raw_src.data_ptr() if return_raw else None,
+                    ws.data_ptr(), ws.numel(), ops._stream())
+            if sched:
+                L.check(lib.mtts_adm_infer_mix_steps_f32(*lat, w_.data_ptr(), T * K, K, *outs))
+            else:
+                L.check(lib.mtts_adm_infer_mix_f32(*lat, w_.data_ptr(), *outs))
             return (dur, raw, raw_src) if return_raw else (dur,)
 
         out = self._graphs().run(("adm_mix", pl.serial, K, B, T, bool(return_raw), tc.stride(0), tc.stride(1),
-                                  ops.launch_policy_now()), (tc, w), run)
+                                  ops.launch_policy_now(), sched), (tc, w), run)
         dur = out[0].unsqueeze(-1)
         return (dur, out[1], out[2]) if return_raw else dur
 
@@ -820,6 +838,13 @@ def _warn_fp16_range(then):
     warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; " + then, stacklevel=2)
 
 
+def _synth_mix_weights(weights, K, B, Tp, what):
+    """The validated (B, K) CPU weights of a synthesis mix, or (B, Tp, K) when ``weights`` has one row per phone."""
+    if S.per_step(weights):
+        return S.mix_step_weights(weights, K, B, Tp, what)
+    return S.mix_weights(weights, K, B, what)
+
+
 class Megatts(nn.Module):
     """Inference orchestrator (models/megatts2.py:295-375).  ``synthesize`` is the tensor-level
     body of the reference's ``forward`` for a batch; ``forward(wavs_dir, text)`` keeps the
@@ -874,13 +899,16 @@ class Megatts(nn.Module):
         (``MegaPLM.infer``), utterance b keyed by ``keys[b]`` (default arange(B)); the ADM durations stay deterministic.
         The bf16x3 rerun above draws with the same seed and keys.
         ``prosody_mels`` (opt-in prosody interpolation): a list of (B, Tm_k, 80) prosody prompts, with ``prosody_weights``
-        (K,) or (B, K), K = 1 + len(prosody_mels); weight 0 belongs to ``mels``.  Each prompt gives a source latent
+        (K,) or (B, K), K = 1 + len(prosody_mels); weight 0 belongs to ``mels``.  ``prosody_weights`` may also be
+        (B, Tp, K), one row per phone: PLM step t then mixes by the row of the phone owning most of its 8 mel frames
+        (``ops.mix_step_weights``, with the durations used), so the prosody changes along the utterance in 8-frame
+        steps; ``return_intermediates`` then adds ``prosody_step_weights`` (B, T, K).  Each prompt gives a source latent
         ``mrte.tc_latent(phone_tokens, prompt)``, length-regulated and max-pooled with the target's durations, and the
         codes come from ``MegaPLM.infer_mix`` over the K sources.  The durations (unless ``duration_weights`` is given),
         the mel decoder and the vocoder keep the target's (``mels``) latent, so the timbre stays the target's.  Not with
         ``causal_decode``.
-        ``duration_weights`` (opt-in duration interpolation, with ``prosody_mels``): (K,) or (B, K), the same K; weight 0
-        belongs to ``mels``.  The durations then come from ``MegaADM.infer_mix`` over [the target's latent, *the prompts'
+        ``duration_weights`` (opt-in duration interpolation, with ``prosody_mels``): (K,) or (B, K), or (B, Tp, K) with one
+        row per phone (the ADM's step t is phone t), the same K; weight 0 belongs to ``mels``.  The durations then come from ``MegaADM.infer_mix`` over [the target's latent, *the prompts'
         latents] instead of ``MegaADM.infer`` on the target's alone, so the rhythm moves toward the prompts as well; each
         prompt's latent is computed once and serves both mixes.  ``forced_durations`` still override them.
         ``plm_context`` (opt-in in-context prompting): a ``PLMContext`` (or a list of them, joined in order), e.g. from
@@ -933,9 +961,9 @@ class Megatts(nn.Module):
             ops._dev(m, name=f"prosody_mels[{k}]")
             if m.dim() != 3 or m.shape[0] != B or m.shape[2] != nb or m.shape[1] < 1:
                 raise L.MttsError(f"prosody_mels[{k}]: expected ({B}, Tm, {nb}), got {tuple(m.shape)}")
-        S.mix_weights(prosody_weights, 1 + len(prosody_mels), B)
+        _synth_mix_weights(prosody_weights, 1 + len(prosody_mels), B, phone_tokens.shape[1], "prosody mix")
         if duration_weights is not None:
-            S.mix_weights(duration_weights, 1 + len(prosody_mels), B, "duration mix")
+            _synth_mix_weights(duration_weights, 1 + len(prosody_mels), B, phone_tokens.shape[1], "duration mix")
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
                     sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None,
@@ -977,10 +1005,11 @@ class Megatts(nn.Module):
         else:
             tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
             dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights)
-        tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats)
+        tc_expand, totals, src, step_w = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats,
+                                                          prosody_weights)
         if prosody_mels is not None:
             tc8 = src[0]
-            p_codes = self.plm.infer_mix(src, prosody_weights, sampling=sampling, keys=keys)
+            p_codes = self.plm.infer_mix(src, prosody_weights if step_w is None else step_w, sampling=sampling, keys=keys)
         else:
             tc8 = src
             p_codes = plm_decode(src, sampling=sampling, keys=keys, context=plm_context)
@@ -1012,8 +1041,11 @@ class Megatts(nn.Module):
                 pw = pw_side
             wav = torch.cat([pw, wav], dim=-1)                        # (:373)
             wav_lens = [n + pw.shape[-1] for n in wav_lens]
-        return dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
-                    mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
+        out = dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
+                   mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
+        if step_w is not None:
+            out["prosody_step_weights"] = step_w
+        return out
 
     def _durations(self, adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights):
         """-> (dt (B, Tp) int32, the prompts' MRTE latents or None).  Without ``duration_weights``: ``adm_decode`` on
@@ -1024,21 +1056,29 @@ class Megatts(nn.Module):
         lats = [self.generator.mrte.tc_latent(phone_tokens, m) for m in prosody_mels]
         return self.adm.infer_mix([tc_latent] + lats, duration_weights)[..., 0], lats
 
-    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels, prosody_latents=None):
+    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels, prosody_latents=None,
+                    prosody_weights=None):
         """The synthesis front end between the ADM and the PLM: the durations (``forced_durations`` if given, else
         ``dt``) expand ``tc_latent`` to frames -> (tc_expand (B, Lmax, tc_dim), the per-utterance frame totals on the host
-        (one host sync), the PLM's source).  The source is tc8, tc_expand max-pooled by 8, or with ``prosody_mels`` the
-        list [tc8, *one latent per prosody prompt]: MRTE on (phone_tokens, prompt) (or its ``prosody_latents`` entry when
-        the duration mix already computed it), length-regulated with the same durations to Lmax frames, max-pooled by 8."""
+        (one host sync), the PLM's source, the PLM's step weights).  The source is tc8, tc_expand max-pooled by 8, or with
+        ``prosody_mels`` the list [tc8, *one latent per prosody prompt]: MRTE on (phone_tokens, prompt) (or its
+        ``prosody_latents`` entry when the duration mix already computed it), length-regulated with the same durations to
+        Lmax frames, max-pooled by 8.  The step weights are None unless ``prosody_weights`` has one row per phone; then
+        they are its (B, ceil(Lmax / 8), K) expansion by the same durations (``ops.mix_step_weights``)."""
         d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
         tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
         tc8 = ops.maxpool_time(tc_expand, 8)
         if prosody_mels is None:
-            return tc_expand, totals, tc8
+            return tc_expand, totals, tc8, None
         mrte, Lmax = self.generator.mrte, tc_expand.shape[1]
         lats = prosody_latents if prosody_latents is not None else (mrte.tc_latent(phone_tokens, m) for m in prosody_mels)
-        return tc_expand, totals, [tc8] + [ops.maxpool_time(ops.length_regulate(lat, d_used, l_out=Lmax)[0], 8)
-                                       for lat in lats]
+        src = [tc8] + [ops.maxpool_time(ops.length_regulate(lat, d_used, l_out=Lmax)[0], 8) for lat in lats]
+        step_w = None
+        if S.per_step(prosody_weights):
+            B, Tp = phone_tokens.shape
+            pw = S.mix_step_weights(prosody_weights, len(src), B, Tp).to(tc8.device)
+            step_w = ops.mix_step_weights(pw, d_used, tc8.shape[1])
+        return tc_expand, totals, src, step_w
 
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
@@ -1100,8 +1140,10 @@ class Megatts(nn.Module):
             tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
             prosody_mels, prosody_weights, duration_weights, plm_context = prosody
             dt, lats = self._durations(self.adm.infer, tc_latent, phone_tokens, prosody_mels, duration_weights)
-            tc_expand, totals, src = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats)
-            dec = self.plm.begin_decode(src, sampling=sampling, keys=keys, weights=prosody_weights, context=plm_context)
+            tc_expand, totals, src, step_w = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels,
+                                                              lats, prosody_weights)
+            dec = self.plm.begin_decode(src, sampling=sampling, keys=keys,
+                                        weights=prosody_weights if step_w is None else step_w, context=plm_context)
             pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
         B, Lmax, T = tc_expand.shape[0], tc_expand.shape[1], dec.T
         if Lmax < 1:

@@ -266,6 +266,23 @@ def adm_readout_mix(xl, w_predict, weights):
     return r, y
 
 
+def mix_step_weights(phone_w, durations, T):
+    """Per-phone mix weights (B, Tp, K) fp32 and phone durations (B, Tp) int32 -> the prosody LM's per-step weights
+    (B, T, K): step t takes the row of the phone owning the most of the mel frames [8t, 8t+8), the earlier phone on a tie;
+    steps past an utterance's end take its last phone with a positive duration (include/megatts2_b200.h,
+    mtts_mix_step_weights_f32).  The rows are copied, not recomputed."""
+    pw = _dev(phone_w, name="phone_w")
+    d = _dev(durations, torch.int32, "durations")
+    if pw.dim() != 3 or d.shape != pw.shape[:2]:
+        raise L.MttsError(f"mix_step_weights: phone_w (B, Tp, K) and durations (B, Tp), got {tuple(pw.shape)} and "
+                          f"{tuple(d.shape)}")
+    B, Tp, K = pw.shape
+    pw, d = pw.contiguous(), d.contiguous()
+    out = torch.empty(B, int(T), K, dtype=_F32, device=pw.device)
+    L.check(L.lib().mtts_mix_step_weights_f32(_ptr(pw), Tp * K, Tp, K, B, _ptr(d), Tp, int(T), _ptr(out), _stream()))
+    return out
+
+
 def philox4x32_10(ctr, key):
     """The sampler's generator: ctr (n, 4) and key (n, 2) uint32 words, as int64 tensors holding values < 2**32, ->
     (n, 4) words (int64, values < 2**32)."""

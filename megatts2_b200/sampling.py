@@ -69,31 +69,62 @@ class Sampling:
 MIX_MAX_SOURCES = 8
 
 
+def _real_weights(weights, what, shapes):
+    """``weights`` as a tensor of real numbers (not yet checked for shape or values)."""
+    try:
+        w = torch.as_tensor(weights).detach()
+    except (TypeError, ValueError, RuntimeError) as e:
+        raise L.MttsError(f"{what}: weights must be a {shapes} array of real numbers ({e})") from None
+    if w.dtype == torch.bool or w.is_complex() or not (w.is_floating_point() or w.dtype in (
+            torch.int64, torch.int32, torch.int16, torch.int8, torch.uint8)):
+        raise L.MttsError(f"{what}: weights must be real numbers, got {w.dtype}")
+    return w
+
+
+def _checked_rows(w64, what):
+    """fp64 weights whose last dim is one weight row -> the rows as a contiguous fp32 tensor, every weight finite and
+    >= 0 and every row with a positive fp32 sum."""
+    if not bool(torch.isfinite(w64).all()) or bool((w64 < 0).any()):
+        raise L.MttsError(f"{what}: every weight must be finite and >= 0")
+    w32 = w64.to(torch.float32).contiguous()
+    s = w32.sum(-1)
+    if not bool(torch.isfinite(s).all()) or bool((s <= 0).any()):
+        raise L.MttsError(f"{what}: every weight row needs a positive, finite sum")
+    return w32
+
+
 def mix_weights(weights, K, B, what="prosody mix"):
     """The mix weights of ``MegaPLM.infer_mix`` and ``MegaADM.infer_mix`` as a validated (B, K) fp32 CPU tensor:
     ``weights`` is (K,) (the same row for every utterance) or (B, K); every weight finite and >= 0, every row with a
     positive fp32 sum.  ``what`` names the mix in the error messages."""
     if not 1 <= K <= MIX_MAX_SOURCES:
         raise L.MttsError(f"{what}: K = {K} sources, expected 1 to {MIX_MAX_SOURCES}")
-    try:
-        w = torch.as_tensor(weights).detach()
-    except (TypeError, ValueError, RuntimeError) as e:
-        raise L.MttsError(f"{what}: weights must be a (K,) or (B, K) array of real numbers ({e})") from None
-    if w.dtype == torch.bool or w.is_complex() or not (w.is_floating_point() or w.dtype in (
-            torch.int64, torch.int32, torch.int16, torch.int8, torch.uint8)):
-        raise L.MttsError(f"{what}: weights must be real numbers, got {w.dtype}")
+    w = _real_weights(weights, what, "(K,) or (B, K)")
     w64 = w.to(device="cpu", dtype=torch.float64)
     if w64.dim() == 1:
         w64 = w64.unsqueeze(0).expand(B, -1)
     if tuple(w64.shape) != (B, K):
         raise L.MttsError(f"{what}: weights of shape {tuple(w.shape)}, expected ({K},) or ({B}, {K})")
-    if not bool(torch.isfinite(w64).all()) or bool((w64 < 0).any()):
-        raise L.MttsError(f"{what}: every weight must be finite and >= 0")
-    w32 = w64.to(torch.float32).contiguous()
-    s = w32.sum(1)
-    if not bool(torch.isfinite(s).all()) or bool((s <= 0).any()):
-        raise L.MttsError(f"{what}: every weight row needs a positive, finite sum")
-    return w32
+    return _checked_rows(w64, what)
+
+
+def per_step(weights):
+    """Whether mix weights are a schedule, (B, T, K) with one row per step, rather than one row per utterance."""
+    try:
+        return torch.as_tensor(weights).dim() == 3
+    except (TypeError, ValueError, RuntimeError):
+        return False
+
+
+def mix_step_weights(weights, K, B, T, what="prosody mix"):
+    """Mix weights that change along the utterance as a validated (B, T, K) fp32 CPU tensor: row (b, t) weighs the K
+    sources at step t of utterance b, under ``mix_weights``'s rules for each row."""
+    if not 1 <= K <= MIX_MAX_SOURCES:
+        raise L.MttsError(f"{what}: K = {K} sources, expected 1 to {MIX_MAX_SOURCES}")
+    w = _real_weights(weights, what, "(B, T, K)")
+    if tuple(w.shape) != (B, T, K):
+        raise L.MttsError(f"{what}: weights of shape {tuple(w.shape)}, expected ({B}, {T}, {K}) (one row per step)")
+    return _checked_rows(w.to(device="cpu", dtype=torch.float64), what)
 
 
 def row_keys(keys, rows, device):
