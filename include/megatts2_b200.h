@@ -117,7 +117,11 @@ typedef struct {
   int32_t accumulate;
   int64_t out_shift;                       /* 0 for ordinary convs */
   int64_t y_batch_elems;                   /* 0 -> Tout*ldy */
-  const int32_t* in_lens;                  /* optional (B): rows >= len read as zero / reflect about len */
+  const int32_t* in_lens;                  /* optional (B): item b's input is its first len = min(in_lens[b], Tin) rows;
+                                              a row index ti outside [0, len) reads as zero (MTTS_PAD_ZERO, or len <= 0),
+                                              as row 0 / len - 1 (MTTS_PAD_REPLICATE) or, MTTS_PAD_REFLECT, as its one
+                                              reflection about row 0 (-ti) or row len - 1 (2 (len - 1) - ti), and as zero
+                                              when that reflection is still outside (a len shorter than the halo) */
   /* tensor-core engine (optional): the same weights as three bf16 planes (3, k, Cout, Cin) and a scratch
    * buffer for the padded activation planes (>= 6*B*(Tout + dil*(k-1))*Cin + 2048 bytes).  Used when the
    * shape is eligible (stride 1, Cin % 8 == 0, Cin >= 32, Cout in {32, 64, >= 128 and % 32 == 0}). */
@@ -147,6 +151,15 @@ typedef struct {
 } mtts_conv_params;
 
 int mtts_conv1d_f32(const mtts_conv_params* p, void* stream);
+/* Diagnostics (host only, no CUDA call; of the pointers in *p only the alignment of x, w, y and res, whether res, in_lens
+ * and tc_scratch are NULL, and tc_scratch_bytes are read): the kernel mtts_conv1d_f32 launches for *p on the exact-fp32
+ * FFMA engine (the calls the tensor-core engine does not take) with n_sms SMs.  A K split (MTTS_FFMA_SPLITK) writes fp32
+ * partial sums into tc_scratch and reduces them in a fixed order.  out8 = {kernel (MTTS_FFMA_*; NONE: no output rows),
+ * rows BM and columns BN of a CTA's output tile (256 x 1 for the Cout = 1 kernels), K splits (1: unsplit), 16-channel
+ * K slices per split (0: unsplit), 16-byte loads of x (1) or scalar ones (0), the same for w, the same for the y / res
+ * epilogue}.  The argument checks and error codes are those of the launch. */
+enum { MTTS_FFMA_NONE = -1, MTTS_FFMA_TILE = 0, MTTS_FFMA_SPLITK = 1, MTTS_FFMA_COUT1 = 2, MTTS_FFMA_COUT1_TILED = 3 };
+int mtts_ffma_plan_query(const mtts_conv_params* p, int32_t n_sms, int32_t* out8);
 
 /* Tensor-core linear layer (wgmma, sm_90a): Y[M,N] = post(pre(X)[M,K] . W[N,K]^T + bias) (+ R) with
  * fp32-grade accuracy from split operands (fp32 accumulation in registers).  w_planes: (3, N, K) bf16 [BF16X3],

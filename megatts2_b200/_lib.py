@@ -118,6 +118,7 @@ SIGNATURES = {
     "mtts_trace_begin": (C.c_int, [vp]),
     "mtts_trace_end": (C.c_int, [C.c_char_p, i32]),
     "mtts_conv1d_f32": (C.c_int, [C.POINTER(ConvParams), vp]),
+    "mtts_ffma_plan_query": (C.c_int, [C.POINTER(ConvParams), i32, C.POINTER(i32)]),
     "mtts_linear_tc_scratch_bytes": (i64, [i64, i32]),
     "mtts_linear_tc_f32": (C.c_int, [vp, i32, i64, i32, vp, i32, vp, vp, i32, vp, i32, i32, f32, i32, vp, i64, i64, i32, vp]),
     "mtts_split_planes_f32": (C.c_int, [vp, i32, i64, i32, vp, i32, vp]),

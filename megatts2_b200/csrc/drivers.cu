@@ -1008,6 +1008,7 @@ int mtts_set_attention_pair_min(int32_t min_len) { return set_attention_pair_min
 int mtts_attention_plan_query(const mtts_attn_params* p, int32_t allow_f16_operands, int32_t pair_min, int32_t* out6) {
   return attention_plan_query(p, allow_f16_operands, pair_min, out6);
 }
+int mtts_ffma_plan_query(const mtts_conv_params* p, int32_t n_sms, int32_t* out8) { return ffma_plan_query(p, n_sms, out8); }
 int mtts_set_sm_limit(int32_t n_sms) { return set_sm_limit(n_sms); }
 int mtts_set_launch_policy(int32_t sm_limit, int32_t allow_pairs, int32_t allow_pdl) {
   return set_launch_policy(sm_limit, allow_pairs, allow_pdl);

@@ -99,6 +99,13 @@ static inline int engine_allows_f16_operands(int engine) { return engine == 2 ||
 int layernorm_ex(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr, float* y,
                  int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, PlanesOut po, cudaStream_t st);
 int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st);
+// conv1d_ffma()'s routing as a pure host function: ffma_check holds the argument checks, ffma_plan picks the kernel
+// (MTTS_FFMA_*) for an SM budget of `sms`: its output tile (BM x BN; 256 x 1 for the Cout = 1 kernels), the K split
+// (splits, 16-channel slices per split; 1, 0 unsplit), the 16-byte load / store paths and the dynamic shared memory
+struct FfmaPlan { int kernel, bm, bn, splits, kk_per_split, vec_a, vec_b, vec_y; size_t smem; };
+int ffma_check(const mtts_conv_params& p);
+FfmaPlan ffma_plan(const mtts_conv_params& p, int sms);
+int ffma_plan_query(const mtts_conv_params* p, int sms, int32_t* out8);
 int conv1d(const mtts_conv_params& p, cudaStream_t st);   // engine dispatch (FFMA today)
 bool conv_tc_eligible(const mtts_conv_params& p);
 // Optional LayerNorm of the rows a split-K tap-GEMM has just reduced (the dense layers of the AR loops' early steps): the

@@ -378,37 +378,36 @@ static int launch_cfg(const mtts_conv_params& p, const ConvFlags& fl, cudaStream
 
 static inline bool al16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
-int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st) {
+int ffma_check(const mtts_conv_params& p) {
   MTTS_REQUIRE(p.x && p.w && p.y, "null pointer");
   MTTS_REQUIRE(p.B >= 0 && p.Tin >= 0 && p.Tout >= 0 && p.Cin > 0 && p.Cout > 0, "bad dims");
   MTTS_REQUIRE(p.k >= 1 && p.stride >= 1 && p.dil >= 1, "bad conv geometry");
   MTTS_REQUIRE(p.ldx >= p.Cin, "ldx < Cin");
   MTTS_REQUIRE(p.pad_mode >= 0 && p.pad_mode <= 2, "bad pad_mode");
+  MTTS_REQUIRE((int64_t)p.B * p.Tout < (int64_t)2147483647 * 32, "too many rows");
+  return 0;
+}
+
+FfmaPlan ffma_plan(const mtts_conv_params& p, int sms) {
+  FfmaPlan pl{MTTS_FFMA_NONE, 0, 0, 1, 0, 0, 0, 0, 0};
   const int64_t M = (int64_t)p.B * p.Tout;
-  if (M == 0) return 0;
-  MTTS_REQUIRE(M < (int64_t)2147483647 * 32, "too many rows");
-  ConvFlags fl;
-  fl.kk_per_split = 0;
-  fl.partial = nullptr;
-  fl.vec_a = (p.Cin % 4 == 0) && (p.ldx % 4 == 0) && (p.x_batch_stride % 4 == 0) && al16(p.x);
-  fl.vec_b = (p.Cout % 4 == 0) && al16(p.w);
-  fl.vec_y = (p.Cout % 4 == 0) && (p.ldy % 4 == 0) && (p.y_batch_stride % 4 == 0) && al16(p.y) &&
+  if (M == 0) return pl;
+  pl.vec_a = (p.Cin % 4 == 0) && (p.ldx % 4 == 0) && (p.x_batch_stride % 4 == 0) && al16(p.x);
+  pl.vec_b = (p.Cout % 4 == 0) && al16(p.w);
+  pl.vec_y = (p.Cout % 4 == 0) && (p.ldy % 4 == 0) && (p.y_batch_stride % 4 == 0) && al16(p.y) &&
              (p.out_shift % 4 == 0) && (p.y_batch_elems % 4 == 0) &&
              (!p.res || ((p.ldr % 4 == 0) && (p.res_batch_stride % 4 == 0) && al16(p.res)));
-  if (p.Cout == 1 && p.out_shift == 0 && fl.vec_a && p.stride == 1 && (p.k * p.Cin) % 4 == 0 && p.Cin <= 128 && p.B <= 65535 &&
+  if (p.Cout == 1 && p.out_shift == 0 && pl.vec_a && p.stride == 1 && (p.k * p.Cin) % 4 == 0 && p.Cin <= 128 && p.B <= 65535 &&
       M >= 4096) {
     const size_t smem = sizeof(float) * ((size_t)((p.k * p.Cin + 3) & ~3) + (size_t)(256 + (p.k - 1) * p.dil) * (p.Cin + 4));
     if (smem <= 48 * 1024) {
-      dim3 grid((unsigned)cdiv64(p.Tout, 256), (unsigned)p.B);
-      launch_k(conv_cout1_tiled_kernel, grid, 256, smem, st, p);
-      MTTS_CHECK_LAUNCH();
-      return 0;
+      pl.kernel = MTTS_FFMA_COUT1_TILED; pl.bm = 256; pl.bn = 1; pl.smem = smem;
+      return pl;
     }
   }
-  if (p.Cout == 1 && p.out_shift == 0 && fl.vec_a && p.k * p.Cin <= 8192 && M >= 4096) {
-    launch_k(conv_cout1_kernel, (unsigned)cdiv64(M, 256), 256, (size_t)p.k * p.Cin * sizeof(float), st, p);
-    MTTS_CHECK_LAUNCH();
-    return 0;
+  if (p.Cout == 1 && p.out_shift == 0 && pl.vec_a && p.k * p.Cin <= 8192 && M >= 4096) {
+    pl.kernel = MTTS_FFMA_COUT1; pl.bm = 256; pl.bn = 1; pl.smem = (size_t)p.k * p.Cin * sizeof(float);
+    return pl;
   }
   // Small-M linear layers (the last-position GEMMs of the AR loops: M = batch rows): a 64x64 tile grid leaves
   // most SMs idle and every CTA walks all of K serially.  Split K over blockIdx.z into the caller's scratch and
@@ -416,7 +415,6 @@ int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st) {
   {
     const int64_t tiles64 = cdiv64(M, 64) * cdiv64(p.Cout, 64);
     const int nk = (p.Cin + 15) / 16;
-    const int sms = cur_device_sms();
     if (p.k == 1 && p.stride == 1 && p.pad == 0 && p.out_shift == 0 && !p.in_lens && M <= 256 && tiles64 <= sms &&
         nk >= 16 && p.tc_scratch) {
       // two CTAs per SM: a lone 8-warp CTA cannot hide the L2 latency of its one-chunk-ahead prefetch
@@ -424,23 +422,71 @@ int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st) {
       if (splits > 16) splits = 16;
       if (splits > nk / 4) splits = nk / 4;
       if (splits >= 2 && (int64_t)splits * M * p.Cout * 4 + 256 <= p.tc_scratch_bytes) {
-        fl.kk_per_split = (nk + splits - 1) / splits;
-        splits = (nk + fl.kk_per_split - 1) / fl.kk_per_split;
-        fl.partial = reinterpret_cast<float*>((((uintptr_t)p.tc_scratch) + 255) & ~(uintptr_t)255);
-        dim3 grid((unsigned)cdiv64(M, 64), (unsigned)cdiv64(p.Cout, 64), (unsigned)splits);
-        launch_k(tapconv_kernel<64, 64, 4, 4>, grid, 256, 0, st, p, fl);
-        MTTS_CHECK_LAUNCH();
-        launch_k(splitk_reduce_kernel, (unsigned)cdiv64(M * p.Cout, 256), 256, 0, st, p, fl.partial, splits);
-        MTTS_CHECK_LAUNCH();
-        return 0;
+        pl.kernel = MTTS_FFMA_SPLITK; pl.bm = 64; pl.bn = 64;
+        pl.kk_per_split = (nk + splits - 1) / splits;
+        pl.splits = (nk + pl.kk_per_split - 1) / pl.kk_per_split;
+        return pl;
       }
     }
   }
   const int64_t tiles128 = cdiv64(M, 128) * cdiv64(p.Cout, 128);
-  if (p.Cout <= 32) return launch_cfg<128, 32, 8, 4>(p, fl, st);
-  if (p.Cout <= 64) return launch_cfg<128, 64, 8, 4>(p, fl, st);
-  if (tiles128 >= 120) return launch_cfg<128, 128, 8, 8>(p, fl, st);
+  pl.kernel = MTTS_FFMA_TILE;
+  if (p.Cout <= 32) { pl.bm = 128; pl.bn = 32; }
+  else if (p.Cout <= 64) { pl.bm = 128; pl.bn = 64; }
+  else if (tiles128 >= 120) { pl.bm = 128; pl.bn = 128; }
+  else { pl.bm = 64; pl.bn = 64; }
+  return pl;
+}
+
+int conv1d_ffma(const mtts_conv_params& p, cudaStream_t st) {
+  MTTS_TRY(ffma_check(p));
+  if ((int64_t)p.B * p.Tout == 0) return 0;
+  const FfmaPlan pl = ffma_plan(p, cur_device_sms());
+  ConvFlags fl;
+  fl.vec_a = pl.vec_a;
+  fl.vec_b = pl.vec_b;
+  fl.vec_y = pl.vec_y;
+  fl.kk_per_split = pl.kk_per_split;
+  fl.partial = nullptr;
+  switch (pl.kernel) {
+    case MTTS_FFMA_COUT1_TILED: {
+      dim3 grid((unsigned)cdiv64(p.Tout, 256), (unsigned)p.B);
+      launch_k(conv_cout1_tiled_kernel, grid, 256, pl.smem, st, p);
+      MTTS_CHECK_LAUNCH();
+      return 0;
+    }
+    case MTTS_FFMA_COUT1:
+      launch_k(conv_cout1_kernel, (unsigned)cdiv64((int64_t)p.B * p.Tout, 256), 256, pl.smem, st, p);
+      MTTS_CHECK_LAUNCH();
+      return 0;
+    case MTTS_FFMA_SPLITK: {
+      const int64_t M = (int64_t)p.B * p.Tout;
+      fl.partial = reinterpret_cast<float*>((((uintptr_t)p.tc_scratch) + 255) & ~(uintptr_t)255);
+      dim3 grid((unsigned)cdiv64(M, 64), (unsigned)cdiv64(p.Cout, 64), (unsigned)pl.splits);
+      launch_k(tapconv_kernel<64, 64, 4, 4>, grid, 256, 0, st, p, fl);
+      MTTS_CHECK_LAUNCH();
+      launch_k(splitk_reduce_kernel, (unsigned)cdiv64(M * p.Cout, 256), 256, 0, st, p, fl.partial, pl.splits);
+      MTTS_CHECK_LAUNCH();
+      return 0;
+    }
+    default: break;
+  }
+  if (pl.bn == 32) return launch_cfg<128, 32, 8, 4>(p, fl, st);
+  if (pl.bn == 64 && pl.bm == 128) return launch_cfg<128, 64, 8, 4>(p, fl, st);
+  if (pl.bn == 128) return launch_cfg<128, 128, 8, 8>(p, fl, st);
   return launch_cfg<64, 64, 4, 4>(p, fl, st);
+}
+
+// diagnostics: the plan conv1d_ffma() launches for *p on `sms` SMs; out8 = {kernel (MTTS_FFMA_*), BM, BN, splits,
+// kk_per_split, vec_a, vec_b, vec_y}
+int ffma_plan_query(const mtts_conv_params* p, int sms, int32_t* out8) {
+  MTTS_REQUIRE(p && out8, "null params");
+  MTTS_REQUIRE(sms >= 1, "bad SM count");
+  MTTS_TRY(ffma_check(*p));
+  const FfmaPlan pl = ffma_plan(*p, sms);
+  out8[0] = pl.kernel; out8[1] = pl.bm; out8[2] = pl.bn; out8[3] = pl.splits;
+  out8[4] = pl.kk_per_split; out8[5] = pl.vec_a; out8[6] = pl.vec_b; out8[7] = pl.vec_y;
+  return 0;
 }
 
 }  // namespace mtts

@@ -51,111 +51,6 @@ def HIFI(weights_cpu):
 
 
 # ------------------------------------------------------------------------------ tap-GEMM
-CONV_CASES = [
-    # B, T, Cin, Cout, k, stride, dil, pad_mode, pre, post, res, acc, scale
-    dict(B=1, T=300, Cin=1024, Cout=4096, k=1),                                  # 64x64 tiles
-    dict(B=4, T=700, Cin=1024, Cout=1024, k=1, res=True),                        # 128x128 tiles
-    dict(B=2, T=125, Cin=20, Cout=384, k=5),                                     # Cin % 16 != 0
-    dict(B=2, T=131, Cin=512, Cout=80, k=5),                                     # Cout = 80
-    dict(B=3, T=257, Cin=32, Cout=1, k=7, pad_mode=1, pre=2, post=3),            # conv_post: reflect, leaky, tanh
-    dict(B=2, T=5000, Cin=32, Cout=1, k=7, pad_mode=1, pre=2, post=3),           # conv_post, single-channel kernel
-    dict(B=2, T=500, Cin=512, Cout=512, k=17, stride=16, pad=8),                 # MRTE strided conv
-    dict(B=2, T=200, Cin=64, Cout=64, k=11, dil=5, pad_mode=1, pre=2, res=True, acc=True, scale=1 / 3),
-    dict(B=2, T=333, Cin=32, Cout=32, k=3, dil=3, pad_mode=1, pre=2),            # 128x32 tiles
-    dict(B=1, T=97, Cin=7, Cout=5, k=3),                                         # scalar loads both sides
-    dict(B=5, T=1, Cin=768, Cout=768, k=1, res=True),                            # last-row GEMM shape (skinny kernel)
-    dict(B=64, T=1, Cin=4096, Cout=1024, k=1, res=True),                         # PLM final-layer FF2, skinny kernel
-    dict(B=1, T=64, Cin=1024, Cout=4096, k=1, post=1),                           # PLM final-layer FF1, skinny kernel
-    dict(B=16, T=2, Cin=1000, Cout=1000, k=1),                                   # skinny kernel, K and N tails
-    dict(B=2, T=64, Cin=80, Cout=512, k=7, pad_mode=1),                          # conv_pre
-    dict(B=2, T=50, Cin=16, Cout=24, k=5, pad_mode=2),                           # replicate padding
-]
-
-
-@pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
-def test_conv1d_vs_torch(case):
-    from megatts2_b200 import ops, pack
-    c = dict(stride=1, dil=1, pad_mode=0, pre=0, post=0, res=False, acc=False, scale=1.0)
-    c.update(case)
-    k, dil = c["k"], c["dil"]
-    pad = c.get("pad", dil * (k - 1) // 2)
-    g = gen(hash(str(case)) % 10000)
-    x = torch.randn(c["B"], c["T"], c["Cin"], generator=g)
-    w = torch.randn(c["Cout"], c["Cin"], k, generator=g) / math.sqrt(c["Cin"] * k)
-    b = torch.randn(c["Cout"], generator=g)
-    xin = x
-    if c["pre"] == 2:
-        xin = F.leaky_relu(x, 0.1)
-    elif c["pre"] == 1:
-        xin = F.relu(x)
-    xt = xin.transpose(1, 2)
-    if pad > 0 and c["pad_mode"] != 0:
-        xt = F.pad(xt, (pad, pad), mode={1: "reflect", 2: "replicate"}[c["pad_mode"]])
-        ref = F.conv1d(xt.double(), w.double(), b.double(), stride=c["stride"], dilation=dil)
-    else:
-        ref = F.conv1d(xt.double(), w.double(), b.double(), stride=c["stride"], dilation=dil, padding=pad)
-    ref = ref.transpose(1, 2)
-    if c["post"] == 3:
-        ref = torch.tanh(ref)
-    elif c["post"] == 1:
-        ref = torch.relu(ref)
-    res = torch.randn(ref.shape, generator=g) if c["res"] else None
-    y0 = torch.randn(ref.shape, generator=g) if c["acc"] else None
-    if res is not None:
-        ref = ref + res.double()
-    ref = ref * c["scale"]
-    if y0 is not None:
-        ref = ref + y0.double()
-    out = y0.clone().to(DEV) if y0 is not None else None
-    y = ops.conv1d(x.to(DEV), pack.pack_conv(w).to(DEV), b.to(DEV), k=k, stride=c["stride"], dil=dil, pad=pad,
-                   pad_mode=c["pad_mode"], pre_act=c["pre"], pre_slope=0.1, post_act=c["post"],
-                   res=res.to(DEV) if res is not None else None, out=out, out_scale=c["scale"], accumulate=c["acc"])
-    assert y.shape == ref.shape
-    # fp32 accumulation over K = Cin*k terms of O(1/sqrt(K)) products: error ~ 1e-6 * sqrt(K)
-    assert maxerr(y, ref) < 2e-5 * max(1.0, ref.abs().max().item())
-
-
-def test_conv1d_in_lens_and_strided_views():
-    from megatts2_b200 import ops, pack
-    g = gen(7)
-    x = torch.randn(3, 40, 48, generator=g)
-    w = torch.randn(16, 24, 5, generator=g) * 0.1
-    lens = torch.tensor([40, 17, 29], dtype=torch.int32)
-    xs = x[..., 8:32]                       # channel slice: ldx = 48, Cin = 24
-    ref = []
-    for b in range(3):
-        xb = xs[b:b + 1, :lens[b]].transpose(1, 2)
-        ref.append(F.conv1d(xb, w, None, padding=2).transpose(1, 2))
-    y = ops.conv1d(xs.to(DEV), pack.pack_conv(w).to(DEV), None, k=5, pad=2, in_lens=lens.to(DEV))
-    for b in range(3):
-        assert maxerr(y[b, :lens[b]], ref[b][0]) < 1e-5
-
-
-def test_conv_transpose_form_vs_torch():
-    from megatts2_b200 import _lib as L
-    from megatts2_b200 import ops, pack
-    import ctypes as C
-    g = gen(11)
-    for (cin, cout, s, T, B) in [(512, 256, 8, 37, 2), (128, 64, 2, 301, 3)]:
-        x = torch.randn(B, T, cin, generator=g)
-        w = torch.randn(cin, cout, 2 * s, generator=g) / math.sqrt(cin * 2)
-        b = torch.randn(cout, generator=g)
-        ref = F.conv_transpose1d(F.leaky_relu(x, 0.1).transpose(1, 2), w, b, stride=s, padding=s // 2).transpose(1, 2)
-        wp, bp = pack.pack_conv_transpose(w, b, s)
-        xd, wp, bp = x.to(DEV), wp.to(DEV), bp.to(DEV)
-        y = torch.empty(B, s * T, cout, device=DEV)
-        p = L.ConvParams()
-        p.x, p.x_batch_stride, p.ldx = xd.data_ptr(), T * cin, cin
-        p.w, p.bias = wp.data_ptr(), bp.data_ptr()
-        p.y, p.y_batch_stride, p.ldy = y.data_ptr(), s * T * cout, s * cout
-        p.B, p.Tin, p.Tout, p.Cin, p.Cout = B, T, T + 1, cin, s * cout
-        p.k, p.stride, p.dil, p.pad, p.pad_mode = 2, 1, 1, 1, 0
-        p.pre_act, p.pre_slope, p.out_scale = L.ACT_LEAKY, 0.1, 1.0
-        p.out_shift, p.y_batch_elems = -(s // 2) * cout, s * T * cout
-        L.check(L.lib().mtts_conv1d_f32(C.byref(p), ops._stream()))
-        assert maxerr(y, ref) < 2e-5
-
-
 def test_conv_linearity_property_full_size():
     """size-independent property at a BASELINE-size GEMM: f(a x1 + x2) == a f(x1) + f(x2) (no bias)."""
     from megatts2_b200 import ops
