@@ -23,7 +23,7 @@ constexpr int MEL_WARPS = 8, MEL_ROUNDS = 2, MEL_FPB = MEL_WARPS * MEL_ROUNDS;  
 // so that the float view of the buffer (the frame's 513 magnitudes, written over it after the untangle) has a frame
 // stride of 4 mod 32 banks and 16-byte aligned rows
 constexpr int MEL_ZPAD = 546;
-constexpr int MEL_FBW = 1536;                   // grouped filterbank floats staged in shared memory (slaney 80 x 513: 1392)
+constexpr int MEL_FBW = 1536;                   // grouped filterbank floats staged in shared memory (slaney 80: 1344, slaney 128: 1584)
 constexpr int MEL_MAXG = 32;                    // groups of 4 mels
 constexpr int MEL_SPAN = MEL_NFFT + (MEL_FPB - 1) * MEL_HOP;   // 4864 samples cover the CTA's 16 frames
 

@@ -58,6 +58,46 @@ def test_peak_normalize_and_prompt_loader():
         assert abs(float(wav[i, :n].abs().max()) - 1.0) < 1e-6
 
 
+def test_peak_normalize_long_clips():
+    """Clips past 131072 samples run on the 64-CTA cap, each CTA striding over the clip: the peak in the last sample, a
+    negative peak, and a larger value just past lens[b] that must not count."""
+    L = 200003
+    x = (torch.rand(3, L, generator=gen(11)) - 0.5).numpy()
+    x[0, L - 1] = 0.75
+    x[1, 150001] = -1.7
+    lens = np.array([L, L, 180000], dtype=np.int32)
+    x[2, 179999], x[2, 180000] = 0.625, 5.0
+    y = audio.peak_normalize(torch.from_numpy(x).to(DEV), torch.from_numpy(lens).to(DEV)).cpu().numpy()
+    for b in range(3):
+        n = int(lens[b])
+        peak = np.abs(x[b, :n]).max()
+        assert peak == np.float32((0.75, 1.7, 0.625)[b]), b
+        assert np.array_equal(y[b, :n], x[b, :n] / peak), b                      # one IEEE division per sample
+        assert np.array_equal(y[b, n:], x[b, n:]), b
+
+
+def test_pcm16_exact_edges():
+    """round-to-nearest-even of x * 32768, saturated to [-32768, 32767]: every tie (k + 0.5) / 32768, +-1 and just past,
+    on a length that is not a multiple of the 256-thread block"""
+    from megatts2_b200 import _lib as L
+    from megatts2_b200 import ops
+    ties = (np.arange(-32768, 32768, dtype=np.float64) + 0.5) / 32768
+    one = np.float32(1.0)
+    edges = [1.0, -1.0, np.nextafter(one, 2), -np.nextafter(one, 2), np.nextafter(one, 0), -np.nextafter(one, 0), 1.5,
+             -2.0, 32767 / 32768, -32767 / 32768, 0.0, -0.0, 0.5 / 32768, -0.5 / 32768, 1.5 / 32768, -1.5 / 32768]
+    x = np.concatenate([ties, np.asarray(edges, dtype=np.float64), np.linspace(-1.1, 1.1, 1001)]).astype(np.float32)
+    n = x.size
+    assert n % 256 != 0
+    out = torch.full((n + 7,), 12345, dtype=torch.int16, device=DEV)
+    L.check(L.lib().mtts_pcm16_f32(torch.from_numpy(x).to(DEV).data_ptr(), n, out.data_ptr(), ops._stream()))
+    out = out.cpu().numpy()
+    ref = np.clip(np.rint(x * np.float32(32768)), -32768, 32767).astype(np.int16)                # np.rint: ties to even
+    assert np.array_equal(out[:n], ref)
+    assert (out[n:] == 12345).all()
+    assert out[65536] == 32767 and out[65537] == -32768 and out[65538] == 32767 and out[65539] == -32768
+    assert (out[0], out[1], out[32767], out[32768], out[65535]) == (-32768, -32766, 0, 0, 32767)           # ties to even
+
+
 def test_wav_writer(tmp_path):
     w = (torch.rand(1, 4097, generator=gen(9)) * 2.2 - 1.1).to(DEV)             # includes samples beyond +-1 (saturation)
     pf, pi = str(tmp_path / "f.wav"), str(tmp_path / "i.wav")
