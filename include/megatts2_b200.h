@@ -651,6 +651,47 @@ int mtts_adm_infer_mix_steps_f32(const mtts_adm* m, int32_t K, const float* tc_l
                                  int32_t* dur_out, float* raw_out, float* raw_src_out, void* workspace,
                                  int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Duration control: phone durations pinned inside the ADM loop, and durations fitted to a speaking rate and a target
+ * length.
+ *
+ * Pins.  pinned (B, T) int32 device, utterance b at pinned + b*pin_sb; pinned[b, t] >= 1 pins phone t of b to that many
+ * frames, a value < 1 (conventionally -1) leaves it free.  At step t the value written into the raw history p[b, t+1] is
+ * (float)pinned[b, t] for a pinned phone and the readout (plain, mixed or scheduled) otherwise, so the rest of the
+ * utterance is decoded after the pinned values.  The reference trains the ADM teacher-forced on integer frame counts cast
+ * to float and skips cuts with a duration >= 128, so a pin in 1..127 is the kind of history the model was trained on.
+ * The durations follow from the history as before; for p in 1..127, (p + 0.5) truncates to p, so a pinned phone comes
+ * out exactly p, and raw_out holds p there.  raw_src_out keeps every source's own readout, pinned or not.
+ * mtts_adm_infer_pinned_f32 takes mtts_adm_infer_mix_steps_f32's arguments (weights NULL only when K = 1: then with
+ * raw_src_out NULL it is the plain decode; (B, K) weights are w_sb = K, w_st = 0) and the pins; pinned NULL pins
+ * nothing.  The pins are read from device memory at every call, so a replayed CUDA graph picks up new pins.  With every
+ * pin < 1 the outputs equal the unpinned entry's bit for bit, with the same launch sequence.  Workspace:
+ * mtts_adm_infer_mix_workspace_bytes.  The causal decode takes no pins. */
+int mtts_adm_infer_pinned_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                              int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st, int32_t* dur_out,
+                              float* raw_out, float* raw_src_out, const int32_t* pinned, int64_t pin_sb, void* workspace,
+                              int64_t workspace_bytes, void* stream);
+/* The fit.  raw (B, Tp) fp32 device, utterance b at raw + b*raw_sb: the ADM's raw values.  scale optional (NULL = 1):
+ * c[b, i] at scale + b*scale_sb + i*scale_st, so strides (0, 0) give one scalar, (1, 0) one value per utterance and
+ * (Tp, 1) one per phone.  pinned optional, as above (pinned phones get their pin).  total optional (B,) int32 device.
+ * dur_out (B, Tp) int32, utterance b at dur_out + b*dur_sb.  For utterance b, F is its set of free phones and
+ * w_i = fl32(raw_i * c_i), a non-finite w or a w <= 0 counting as 0.
+ *   No total: free phone i gets clamp(trunc(fl32(w_i + 0.5)), 1, 128), the ADM's own rounding applied to w; with c = 1
+ *   that is mtts_adm_infer_f32's dur_out, bit for bit.  For finite w the fp32 add never moves the truncation across an
+ *   integer, so this is clamp(floor(w_i + 1/2), 1, 128) exactly.
+ *   Total L_b: N = L_b - sum of pins - |F| frames above one per free phone, 0 <= N <= 127 |F| (the feasible totals are
+ *   [|F| + sum pins, 128 |F| + sum pins]; the host validates them, the device clamps N into that range).  The candidates
+ *   are v_ik = w_i / (k + 1/2), i in F, k = 1..127; the N largest are taken, ordered by value descending, then phone
+ *   index ascending, and free phone i gets 1 + (the number of its candidates taken).  This is Sainte-Lague apportionment
+ *   with per-phone bounds 1 and 128: the same as rounding w_i / theta for one common theta, so theta = 1 is the no-total
+ *   rule and durations that already sum to L_b come back unchanged.  Candidates compare exactly, as w_i (2m+1) against
+ *   w_j (2k+1).
+ * One CTA per utterance; 1 <= Tp <= 8192 (MTTS_ERR_UNSUPPORTED above); B <= 0 does nothing.  Device-only, so it can be
+ * captured in a CUDA graph. */
+int mtts_fit_durations_f32(const float* raw, int64_t raw_sb, int32_t Tp, int32_t B, const float* scale, int64_t scale_sb,
+                           int64_t scale_st, const int32_t* pinned, int64_t pin_sb, const int32_t* total, int32_t* dur_out,
+                           int64_t dur_sb, void* stream);
+
 /* ConvNet family (modules/convnet.py).  One ConvBlock = ReLU -> Conv1d(C,C,k,same) -> LN(C). */
 typedef struct { const float *w, *b, *ln_g, *ln_b; const void* w_tc; } mtts_conv_block;   /* w packed (k,C,C); w_tc (3,k,C,C) bf16 or NULL */
 

@@ -174,6 +174,9 @@ SIGNATURES = {
     "mtts_adm_infer_mix_f32": (C.c_int, [C.POINTER(ADM), i32, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp]),
     "mtts_adm_infer_mix_steps_f32": (C.c_int, [C.POINTER(ADM), i32, vp, i64, i32, i32, i32, vp, i64, i64, vp, vp, vp, vp,
                                                i64, vp]),
+    "mtts_adm_infer_pinned_f32": (C.c_int, [C.POINTER(ADM), i32, vp, i64, i32, i32, i32, vp, i64, i64, vp, vp, vp, vp, i64,
+                                            vp, i64, vp]),
+    "mtts_fit_durations_f32": (C.c_int, [vp, i64, i32, i32, vp, i64, i64, vp, i64, vp, vp, i64, vp]),
     "mtts_plm_decode_causal_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32]),
     "mtts_plm_decode_causal_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, vp, vp, i64, vp]),
     "mtts_adm_decode_causal_workspace_bytes": (i64, [C.POINTER(ADM), i32, i32]),

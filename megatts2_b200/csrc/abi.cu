@@ -128,6 +128,13 @@ int mtts_mix_step_weights_f32(const float* phone_w, int64_t pw_sb, int32_t Tp, i
   return mix_step_weights(phone_w, pw_sb, Tp, K, B, durations, dur_sb, T, out, (cudaStream_t)stream);
 }
 
+int mtts_fit_durations_f32(const float* raw, int64_t raw_sb, int32_t Tp, int32_t B, const float* scale, int64_t scale_sb,
+                           int64_t scale_st, const int32_t* pinned, int64_t pin_sb, const int32_t* total, int32_t* dur_out,
+                           int64_t dur_sb, void* stream) {
+  return fit_durations(raw, raw_sb, Tp, B, scale, scale_sb, scale_st, pinned, pin_sb, total, dur_out, dur_sb,
+                       (cudaStream_t)stream);
+}
+
 int mtts_sample_rows_f32(const float* logits, int64_t ld, int32_t V, int32_t rows, int32_t step, const mtts_sampling* s,
                          int64_t* out, int64_t ld_out, void* stream) {
   MTTS_REQUIRE(s, "null sampling parameters");

@@ -365,16 +365,18 @@ static int64_t adm_ws_floats(const mtts_adm* m, int B, int T) {
 // b), all reading the shared (B, T+1) raw history.  tc_linear_emb and each step's encoder run once over the K*B rows, then
 // adm_readout_mix writes the mixed value into the history (and, with raw_src_out (K, B, T), every source's readout).
 // Step t of utterance b reads the weight row weights + b w_sb + t w_st (w_st = 0: one row for every step).
-// K = 1 without weights or raw_src_out is the plain decode.
+// K = 1 without weights or raw_src_out is the plain decode.  pin (optional, (B, T) at batch stride pin_sb): step t of
+// utterance b feeds back pin[b, t] instead of its readout when that pin is >= 1 (mtts_adm_infer_pinned_f32).
 static int adm_infer(const mtts_adm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int32_t* dur_out,
                      float* raw_out, void* ws, int64_t ws_bytes, cudaStream_t st, int K = 1, const float* weights = nullptr,
-                     int64_t w_sb = 0, int64_t w_st = 0, float* raw_src_out = nullptr) {
+                     int64_t w_sb = 0, int64_t w_st = 0, float* raw_src_out = nullptr, const int32_t* pin = nullptr,
+                     int64_t pin_sb = 0) {
   const int D = m->enc.d_model;
   MTTS_REQUIRE(D == m->emb_dim + m->tc_emb_dim, "d_model != emb_dim + tc_emb_dim");
   MTTS_REQUIRE(tc && dur_out && m->w_dt && m->w_tc && m->w_predict && m->pe, "null pointer");
   MTTS_TRY(adm_mix_check(K));
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
-  MTTS_REQUIRE(w_sb >= 0 && w_st >= 0, "weight strides must be >= 0");
+  MTTS_REQUIRE(w_sb >= 0 && w_st >= 0 && pin_sb >= 0, "strides must be >= 0");
   if (B <= 0 || T <= 0) return 0;
   const bool mix = weights || raw_src_out;
   const int R = K * B;                                       // latent rows: the K sources of the B utterances
@@ -409,9 +411,9 @@ static int adm_infer(const mtts_adm* m, const float* tc, int64_t tc_sb, int tc_l
     MTTS_TRY(encoder_forward(&m->enc, X, xl, R, S, nullptr, 0, 0, 0, 1, ar, &tcs, st));
     if (mix)
       MTTS_TRY(adm_readout_mix(xl, D, m->w_predict, K, B, weights ? weights + t * w_st : nullptr, w_sb, praw + (t + 1),
-                               T + 1, raw_src_out ? raw_src_out + t : nullptr, T, st));
+                               T + 1, raw_src_out ? raw_src_out + t : nullptr, T, st, pin ? pin + t : nullptr, pin_sb));
     else
-      MTTS_TRY(adm_readout(xl, D, m->w_predict, B, praw, T + 1, t + 1, st));
+      MTTS_TRY(adm_readout(xl, D, m->w_predict, B, praw, T + 1, t + 1, st, pin ? pin + t : nullptr, pin_sb));
   }
   MTTS_TRY(adm_finalize(praw, T + 1, B, T, dur_out, raw_out, st));
   return 0;
@@ -1153,6 +1155,15 @@ int mtts_adm_infer_mix_steps_f32(const mtts_adm* m, int32_t K, const float* tc_l
   MTTS_REQUIRE(m && m->enc.layers && workspace && weights, "null pointer");
   return adm_infer(m, tc_latent, tc_sb, tc_ld, B, T, dur_out, raw_out, workspace, workspace_bytes, (cudaStream_t)stream,
                    K, weights, w_sb, w_st, raw_src_out);
+}
+
+int mtts_adm_infer_pinned_f32(const mtts_adm* m, int32_t K, const float* tc_latent, int64_t tc_sb, int32_t tc_ld,
+                              int32_t B, int32_t T, const float* weights, int64_t w_sb, int64_t w_st, int32_t* dur_out,
+                              float* raw_out, float* raw_src_out, const int32_t* pinned, int64_t pin_sb, void* workspace,
+                              int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace, "null pointer");
+  return adm_infer(m, tc_latent, tc_sb, tc_ld, B, T, dur_out, raw_out, workspace, workspace_bytes, (cudaStream_t)stream,
+                   K, weights, w_sb, w_st, raw_src_out, pinned, pin_sb);
 }
 
 int64_t mtts_plm_decode_causal_workspace_bytes(const mtts_plm* m, int32_t B, int32_t T) {

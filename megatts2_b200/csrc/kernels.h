@@ -202,16 +202,23 @@ int fill_f32(float* p, int64_t stride, int n, float v, cudaStream_t st);
 int adm_build_input(const float* tc_emb, int64_t te_sb, int te_ld, int tc_emb_dim, const float* praw, int p_ld,
                     int B_hist, const float* w_dt, int emb_dim, const float* pe, float alpha, int B, int S, float* X,
                     cudaStream_t st);
-int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st);
+// pin (optional): the pins of this step's phone, utterance b at pin[b * pin_sb]; a pin >= 1 is fed back in place of the
+// readout (mtts_adm_infer_pinned_f32)
+int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st,
+                const int32_t* pin = nullptr, int64_t pin_sb = 0);
 // duration mix: r_b from the K rows k*B + b of xl and the weight rows weights + b ldw into out[b * ld_out]; y_out
 // (optional) gets every source's readout.  adm_mix_check validates K before a driver enqueues anything.
 int adm_mix_check(int K);
 int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, int64_t ldw, float* out,
-                    int64_t ld_out, float* y_out, int64_t ld_y, cudaStream_t st);
+                    int64_t ld_out, float* y_out, int64_t ld_y, cudaStream_t st, const int32_t* pin = nullptr,
+                    int64_t pin_sb = 0);
 // per-phone mix weights (B, Tp, K) -> per-PLM-step weights (B, T, K) by the durations (mtts_mix_step_weights_f32)
 int mix_step_weights(const float* pw, int64_t pw_sb, int Tp, int K, int B, const int32_t* dur, int64_t dur_sb, int T,
                      float* out, cudaStream_t st);
 int adm_finalize(const float* praw, int p_ld, int B, int T, int32_t* dur, float* raw_out, cudaStream_t st);
+// raw ADM values -> durations fitted to a scale, pins and a target total (mtts_fit_durations_f32)
+int fit_durations(const float* raw, int64_t raw_sb, int Tp, int B, const float* scale, int64_t sc_sb, int64_t sc_st,
+                  const int32_t* pin, int64_t pin_sb, const int32_t* total, int32_t* dur, int64_t dur_sb, cudaStream_t st);
 
 // convenience: dense linear layer  Y[M,N] = act(X[M,K] W + b) (+ res)
 inline mtts_conv_params linear_params(const float* x, int ldx, const float* w, const float* bias, float* y, int ldy,

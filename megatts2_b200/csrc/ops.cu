@@ -952,19 +952,29 @@ __device__ __forceinline__ float adm_readout_dot(const float* __restrict__ xl, i
   return warp_sum(s);
 }
 
+// The value a step feeds back: a pinned phone (pin[b pin_sb] >= 1, pin already at this step's phone) its frame count,
+// any other phone the readout r.
+__device__ __forceinline__ float adm_pinned(float r, const int32_t* __restrict__ pin, int64_t pin_sb, int b) {
+  if (!pin) return r;
+  const int32_t p = pin[(int64_t)b * pin_sb];
+  return p >= 1 ? (float)p : r;
+}
+
 // ADM readout (models/megatts2.py:272-273): p[b, s_next] = x_last[b,:] . w_predict ; one warp per b
 __global__ void adm_readout_kernel(const float* __restrict__ xl, int D, const float* __restrict__ w, int B,
-                                   float* __restrict__ praw, int p_ld, int s_next) {
+                                   float* __restrict__ praw, int p_ld, int s_next, const int32_t* __restrict__ pin,
+                                   int64_t pin_sb) {
   pdl_entry();
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (b >= B) return;
   const float s = adm_readout_dot(xl, b, D, w, lane);
-  if (lane == 0) praw[(int64_t)b * p_ld + s_next] = s;
+  if (lane == 0) praw[(int64_t)b * p_ld + s_next] = adm_pinned(s, pin, pin_sb, b);
 }
-int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st) {
+int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int p_ld, int s_next, cudaStream_t st,
+                const int32_t* pin, int64_t pin_sb) {
   if (B <= 0) return 0;
-  launch_k(adm_readout_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, B, praw, p_ld, s_next);
+  launch_k(adm_readout_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, B, praw, p_ld, s_next, pin, pin_sb);
   MTTS_CHECK_LAUNCH();
   return 0;
 }
@@ -975,7 +985,8 @@ int adm_readout(const float* xl, int D, const float* w, int B, float* praw, int 
 constexpr int ADM_MIX_MAX_K = 8;
 __global__ void adm_readout_mix_kernel(const float* __restrict__ xl, int D, const float* __restrict__ w, int K, int B,
                                        const float* __restrict__ weights, int64_t ldw, float* __restrict__ out,
-                                       int64_t ld_out, float* __restrict__ y_out, int64_t ld_y) {
+                                       int64_t ld_out, float* __restrict__ y_out, int64_t ld_y,
+                                       const int32_t* __restrict__ pin, int64_t pin_sb) {
   pdl_entry();
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -1002,7 +1013,7 @@ __global__ void adm_readout_mix_kernel(const float* __restrict__ xl, int D, cons
     r = first ? wn * y : fmaf(wn, y, r);
     first = false;
   }
-  if (lane == 0) out[(int64_t)b * ld_out] = r;
+  if (lane == 0) out[(int64_t)b * ld_out] = adm_pinned(r, pin, pin_sb, b);
 }
 
 int adm_mix_check(int K) {
@@ -1013,14 +1024,14 @@ int adm_mix_check(int K) {
 }
 
 int adm_readout_mix(const float* xl, int D, const float* w, int K, int B, const float* weights, int64_t ldw, float* out,
-                    int64_t ld_out, float* y_out, int64_t ld_y, cudaStream_t st) {
+                    int64_t ld_out, float* y_out, int64_t ld_y, cudaStream_t st, const int32_t* pin, int64_t pin_sb) {
   MTTS_TRY(adm_mix_check(K));
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
   MTTS_REQUIRE(D >= 1 && ldw >= 0 && ld_out >= 0 && ld_y >= 0, "D must be >= 1 and ld >= 0");
   if (B <= 0) return 0;
   MTTS_REQUIRE(xl && w && out, "null pointer");
   launch_k(adm_readout_mix_kernel, (unsigned)cdiv64(B, 4), 128, 0, st, xl, D, w, K, B, weights, ldw, out, ld_out, y_out,
-           ld_y);
+           ld_y, pin, pin_sb);
   MTTS_CHECK_LAUNCH();
   return 0;
 }
@@ -1130,6 +1141,139 @@ __global__ void adm_finalize_kernel(const float* __restrict__ praw, int p_ld, in
 int adm_finalize(const float* praw, int p_ld, int B, int T, int32_t* dur, float* raw_out, cudaStream_t st) {
   if (B * T <= 0) return 0;
   launch_k(adm_finalize_kernel, (unsigned)cdiv64((int64_t)B * T, 256), 256, 0, st, praw, p_ld, B, T, dur, raw_out);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
+// Duration fit (the contract is stated with mtts_fit_durations_f32 in include/megatts2_b200.h): one CTA per utterance,
+// each thread a contiguous run of phones.  Free phone i with weight w_i >= 0 has the candidates v_ik = fl64(w_i / (k + ½)),
+// k = 1..FIT_EXTRA.  fp64 division is correctly rounded and two different candidates differ by at least 2^-33 of their
+// size (w_i (2k+1) vs w_j (2m+1) are fp32 values times integers <= 255), so the fp64 values order and tie exactly as the
+// rationals do.  The CTA bisects the bit pattern of a threshold th >= 0 for the largest th with N candidates >= th (the
+// N-th largest candidate), then gives each phone its candidates > th and hands the N - #(> th) candidates equal to th to
+// the phones in index order by a block scan.
+constexpr int FIT_THREADS = 256;
+constexpr int FIT_MAX_TP = 8192;
+constexpr int FIT_EXTRA = 127;            // frames above the first that a free phone can take (durations 1..128)
+
+// #{k in 1..FIT_EXTRA : fl64(w / (k + 0.5)) >= th} for w >= 0, th >= 0: an estimate, then exact steps to the boundary
+__device__ __forceinline__ int fit_count_ge(float w, double th) {
+  if (th <= 0.0) return FIT_EXTRA;
+  if (w <= 0.f) return 0;
+  const double wd = w;
+  const double e = wd / th - 0.5;
+  int k = e >= (double)FIT_EXTRA ? FIT_EXTRA : (e < 1.0 ? 0 : (int)e);
+  while (k < FIT_EXTRA && wd / (k + 1.5) >= th) ++k;
+  while (k > 0 && wd / (k + 0.5) < th) --k;
+  return k;
+}
+
+// block-wide sums of two ints; every thread gets them.  s holds 2 * (FIT_THREADS / 32) ints.
+__device__ __forceinline__ int2 fit_block_sum2(int a, int c, int* s) {
+  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    c += __shfl_xor_sync(0xffffffffu, c, o);
+  }
+  __syncthreads();                                           // s is free: the previous call's readers are done
+  if (lane == 0) { s[wp] = a; s[FIT_THREADS / 32 + wp] = c; }
+  __syncthreads();
+  int2 r = make_int2(0, 0);
+#pragma unroll
+  for (int i = 0; i < FIT_THREADS / 32; ++i) { r.x += s[i]; r.y += s[FIT_THREADS / 32 + i]; }
+  return r;
+}
+
+__global__ void __launch_bounds__(FIT_THREADS)
+fit_durations_kernel(const float* __restrict__ raw, int64_t raw_sb, int Tp, const float* __restrict__ scale,
+                     int64_t sc_sb, int64_t sc_st, const int32_t* __restrict__ pin, int64_t pin_sb,
+                     const int32_t* __restrict__ total, int32_t* __restrict__ dur, int64_t dur_sb) {
+  extern __shared__ float w_s[];                              // Tp: w_i of a free phone, -1 for a pinned one
+  __shared__ int s_red[2 * (FIT_THREADS / 32)];
+  pdl_entry();
+  const int b = blockIdx.x, lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+  const int per = (Tp + FIT_THREADS - 1) / FIT_THREADS;
+  const int i0 = min((int)threadIdx.x * per, Tp), i1 = min(i0 + per, Tp);
+  int32_t* d = dur + (int64_t)b * dur_sb;
+  int n_free = 0, pinned = 0;
+  for (int i = i0; i < i1; ++i) {
+    const int32_t p = pin ? pin[(int64_t)b * pin_sb + i] : -1;
+    if (p >= 1) {
+      w_s[i] = -1.f;
+      pinned += p;
+      d[i] = p;
+      continue;
+    }
+    const float c = scale ? scale[(int64_t)b * sc_sb + (int64_t)i * sc_st] : 1.f;
+    float w = __fmul_rn(raw[(int64_t)b * raw_sb + i], c);
+    if (!(w > 0.f) || isinf(w)) w = 0.f;                      // NaN, +-inf and w <= 0 count as 0
+    w_s[i] = w;
+    ++n_free;
+    if (!total) {                                             // adm_finalize's rounding of w
+      const int v = (int)(w + 0.5f);
+      d[i] = v < 1 ? 1 : (v > FIT_EXTRA + 1 ? FIT_EXTRA + 1 : v);
+    }
+  }
+  if (!total) return;
+  const int2 fp = fit_block_sum2(n_free, pinned, s_red);
+  // frames above one per free phone; the host checks feasibility, the device clamps to the feasible range
+  const int N = max(0, min(total[b] - fp.y - fp.x, FIT_EXTRA * fp.x));
+  // the largest th (as fp64 bits) with F(th) = #{candidates >= th} >= N: F(0) = FIT_EXTRA |F| >= N, F(+inf) = 0 < N
+  unsigned long long lo = 0ull, hi = 0x7FF0000000000000ull;
+  while (N > 0 && hi - lo > 1) {
+    const unsigned long long mid = lo + ((hi - lo) >> 1);
+    const double th = __longlong_as_double((long long)mid);
+    int cnt = 0;
+    for (int i = i0; i < i1; ++i)
+      if (w_s[i] >= 0.f) cnt += fit_count_ge(w_s[i], th);
+    if (fit_block_sum2(cnt, 0, s_red).x >= N) lo = mid; else hi = mid;
+  }
+  // each free phone: g candidates > th (>= the next double), e == th; the N - G ties go to the lowest phone indices
+  const double th = __longlong_as_double((long long)lo), th_up = __longlong_as_double((long long)hi);
+  int g_own = 0, e_own = 0;
+  for (int i = i0; i < i1; ++i)
+    if (N > 0 && w_s[i] >= 0.f) {
+      const int g = fit_count_ge(w_s[i], th_up);
+      g_own += g;
+      e_own += fit_count_ge(w_s[i], th) - g;
+    }
+  const int G = fit_block_sum2(g_own, 0, s_red).x;
+  int incl = e_own;                                          // block scan of the ties: warp shuffles, then warp totals
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  __syncthreads();
+  if (lane == 31) s_red[wp] = incl;
+  __syncthreads();
+  int before = incl - e_own;
+  for (int j = 0; j < wp; ++j) before += s_red[j];
+  int left = N - G - before;                                 // ties still to hand out when this thread's run starts
+  for (int i = i0; i < i1; ++i) {
+    if (w_s[i] < 0.f) continue;
+    int g = 0, t = 0;
+    if (N > 0) {
+      g = fit_count_ge(w_s[i], th_up);
+      const int e = fit_count_ge(w_s[i], th) - g;
+      t = max(0, min(left, e));
+      left -= e;
+    }
+    d[i] = 1 + g + t;
+  }
+}
+
+int fit_durations(const float* raw, int64_t raw_sb, int Tp, int B, const float* scale, int64_t sc_sb, int64_t sc_st,
+                  const int32_t* pin, int64_t pin_sb, const int32_t* total, int32_t* dur, int64_t dur_sb, cudaStream_t st) {
+  MTTS_REQUIRE(Tp >= 1, "Tp must be >= 1");
+  if (Tp > FIT_MAX_TP)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: Tp = %lld phones is above the bound of %lld", "fit_durations", Tp, FIT_MAX_TP);
+  MTTS_REQUIRE(raw_sb >= 0 && sc_sb >= 0 && sc_st >= 0 && pin_sb >= 0 && dur_sb >= 0, "strides must be >= 0");
+  if (B <= 0) return 0;
+  MTTS_REQUIRE(raw && dur, "null pointer");
+  launch_k(fit_durations_kernel, (unsigned)B, FIT_THREADS, (size_t)Tp * sizeof(float), st, raw, raw_sb, Tp, scale, sc_sb,
+           sc_st, pin, pin_sb, total, dur, dur_sb);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

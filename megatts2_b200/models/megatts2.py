@@ -533,33 +533,44 @@ class MegaADM(pack.PlanMixin, nn.Module):
         pred = ops.linear(h, pack.pack_linear(self.predict_layer.weight))[..., 0]
         return pred, duration_tokens[:, 1:, 0]
 
-    def infer(self, tc_latents: torch.Tensor, return_raw: bool = False):
+    def infer(self, tc_latents: torch.Tensor, return_raw: bool = False, pinned=None):
         """AR duration regression, raw float feedback, non-causal full recompute, final
         (p + 0.5) -> int32 -> clamp(1, 128)  (models/megatts2.py:257-275).
-        tc_latents (B,T,512) -> (B,T,1) int32 [, raw (B,T) fp32]."""
+        tc_latents (B,T,512) -> (B,T,1) int32 [, raw (B,T) fp32].
+
+        ``pinned`` (B, T) ints, -1 free or 1..127 frames: a pinned phone's value is fed back into the loop in place of
+        the prediction, so the later phones are decoded after it, and it comes out exactly as pinned (raw holds it too;
+        include/megatts2_b200.h, mtts_adm_infer_pinned_f32).  The pins are an input of the replayed CUDA graph."""
         _eval_only(self)
         tc = _dev_rows(tc_latents, "tc_latents")
         B, T, _ = tc.shape
+        pin = None if pinned is None else S.pinned_durations(pinned, B, T).to(tc.device)
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
 
-        def run(tc_):
+        def run(tc_, *pin_):
             dur = torch.empty(B, T, dtype=torch.int32, device=tc_.device)
             raw = torch.empty(B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
+            outs = (dur.data_ptr(), raw.data_ptr() if return_raw else None)
+            if pin_:
+                ws = ops.workspace(lib.mtts_adm_infer_mix_workspace_bytes(C.byref(pl.struct), 1, B, T), tc_.device)
+                L.check(lib.mtts_adm_infer_pinned_f32(C.byref(pl.struct), 1, tc_.data_ptr(), tc_.stride(0),
+                                                      tc_.stride(1), B, T, None, 0, 0, *outs, None, pin_[0].data_ptr(),
+                                                      T, ws.data_ptr(), ws.numel(), ops._stream()))
+                return (dur, raw) if return_raw else (dur,)
             ws = ops.workspace(lib.mtts_adm_infer_workspace_bytes(C.byref(pl.struct), B, T), tc_.device)
             L.check(lib.mtts_adm_infer_f32(C.byref(pl.struct), tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T,
-                                           dur.data_ptr(), raw.data_ptr() if return_raw else None,
-                                           ws.data_ptr(), ws.numel(), ops._stream()))
+                                           *outs, ws.data_ptr(), ws.numel(), ops._stream()))
             return (dur, raw) if return_raw else (dur,)
 
         out = self._graphs().run(("adm", pl.serial, B, T, bool(return_raw), tc.stride(0), tc.stride(1),
-                                  ops.launch_policy_now()), (tc,), run)
+                                  ops.launch_policy_now(), pin is not None), (tc,) if pin is None else (tc, pin), run)
         dur = out[0]
         raw = out[1] if return_raw else None
         dur = dur.unsqueeze(-1)
         return (dur, raw) if return_raw else dur
 
-    def infer_mix(self, tc_latents, weights, return_raw: bool = False):
+    def infer_mix(self, tc_latents, weights, return_raw: bool = False, pinned=None):
         """Duration interpolation: the ``infer`` decode of B utterances from a weighted mean of K sources' duration
         predictions.  ``tc_latents``: K tensors (B, T, tc_dim), one per source (e.g. ``tc_latent`` of different prompts);
         ``weights``: (K,) or (B, K), >= 0, each row with a positive sum (normalised per utterance).  All sources share one
@@ -570,15 +581,17 @@ class MegaADM(pack.PlanMixin, nn.Module):
         weights, so new weight values need no new capture.
 
         ``weights`` may also be a schedule (B, T, K), one row per phone: step t, the duration of phone t, mixes by row
-        (b, t)."""
+        (b, t).  ``pinned`` (B, T) as in ``infer``: a pinned phone feeds back its pin in place of the mixed value (raw_src
+        keeps every source's own readout)."""
         _eval_only(self)
         tc, w = _mix_sources(tc_latents, weights, self.tc_latent_dim, "duration mix")
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
         sched = w.dim() == 3
+        pin = None if pinned is None else S.pinned_durations(pinned, B, T).to(tc.device)
         pl = self._plan_get(tc.device, T)
         lib = L.lib()
 
-        def run(tc_, w_):
+        def run(tc_, w_, *pin_):
             dur = torch.empty(B, T, dtype=torch.int32, device=tc_.device)
             raw = torch.empty(B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
             raw_src = torch.empty(K, B, T, dtype=torch.float32, device=tc_.device) if return_raw else None
@@ -586,14 +599,18 @@ class MegaADM(pack.PlanMixin, nn.Module):
             lat = (C.byref(pl.struct), K, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T)
             outs = (dur.data_ptr(), raw.data_ptr() if return_raw else None, raw_src.data_ptr() if return_raw else None,
                     ws.data_ptr(), ws.numel(), ops._stream())
-            if sched:
+            if pin_:
+                L.check(lib.mtts_adm_infer_pinned_f32(*lat, w_.data_ptr(), *((T * K, K) if sched else (K, 0)),
+                                                      *outs[:3], pin_[0].data_ptr(), T, *outs[3:]))
+            elif sched:
                 L.check(lib.mtts_adm_infer_mix_steps_f32(*lat, w_.data_ptr(), T * K, K, *outs))
             else:
                 L.check(lib.mtts_adm_infer_mix_f32(*lat, w_.data_ptr(), *outs))
             return (dur, raw, raw_src) if return_raw else (dur,)
 
         out = self._graphs().run(("adm_mix", pl.serial, K, B, T, bool(return_raw), tc.stride(0), tc.stride(1),
-                                  ops.launch_policy_now(), sched), (tc, w), run)
+                                  ops.launch_policy_now(), sched, pin is not None),
+                                 (tc, w) if pin is None else (tc, w, pin), run)
         dur = out[0].unsqueeze(-1)
         return (dur, out[1], out[2]) if return_raw else dur
 
@@ -845,6 +862,19 @@ def _synth_mix_weights(weights, K, B, Tp, what):
     return S.mix_weights(weights, K, B, what)
 
 
+def _duration_control(phone_tokens, forced_durations, causal_decode, duration_scale, total_frames, pinned_durations):
+    """The validated (scale, total, pins) CPU tensors of a synthesis call's duration control, or None without any."""
+    if duration_scale is None and total_frames is None and pinned_durations is None:
+        return None
+    if forced_durations is not None:
+        raise L.MttsError("forced_durations replace the ADM's durations; they do not combine with duration_scale, "
+                          "total_frames or pinned_durations")
+    if pinned_durations is not None and causal_decode:
+        raise L.MttsError("pinned_durations run inside the reference-faithful ADM loop, not with causal_decode=True")
+    B, Tp = phone_tokens.shape
+    return S.duration_control(duration_scale, total_frames, pinned_durations, B, Tp)
+
+
 class Megatts(nn.Module):
     """Inference orchestrator (models/megatts2.py:295-375).  ``synthesize`` is the tensor-level
     body of the reference's ``forward`` for a batch; ``forward(wavs_dir, text)`` keeps the
@@ -871,7 +901,8 @@ class Megatts(nn.Module):
                    return_intermediates: bool = False, causal_decode: bool = False, prompt_mels: torch.Tensor = None,
                    return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None,
                    sampling: S.Sampling = None, keys=None, prosody_mels=None, prosody_weights=None,
-                   duration_weights=None, plm_context=None):
+                   duration_weights=None, plm_context=None, duration_scale=None, total_frames=None,
+                   pinned_durations=None):
         """phone_tokens (B,Tp) int64, mels (B,Tm,80) prompt mel (frames-major) -> wav (B,1,256*(max sum d + 10)).
         Steps = models/megatts2.py:354-373; every utterance's result equals the reference's batch-1 run on it
         (utterances are independent; the only cross-utterance coupling would be the zero rows the LengthRegulator
@@ -915,11 +946,21 @@ class Megatts(nn.Module):
         ``generator.plm_context`` on same-speaker prompt utterances; the prosody codes come from ``MegaPLM.infer`` (or
         ``infer_causal`` with ``causal_decode``) with ``context=plm_context``, so the target continues the prompts'
         prosody as in training.  The durations, the mel decoder and the vocoder see the target only.  Not with
-        ``prosody_mels``."""
+        ``prosody_mels``.
+        Duration control (opt-in; none of it with ``forced_durations``; include/megatts2_b200.h states the rules):
+        ``duration_scale``: a number, (B,) or (B, Tp), finite and > 0, multiplies the ADM's raw durations (above 1 is
+        slower); ``total_frames`` (B,) ints: utterance b gets exactly that many mel frames (``wav_lens`` = 256 (L_b + 10)),
+        the phones sharing them in proportion to their (scaled) predictions; ``pinned_durations`` (B, Tp) ints, -1 free
+        or 1..127: those phones get exactly that many frames, fed back inside the ADM loop so the rest of the utterance
+        follows from them (not with ``causal_decode``).  They combine with each other and with ``duration_weights``;
+        ``return_intermediates["dt"]`` holds the durations used (``ops.fit_durations`` of the ADM's raw values when a
+        scale or a total is given).  All arguments are checked on the host before any device work."""
         dev = phone_tokens.device
         self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights, plm_context)
+        control = _duration_control(phone_tokens, forced_durations, causal_decode, duration_scale, total_frames,
+                                    pinned_durations)
         args = (phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt, sampling, keys,
-                prosody_mels, prosody_weights, duration_weights, plm_context)
+                prosody_mels, prosody_weights, duration_weights, plm_context, control)
         out = self._synthesize(*args)
         if check_range and _fp16_operands() and ops.tc_overflow(dev):
             _warn_fp16_range("re-running this batch on the bf16x3 engine")
@@ -967,7 +1008,7 @@ class Megatts(nn.Module):
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
                     sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None,
-                    plm_context=None):
+                    plm_context=None, control=None):
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -999,12 +1040,12 @@ class Megatts(nn.Module):
             with ops.launch_policy(nsm - V, pairs=False, pdl=True):
                 if start != "adm":
                     tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
-                dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights)
+                dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights, control)
             main.wait_stream(side)
             pw_side.record_stream(main)
         else:
             tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
-            dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights)
+            dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights, control)
         tc_expand, totals, src, step_w = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats,
                                                           prosody_weights)
         if prosody_mels is not None:
@@ -1047,14 +1088,26 @@ class Megatts(nn.Module):
             out["prosody_step_weights"] = step_w
         return out
 
-    def _durations(self, adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights):
+    def _durations(self, adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights, control=None):
         """-> (dt (B, Tp) int32, the prompts' MRTE latents or None).  Without ``duration_weights``: ``adm_decode`` on
         ``tc_latent``, and the prompts' latents are left to ``_plm_source``.  With them: MRTE on (phone_tokens, prompt) for
-        each prosody prompt, then ``MegaADM.infer_mix`` over [tc_latent, *those latents]."""
+        each prosody prompt, then ``MegaADM.infer_mix`` over [tc_latent, *those latents].  ``control``, the validated
+        (scale, total, pins) of ``_duration_control``: the pins go into the ADM loop, and with a scale or a total the
+        durations are ``ops.fit_durations`` of the decode's raw values."""
+        scale, total, pins = control if control is not None else (None, None, None)
+        fit = scale is not None or total is not None
+        kw = {} if pins is None else {"pinned": pins}
+        if fit:
+            kw["return_raw"] = True
+        lats = None
         if duration_weights is None:
-            return adm_decode(tc_latent)[..., 0], None
-        lats = [self.generator.mrte.tc_latent(phone_tokens, m) for m in prosody_mels]
-        return self.adm.infer_mix([tc_latent] + lats, duration_weights)[..., 0], lats
+            out = adm_decode(tc_latent, **kw)
+        else:
+            lats = [self.generator.mrte.tc_latent(phone_tokens, m) for m in prosody_mels]
+            out = self.adm.infer_mix([tc_latent] + lats, duration_weights, **kw)
+        if fit:
+            return ops.fit_durations(out[1], scale, total, pins), lats
+        return out[..., 0], lats
 
     def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels, prosody_latents=None,
                     prosody_weights=None):
@@ -1083,7 +1136,8 @@ class Megatts(nn.Module):
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
                           chunk_frames: int = 64, prosody_mels=None, prosody_weights=None, duration_weights=None,
-                          plm_context=None, **unsupported):
+                          plm_context=None, duration_scale=None, total_frames=None, pinned_durations=None,
+                          **unsupported):
         """``synthesize`` as a generator of waveform chunks, each yielded as soon as the prosody LM has decoded the codes
         its samples depend on.  Arguments as in ``synthesize``; ``chunk_frames`` mel frames (hop = 256 samples each) per
         chunk.  Each chunk is a dict: ``wav`` (B, 1, n) device tensor, ``offset`` (its first sample's index in the waveform
@@ -1108,22 +1162,25 @@ class Megatts(nn.Module):
         if int(chunk_frames) < 1:
             raise L.MttsError(f"synthesize_stream: chunk_frames must be >= 1, got {chunk_frames}")
         self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False, duration_weights, plm_context)
+        control = _duration_control(phone_tokens, forced_durations, False, duration_scale, total_frames,
+                                    pinned_durations)
         guard = check_range and _fp16_operands()
         return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
-                                  int(chunk_frames), (prosody_mels, prosody_weights, duration_weights, plm_context))
+                                  int(chunk_frames), (prosody_mels, prosody_weights, duration_weights, plm_context),
+                                  control)
 
     def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
-                      prosody):
+                      prosody, control):
         try:
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
-                                    prosody)
+                                    prosody, control)
         except _RangeRestart:
             _warn_fp16_range("restarting this stream on the bf16x3 engine")
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, False, chunk_frames,
-                                    prosody, engine=pack.ENGINE_BF16X3)
+                                    prosody, control, engine=pack.ENGINE_BF16X3)
 
     def _stream(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames, prosody,
-                engine=None):
+                control, engine=None):
         # The engine scope is entered around each computing step only, never across a yield: the caller's own work between
         # chunks keeps its engine.
         from .. import stream as SCH
@@ -1139,7 +1196,7 @@ class Megatts(nn.Module):
         with torch.no_grad(), scope():
             tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
             prosody_mels, prosody_weights, duration_weights, plm_context = prosody
-            dt, lats = self._durations(self.adm.infer, tc_latent, phone_tokens, prosody_mels, duration_weights)
+            dt, lats = self._durations(self.adm.infer, tc_latent, phone_tokens, prosody_mels, duration_weights, control)
             tc_expand, totals, src, step_w = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels,
                                                               lats, prosody_weights)
             dec = self.plm.begin_decode(src, sampling=sampling, keys=keys,
@@ -1217,9 +1274,17 @@ class Megatts(nn.Module):
         (modules/mrte.py:154-171), so padding either would change results - and each bucket runs as one batch.
         Returns a list of 1-D waveforms (valid samples only), in input order.  With ``sampling``, utterance i is keyed
         by its index i in ``items``, so the bucketing and ``max_batch`` do not change what it draws.  Prosody prompts
-        (``prosody_mels``) are not taken here: call ``synthesize`` per batch."""
+        (``prosody_mels``) are not taken here: call ``synthesize`` per batch.  Of the duration controls only a scalar
+        ``duration_scale`` is: the buckets regroup the utterances, so per-utterance values would not line up."""
         if "prosody_mels" in kw or "prosody_weights" in kw or "plm_context" in kw:
             raise L.MttsError("synthesize_many does not take prosody prompts or a PLM context; call synthesize per batch")
+        if "total_frames" in kw or "pinned_durations" in kw:
+            raise L.MttsError("synthesize_many does not take total_frames or pinned_durations (per-utterance values); "
+                              "call synthesize per batch")
+        if kw.get("duration_scale") is not None:
+            kw["duration_scale"] = S.duration_scale(kw["duration_scale"], 1, 1)
+            if kw["duration_scale"].dim() != 0:
+                raise L.MttsError("synthesize_many takes a scalar duration_scale only")
         if sampling is not None:
             kw["sampling"] = sampling
         buckets = {}

@@ -283,6 +283,31 @@ def mix_step_weights(phone_w, durations, T):
     return out
 
 
+def fit_durations(raw, scale=None, total=None, pinned=None):
+    """Raw ADM values (B, Tp) fp32 -> phone durations (B, Tp) int32 fitted to a speaking rate and a length
+    (include/megatts2_b200.h, mtts_fit_durations_f32).  ``scale``: a number, (B,) or (B, Tp), finite and > 0, multiplying
+    the raw values (above 1 is slower); ``pinned`` (B, Tp): -1 free, else 1..127 frames, kept as they are; ``total``
+    (B,): the frames of each utterance, then the free phones share the frames left by Sainte-Lague apportionment of the
+    scaled values.  Without ``total`` a free phone gets the ADM's own rounding of its scaled value, so
+    ``fit_durations(raw)`` is ``MegaADM.infer``'s durations."""
+    from . import sampling as S
+    raw = _dev(raw, name="raw")
+    if raw.dim() != 2:
+        raise L.MttsError(f"raw: expected (B, Tp), got shape {tuple(raw.shape)}")
+    B, Tp = raw.shape
+    sc, tot, pin = S.duration_control(scale, total, pinned, B, Tp)
+    if Tp > S.FIT_MAX_PHONES:
+        raise L.MttsError(f"fit_durations: Tp = {Tp} phones is above the bound of {S.FIT_MAX_PHONES}")
+    dev = raw.device
+    raw = raw if raw.stride(1) == 1 else raw.contiguous()
+    sc, tot, pin = (None if t is None else t.to(dev) for t in (sc, tot, pin))
+    sc_strides = (0, 0) if sc is None else {0: (0, 0), 1: (1, 0), 2: (Tp, 1)}[sc.dim()]
+    out = torch.empty(B, Tp, dtype=torch.int32, device=dev)
+    L.check(L.lib().mtts_fit_durations_f32(_ptr(raw), raw.stride(0), Tp, B, _ptr(sc), *sc_strides, _ptr(pin), Tp,
+                                           _ptr(tot), _ptr(out), Tp, _stream()))
+    return out
+
+
 def philox4x32_10(ctr, key):
     """The sampler's generator: ctr (n, 4) and key (n, 2) uint32 words, as int64 tensors holding values < 2**32, ->
     (n, 4) words (int64, values < 2**32)."""

@@ -127,6 +127,76 @@ def mix_step_weights(weights, K, B, T, what="prosody mix"):
     return _checked_rows(w.to(device="cpu", dtype=torch.float64), what)
 
 
+DURATION_MAX = 128          # the ADM's durations are 1..128 frames
+PIN_MAX = 127               # the reference's ADM never trains on a duration >= 128
+FIT_MAX_PHONES = 8192       # mtts_fit_durations_f32's bound on Tp
+
+
+def _integers(v, what, shapes):
+    """``v`` as an int64 CPU tensor (the one device-to-host read when ``v`` is a device tensor)."""
+    try:
+        t = torch.as_tensor(v).detach()
+    except (TypeError, ValueError, RuntimeError) as e:
+        raise L.MttsError(f"{what}: expected a {shapes} array of integers ({e})") from None
+    if t.dtype not in (torch.int64, torch.int32, torch.int16, torch.int8, torch.uint8):
+        raise L.MttsError(f"{what}: expected integers, got {t.dtype}")
+    return t.to(device="cpu", dtype=torch.int64)
+
+
+def duration_scale(scale, B, Tp):
+    """``duration_scale`` as a validated fp32 CPU tensor: () (one value), (B,) (one per utterance) or (B, Tp) (one per
+    phone), every value finite and > 0 as an fp32 number.  Above 1 the utterance is slower."""
+    if isinstance(scale, bool):
+        raise L.MttsError(f"duration_scale must be a real number or a tensor of them, got {scale!r}")
+    s = _real_weights(scale, "duration_scale", "(), (B,) or (B, Tp)").to(device="cpu", dtype=torch.float64)
+    if tuple(s.shape) not in ((), (B,), (B, Tp)):
+        raise L.MttsError(f"duration_scale: shape {tuple(s.shape)}, expected (), ({B},) or ({B}, {Tp})")
+    s32 = s.to(torch.float32)
+    if not bool(torch.isfinite(s32).all()) or bool((s32 <= 0).any()):
+        raise L.MttsError("duration_scale: every value must be finite and > 0 (as an fp32 number)")
+    return s32.contiguous()
+
+
+def pinned_durations(pinned, B, Tp):
+    """``pinned_durations`` as a validated (B, Tp) int32 CPU tensor: -1 leaves a phone free, 1..127 pins it to that many
+    frames (the range the ADM is trained on)."""
+    p = _integers(pinned, "pinned_durations", "(B, Tp)")
+    if tuple(p.shape) != (B, Tp):
+        raise L.MttsError(f"pinned_durations: shape {tuple(p.shape)}, expected ({B}, {Tp})")
+    bad = (p != -1) & ((p < 1) | (p > PIN_MAX))
+    if bool(bad.any()):
+        b, i = (int(x) for x in bad.nonzero()[0])
+        raise L.MttsError(f"pinned_durations[{b}, {i}] = {int(p[b, i])}: expected -1 (free) or 1..{PIN_MAX}")
+    return p.to(torch.int32).contiguous()
+
+
+def total_frames(total, B, Tp, pinned=None):
+    """``total_frames`` as a validated (B,) int32 CPU tensor, each total feasible for its utterance: with F its free
+    phones (all phones without ``pinned``, a validated (B, Tp) tensor) and P the sum of its pins, [|F| + P, 128 |F| + P]."""
+    t = _integers(total, "total_frames", "(B,)")
+    if tuple(t.shape) != (B,):
+        raise L.MttsError(f"total_frames: shape {tuple(t.shape)}, expected ({B},)")
+    pins = pinned.to(torch.int64) if pinned is not None else torch.full((B, Tp), -1, dtype=torch.int64)
+    free = (pins < 1).sum(1)
+    psum = pins.clamp(min=0).sum(1)
+    lo, hi = free + psum, DURATION_MAX * free + psum
+    for b in range(B):
+        if not int(lo[b]) <= int(t[b]) <= int(hi[b]):
+            raise L.MttsError(f"total_frames[{b}] = {int(t[b])} is outside utterance {b}'s feasible range "
+                              f"[{int(lo[b])}, {int(hi[b])}] ({int(free[b])} free phones, {int(psum[b])} pinned frames)")
+    return t.to(torch.int32).contiguous()
+
+
+def duration_control(scale, total, pinned, B, Tp):
+    """The validated (scale, total, pinned) CPU tensors of a duration-controlled call (each None when not given)."""
+    pins = None if pinned is None else pinned_durations(pinned, B, Tp)
+    if (scale is not None or total is not None) and Tp > FIT_MAX_PHONES:
+        raise L.MttsError(f"duration_scale / total_frames: Tp = {Tp} phones is above the bound of {FIT_MAX_PHONES}")
+    sc = None if scale is None else duration_scale(scale, B, Tp)
+    tot = None if total is None else total_frames(total, B, Tp, pins)
+    return sc, tot, pins
+
+
 def row_keys(keys, rows, device):
     """Per-row 64-bit keys as a contiguous (rows,) int64 device tensor; None -> arange(rows)."""
     if keys is None:
