@@ -600,6 +600,23 @@ int mtts_plm_infer_ctx_range_f32(const mtts_plm* m, const float* tc_latent, int6
                                  int64_t ctx_codes_sb, int32_t P, int32_t j0, int32_t j1, int64_t* code_state,
                                  int64_t* codes_out, float* logits_out, const mtts_sampling* s, void* workspace,
                                  int64_t workspace_bytes, void* stream);
+/* Code pins: the range decode with some of its picks fixed, the prosody half of speech editing.  pinned (B, T) int32
+ * device, utterance b at pinned + b*pin_sb (NULL pins nothing).  A pin in [0, vq_bins) is written into state column
+ * P + 1 + j and into codes_out[b, j] in place of target step j's pick (greedy or sampled: a pinned row draws nothing, and
+ * the other rows' draws, keyed by (seed, keys[b], j), do not change); any other value, conventionally -1, leaves the step
+ * free, so no out-of-range code can reach the embedding lookup.  Step j reads state columns <= P + j and writes column
+ * P + 1 + j only, so a caller may leave out steps at which every utterance is pinned, provided their pins are already in
+ * its state: steps below j0 must already be in the caller's state, pinned steps it never enqueues included.  The pins are
+ * read from device memory at every call, so a replayed CUDA graph picks up new values.  With every pin free (or pinned
+ * NULL) the outputs and launch sequence equal mtts_plm_infer_ctx_range_f32's; P = 0 with NULL context pointers is the
+ * plain range decode (mtts_plm_infer_range_f32, or mtts_plm_infer_range_sample_f32 when s is given).  logits_out, when
+ * given, holds the model's logits at every enqueued step, pinned ones included: at a pinned step they score the pinned
+ * history, i.e. teacher forcing.  Workspace: mtts_plm_infer_ctx_workspace_bytes.  There is no mixed or causal variant. */
+int mtts_plm_infer_pinned_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                              int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
+                              int64_t ctx_codes_sb, int32_t P, int32_t j0, int32_t j1, int64_t* code_state,
+                              int64_t* codes_out, float* logits_out, const mtts_sampling* s, const int32_t* pinned,
+                              int64_t pin_sb, void* workspace, int64_t workspace_bytes, void* stream);
 /* The causal decode with a context.  The P context rows run through the stack once, as one teacher-forced causal pass of
  * B*P rows per layer that fills the K/V caches of positions 0..P-1; T single-row steps from position P follow. */
 int64_t mtts_plm_decode_causal_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T);

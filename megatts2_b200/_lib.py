@@ -206,6 +206,8 @@ SIGNATURES = {
                                          C.POINTER(Sampling), vp, i64, vp]),
     "mtts_plm_infer_ctx_range_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, i32, i32,
                                                vp, vp, vp, C.POINTER(Sampling), vp, i64, vp]),
+    "mtts_plm_infer_pinned_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, i32, i32,
+                                            vp, vp, vp, C.POINTER(Sampling), vp, i64, vp, i64, vp]),
     "mtts_plm_decode_causal_ctx_workspace_bytes": (i64, [C.POINTER(PLM), i32, i32, i32]),
     "mtts_plm_decode_causal_ctx_f32": (C.c_int, [C.POINTER(PLM), vp, i64, i32, i32, i32, vp, i64, i32, vp, i64, i32, vp, vp,
                                                  C.POINTER(Sampling), vp, i64, vp]),

@@ -285,6 +285,8 @@ static int64_t plm_ws_floats(const mtts_plm* m, int B, int T) {
 // Prompt context (ctx != nullptr, K = 1): the decode runs over N = P + T positions, the first P latent rows from ctx->tc
 // and the codes of columns 1..P of the (B, N+1) code state from ctx->codes (written here when t0 = 0).  t0, t1, codes_out,
 // logits_out and the sampler's step key stay in target steps: target step j is position P + j.  P = 0 is the plain decode.
+// Code pins (pin != nullptr, K = 1; (B, T) at batch stride pin_sb): target step j of utterance b writes pin[b, j] into the
+// state and codes_out instead of its pick when that pin is in [0, V) (mtts_plm_infer_pinned_f32).
 struct PlmCtx {
   const float* tc; int64_t tc_sb; int tc_ld;           // (Bc, P, tc_dim); tc_sb = 0: one context for every utterance
   const int64_t* codes; int64_t codes_sb;              // (Bc, P); codes_sb = 0 likewise
@@ -293,13 +295,15 @@ struct PlmCtx {
 static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, int tc_ld, int B, int T, int t0, int t1,
                            int64_t* state, int64_t* codes_out, float* logits_out, void* ws, int64_t ws_bytes, cudaStream_t st,
                            const mtts_sampling* smp, int K = 1, const float* weights = nullptr, int64_t w_sb = 0,
-                           int64_t w_st = 0, const PlmCtx* ctx = nullptr) {
+                           int64_t w_st = 0, const PlmCtx* ctx = nullptr, const int32_t* pin = nullptr,
+                           int64_t pin_sb = 0) {
   const int D = m->enc.d_model, V = m->vq_bins;
   MTTS_REQUIRE(D == m->tc_dim + m->vq_dim, "d_model != tc_dim + vq_dim");
   MTTS_REQUIRE(tc && codes_out && m->pc_embedding && m->w_predict && m->pe, "null pointer");
   MTTS_REQUIRE(0 <= t0 && t0 <= t1 && t1 <= (T > 0 ? T : 0), "step range outside [0, T]");
   MTTS_REQUIRE(weights || K == 1, "K > 1 sources need weights");
   MTTS_REQUIRE(w_sb >= 0 && w_st >= 0, "weight strides must be >= 0");
+  MTTS_REQUIRE(!pin || (K == 1 && pin_sb >= 0), "code pins need K = 1 and pin_sb >= 0");
   MTTS_REQUIRE(!ctx || (K == 1 && ctx->P >= 0 && (ctx->P == 0 || (ctx->tc && ctx->codes))), "bad context");
   if (weights) MTTS_TRY(mix_logprob_check(V, K));
   if (B <= 0 || T <= 0 || t0 == t1) return 0;
@@ -342,8 +346,10 @@ static int plm_infer_steps(const mtts_plm* m, const float* tc, int64_t tc_sb, in
       MTTS_TRY(mix_logprob_rows(lg, lg_sb, V, K, B, weights + j * w_st, w_sb, mixed, V, st));
       pick_from = mixed; pick_ld = V;
     }
-    if (smp) MTTS_TRY(sample_rows(pick_from, pick_ld, V, B, j, *smp, codes + (t + 1), N + 1, codes_out + j, T, st));
-    else MTTS_TRY(argmax_rows(pick_from, pick_ld, V, B, codes + (t + 1), N + 1, codes_out + j, T, st));
+    const int32_t* pj = pin ? pin + j : nullptr;
+    if (smp)
+      MTTS_TRY(sample_rows(pick_from, pick_ld, V, B, j, *smp, codes + (t + 1), N + 1, codes_out + j, T, st, pj, pin_sb));
+    else MTTS_TRY(argmax_rows(pick_from, pick_ld, V, B, codes + (t + 1), N + 1, codes_out + j, T, st, pj, pin_sb));
   }
   return 0;
 }
@@ -1118,6 +1124,18 @@ int mtts_plm_infer_ctx_range_f32(const mtts_plm* m, const float* tc_latent, int6
   const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
   return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, j0, j1, code_state, codes_out, logits_out, workspace,
                          workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, 0, 0, &c);
+}
+int mtts_plm_infer_pinned_f32(const mtts_plm* m, const float* tc_latent, int64_t tc_sb, int32_t tc_ld, int32_t B,
+                              int32_t T, const float* ctx_tc, int64_t ctx_sb, int32_t ctx_ld, const int64_t* ctx_codes,
+                              int64_t ctx_codes_sb, int32_t P, int32_t j0, int32_t j1, int64_t* code_state,
+                              int64_t* codes_out, float* logits_out, const mtts_sampling* s, const int32_t* pinned,
+                              int64_t pin_sb, void* workspace, int64_t workspace_bytes, void* stream) {
+  MTTS_REQUIRE(m && m->enc.layers && workspace && code_state, "null pointer");
+  MTTS_REQUIRE(pin_sb >= 0, "pin_sb must be >= 0");
+  if (s) MTTS_TRY(sampling_check(s, m->vq_bins));
+  const PlmCtx c{ctx_tc, ctx_sb, ctx_ld, ctx_codes, ctx_codes_sb, P};
+  return plm_infer_steps(m, tc_latent, tc_sb, tc_ld, B, T, j0, j1, code_state, codes_out, logits_out, workspace,
+                         workspace_bytes, (cudaStream_t)stream, s, 1, nullptr, 0, 0, &c, pinned, pin_sb);
 }
 int64_t mtts_plm_decode_causal_ctx_workspace_bytes(const mtts_plm* m, int32_t B, int32_t P, int32_t T) {
   return plm_causal_ws_floats(m, B, T, P > 0 ? P : 0) * 4 + 8192;

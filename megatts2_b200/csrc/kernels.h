@@ -183,13 +183,17 @@ int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const
 int copy_codes(const int64_t* x, int64_t x_sb, int64_t* y, int64_t ldy, int B, int n, cudaStream_t st);
 // additive causal mask (T, T): 0 where key <= query, -inf above the diagonal
 int causal_mask(float* m, int T, cudaStream_t st);
+// pin (optional, code pins of the PLM decode): row r writes pin[r * pin_sb] instead of its pick when that value is in
+// [0, V); any other value leaves the row free
 int argmax_rows(const float* x, int64_t ldx, int V, int rows, int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb,
-                cudaStream_t st);
+                cudaStream_t st, const int32_t* pin = nullptr, int64_t pin_sb = 0);
 // opt-in sampler (sample.cu): validates s against V, then draws one code per row (argmax_rows when temperature == 0 or
-// top_k == 1); sampling_check alone lets a driver reject bad parameters before it enqueues anything
+// top_k == 1); sampling_check alone lets a driver reject bad parameters before it enqueues anything.  pin as argmax_rows';
+// a pinned row draws nothing and leaves the other rows' draws unchanged
 int sampling_check(const mtts_sampling* s, int V);
 int sample_rows(const float* x, int64_t ldx, int V, int rows, int step, const mtts_sampling& s, int64_t* out_a,
-                int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st);
+                int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st, const int32_t* pin = nullptr,
+                int64_t pin_sb = 0);
 int philox4x32_10_words(const uint32_t* ctr, const uint32_t* key, uint32_t* out, int64_t n, cudaStream_t st);
 // prosody mix (sample.cu): l (B, V) from K source rows per utterance and the weight rows w + b ldw; mix_logprob_check
 // validates (V, K) before a driver enqueues anything

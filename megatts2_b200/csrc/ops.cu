@@ -824,13 +824,25 @@ int plm_build_input(const float* tc, int64_t tc_sb, int tc_ld, int tc_dim, const
 }
 
 // argmax over the last dim, first index on ties (torch.argmax on CPU); one warp per row.
-// writes out_a[row*lda] and (optionally) out_b[row*ldb].
+// writes out_a[row*lda] and (optionally) out_b[row*ldb].  pin (optional): a row whose pin[row*pin_sb] is in [0, V) writes
+// that value instead of its argmax; any other pin value leaves the row free.
 __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t ldx, int V, int rows, int64_t* out_a,
-                                   int64_t lda, int64_t* out_b, int64_t ldb) {
+                                   int64_t lda, int64_t* out_b, int64_t ldb, const int32_t* __restrict__ pin,
+                                   int64_t pin_sb) {
   pdl_entry();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
+  if (pin) {
+    const int32_t p = pin[(int64_t)row * pin_sb];
+    if (p >= 0 && p < V) {
+      if (lane == 0) {
+        out_a[(int64_t)row * lda] = p;
+        if (out_b) out_b[(int64_t)row * ldb] = p;
+      }
+      return;
+    }
+  }
   const float* xr = x + (int64_t)row * ldx;
   float best = -INFINITY;
   int bi = 0x7fffffff;
@@ -852,9 +864,10 @@ __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t ldx, int
 }
 
 int argmax_rows(const float* x, int64_t ldx, int V, int rows, int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb,
-                cudaStream_t st) {
+                cudaStream_t st, const int32_t* pin, int64_t pin_sb) {
   if (rows <= 0) return 0;
-  launch_k(argmax_rows_kernel, (unsigned)cdiv64(rows, 4), 128, 0, st, x, ldx, V, rows, out_a, lda, out_b, ldb);
+  launch_k(argmax_rows_kernel, (unsigned)cdiv64(rows, 4), 128, 0, st, x, ldx, V, rows, out_a, lda, out_b, ldb, pin,
+           pin_sb);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

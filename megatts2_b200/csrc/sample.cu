@@ -100,11 +100,22 @@ __device__ double block_scan(double v, double* total) {
 __global__ void __launch_bounds__(SAMPLE_THREADS)
 sample_rows_kernel(const float* __restrict__ x, int64_t ldx, int V, int step, float temperature, int top_k, float top_p,
                    int filter, int n_sort, const uint64_t* __restrict__ seed, const uint64_t* __restrict__ keys,
-                   int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb) {
+                   int64_t* out_a, int64_t lda, int64_t* out_b, int64_t ldb, const int32_t* __restrict__ pin,
+                   int64_t pin_sb) {
   extern __shared__ uint64_t s_key[];
   __shared__ int s_n, s_cut;
   pdl_entry();
   const int row = blockIdx.x;
+  if (pin) {                                               // a pinned row: the whole CTA leaves before any barrier
+    const int32_t p = pin[(int64_t)row * pin_sb];
+    if (p >= 0 && p < V) {
+      if (threadIdx.x == 0) {
+        out_a[(int64_t)row * lda] = p;
+        if (out_b) out_b[(int64_t)row * ldb] = p;
+      }
+      return;
+    }
+  }
   const float* xr = x + (int64_t)row * ldx;
   const uint64_t sd = seed[0], kr = keys[row];
   const uint2 pkey = make_uint2((uint32_t)sd, (uint32_t)(sd >> 32));      // Philox key (seed_lo, seed_hi)
@@ -306,17 +317,18 @@ int sampling_check(const mtts_sampling* s, int V) {
 }
 
 int sample_rows(const float* x, int64_t ldx, int V, int rows, int step, const mtts_sampling& s, int64_t* out_a,
-                int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st) {
+                int64_t lda, int64_t* out_b, int64_t ldb, cudaStream_t st, const int32_t* pin, int64_t pin_sb) {
   MTTS_TRY(sampling_check(&s, V));
   MTTS_REQUIRE(x && out_a, "null pointer");
   MTTS_REQUIRE(step >= 0 && ldx >= 0, "step and ld must be >= 0");
   if (rows <= 0) return 0;
-  if (s.temperature == 0.f || s.top_k == 1) return argmax_rows(x, ldx, V, rows, out_a, lda, out_b, ldb, st);
+  if (s.temperature == 0.f || s.top_k == 1)
+    return argmax_rows(x, ldx, V, rows, out_a, lda, out_b, ldb, st, pin, pin_sb);
   const int filter = (s.top_k > 0 && s.top_k < V) || s.top_p < 1.f;
   int n_sort = SAMPLE_THREADS;
   while (n_sort < V) n_sort <<= 1;
   launch_k(sample_rows_kernel, (unsigned)rows, SAMPLE_THREADS, filter ? (size_t)n_sort * 8 : 0, st, x, ldx, V, step,
-           s.temperature, s.top_k, s.top_p, filter, n_sort, s.seed, s.keys, out_a, lda, out_b, ldb);
+           s.temperature, s.top_k, s.top_p, filter, n_sort, s.seed, s.keys, out_a, lda, out_b, ldb, pin, pin_sb);
   MTTS_CHECK_LAUNCH();
   return 0;
 }

@@ -18,6 +18,7 @@ import yaml
 from .. import _lib as L
 from .. import autograd as A
 from .. import ops, pack
+from .. import edit as ED
 from .. import sampling as S
 from ..modules.convnet import ConvNet
 from ..modules.embedding import SinePositionalEmbedding
@@ -134,6 +135,11 @@ def _ctx_args(ctx):
     one = tc8.shape[0] == 1
     return (tc8.data_ptr(), 0 if one else tc8.stride(0), tc8.stride(1), codes.data_ptr(), 0 if one else codes.stride(0),
             tc8.shape[1])
+
+
+def _no_code_pins(pinned, what):
+    if pinned is not None:
+        raise L.MttsError(f"{what} does not take code pins: they are built for MegaPLM.infer's decode only")
 
 
 def _ar_plan(model, enc, pos, struct, device, T, fill):
@@ -273,7 +279,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         return logits, p_codes[:, 1:]
 
     def infer(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None, keys=None,
-              context=None):
+              context=None, pinned=None):
         """Greedy AR decode, BOS = vq_bins, exactly T steps, NON-causal full recompute per step
         (models/megatts2.py:165-181).  tc_latent (B,T,tc_dim) -> (B,T) int64 [, (B,T,vq_bins) logits].
 
@@ -285,12 +291,64 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         decoded as the continuation of the context's P rows, as the model was trained: step j sees the latents
         [context; tc_latent[:, :j+1]] at positions 0..P+j and the codes [BOS, context codes, c_0 .. c_{j-1}].  The codes
         and logits are the target's only; a sampled step j draws the noise of ``infer``'s step j.  The context is a graph
-        input, so a new context of the same shape needs no new capture."""
+        input, so a new context of the same shape needs no new capture.
+
+        ``pinned`` (opt-in code pins, the prosody half of speech editing): (B, T) ints, -1 leaves step j of utterance b
+        free and 0..vq_bins-1 fixes its code, which is written into the history in place of the pick, so the free steps
+        decode after it (include/megatts2_b200.h, mtts_plm_infer_pinned_f32).  A step pinned in every utterance is never
+        enqueued: step j reads the codes of steps < j only, so the free steps run the same kernels on the same data as a
+        decode of every step, and an edit costs the free steps alone.  The codes returned hold the pins.  With
+        ``return_logits`` every step runs, and a pinned step's logits score its pinned history (teacher forcing).  The pins
+        are a graph input; which steps run is part of the graph key, so new pin values with the same free steps replay
+        without a new capture.  Combines with ``sampling`` (a pinned row draws nothing; the other rows' draws do not
+        change) and ``context``."""
         _eval_only(self)
         tc = _dev_rows(tc_latent, "tc_latent")
         B, T, _ = tc.shape
+        pin = None if pinned is None else S.pinned_codes(pinned, B, T, self.vq_bins)
         ctx = _context_inputs(context, B, self.tc_latent_dim, self.vq_bins, tc.device)
-        return self._decode(tc, 1, None, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits, ctx)
+        smp = _sampling_inputs(sampling, keys, B, tc.device)
+        if pin is not None:
+            return self._decode_pinned(tc, smp, ctx, pin.to(tc.device), S.pinned_runs(pin, return_logits),
+                                       return_logits)
+        return self._decode(tc, 1, None, smp, 0, T, None, return_logits, ctx)
+
+    def _decode_pinned(self, tc, smp, ctx, pin, runs, return_logits):
+        """``infer`` with the (B, T) int32 device code pins ``pin``: one graphed call that builds the code state (BOS, the
+        context's codes, the pins >= 0) and enqueues mtts_plm_infer_pinned_f32 once per run [j0, j1) of ``runs``, the
+        steps with a free row.  -> the state's target columns (B, T) int64 [, logits (B, T, V)]."""
+        B, T, V = tc.shape[0], tc.shape[1], self.vq_bins
+        P = 0 if ctx is None else ctx[0].shape[1]
+        pl = self._plan_get(tc.device, P + T)
+        lib = L.lib()
+        m = C.byref(pl.struct)
+
+        def run(tc_, pin_, *rest):
+            ctx_, rest = (rest[:2], rest[2:]) if ctx is not None else (None, rest)
+            state = torch.full((B, P + T + 1), V, dtype=torch.int64, device=tc_.device)     # column 0 = BOS
+            if P:
+                state[:, 1:P + 1] = ctx_[1]
+            target = state[:, P + 1:]
+            target.copy_(torch.where(pin_ >= 0, pin_.to(torch.int64), target))
+            codes = torch.empty(B, T, dtype=torch.int64, device=tc_.device)
+            logits = torch.empty(B, T, V, dtype=torch.float32, device=tc_.device) if return_logits else None
+            if runs:
+                ws = ops.workspace(lib.mtts_plm_infer_ctx_workspace_bytes(m, B, P, T), tc_.device)
+                s = C.byref(smp[0].struct(*rest)) if smp is not None else None
+                c_args = _ctx_args(ctx_) if ctx is not None else (None, 0, 0, None, 0, 0)
+                for j0, j1 in runs:
+                    L.check(lib.mtts_plm_infer_pinned_f32(m, tc_.data_ptr(), tc_.stride(0), tc_.stride(1), B, T, *c_args,
+                                                          j0, j1, state.data_ptr(), codes.data_ptr(),
+                                                          logits.data_ptr() if return_logits else None, s,
+                                                          pin_.data_ptr(), T, ws.data_ptr(), ws.numel(), ops._stream()))
+            target = target.contiguous()
+            return (target, logits) if return_logits else (target,)
+
+        inputs = (tc, pin) + (tuple(ctx) if ctx is not None else ()) + (smp[1:] if smp is not None else ())
+        key = (pl.serial, B, T, runs, bool(return_logits), tc.stride(0), tc.stride(1), ops.launch_policy_now(),
+               None if smp is None else smp[0].graph_key(), None if ctx is None else (ctx[0].shape[0], P))
+        out = self._graphs("pinned").run(key, inputs, run)
+        return out if return_logits else out[0]
 
     def _decode(self, tc, K, weights, smp, t0, t1, state, return_logits, ctx=None):
         """Steps [t0, t1) of the decode of B utterances from ``tc``, the (K*B, T, tc_dim) stack of K sources mixed by the
@@ -356,7 +414,8 @@ class MegaPLM(pack.PlanMixin, nn.Module):
             return out[0]
         return out[0], (out[1].reshape(K, B, t1 - t0, V) if mix else out[1])
 
-    def infer_mix(self, tc_latents, weights, return_logits: bool = False, sampling: S.Sampling = None, keys=None):
+    def infer_mix(self, tc_latents, weights, return_logits: bool = False, sampling: S.Sampling = None, keys=None,
+                  pinned=None):
         """Prosody interpolation (Mega-TTS 2): the ``infer`` decode of B utterances from a weighted mixture of K sources'
         code distributions.  ``tc_latents``: K tensors (B, T, tc_dim), one per source (e.g. ``tc_latent`` from different
         prosody prompts); ``weights``: (K,) or (B, K), >= 0, each row with a positive sum (normalised per utterance).  All
@@ -368,18 +427,21 @@ class MegaPLM(pack.PlanMixin, nn.Module):
 
         ``weights`` may also be a schedule (B, T, K): step t of utterance b then mixes by row (b, t), under the same rules
         per row, so the prosody can follow one prompt in one part of the utterance and another elsewhere
-        (``ops.mix_step_weights`` makes such a schedule from per-phone weights)."""
+        (``ops.mix_step_weights`` makes such a schedule from per-phone weights).  Code pins are not built for the mix."""
         _eval_only(self)
+        _no_code_pins(pinned, "infer_mix")
         tc, w = _mix_sources(tc_latents, weights, self.tc_latent_dim, "prosody mix")
         K, (B, T, _) = len(tc_latents), tc_latents[0].shape
         return self._decode(tc, K, w, _sampling_inputs(sampling, keys, B, tc.device), 0, T, None, return_logits)
 
-    def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None, context=None) -> "PLMDecode":
+    def begin_decode(self, tc_latent, sampling: S.Sampling = None, keys=None, weights=None, context=None,
+                     pinned=None) -> "PLMDecode":
         """Start a resumable ``infer``: returns the decode state that ``decode_until`` advances.  Decoding through step T in
         any number of ranges gives ``infer``'s codes and logits (same ``sampling``, ``keys`` and ``context``).  With
         ``weights`` ((K,), (B, K) or a (B, T, K) schedule), ``tc_latent`` is the list of K sources of ``infer_mix`` and the
-        ranges give ``infer_mix``'s codes and logits (not with a context)."""
+        ranges give ``infer_mix``'s codes and logits (not with a context).  Code pins are ``infer``'s alone."""
         _eval_only(self)
+        _no_code_pins(pinned, "begin_decode")
         K, w = 1, None
         if weights is not None:
             if context is not None:
@@ -419,7 +481,7 @@ class MegaPLM(pack.PlanMixin, nn.Module):
         return out
 
     def infer_causal(self, tc_latent: torch.Tensor, return_logits: bool = False, sampling: S.Sampling = None,
-                     keys=None, context=None):
+                     keys=None, context=None, pinned=None):
         """OPT-IN causal KV-cache greedy decode (SURVEY.md 8f-1) - NOT what the reference's ``infer`` computes.
 
         ``infer`` re-runs the stack bidirectionally every step (models/megatts2.py:177); this decode follows the
@@ -430,8 +492,10 @@ class MegaPLM(pack.PlanMixin, nn.Module):
 
         ``context`` (as in ``infer``): the causal form of the in-context decode.  The context's P rows run through the stack
         once, as one teacher-forced causal pass that fills the K/V caches, then T single-row steps follow; the logits
-        equal the teacher-forced ``forward`` over [context; target] at the decoded codes."""
+        equal the teacher-forced ``forward`` over [context; target] at the decoded codes.  Code pins are ``infer``'s
+        alone."""
         _eval_only(self)
+        _no_code_pins(pinned, "infer_causal")
         tc = _dev_rows(tc_latent, "tc_latent")
         B, T, _ = tc.shape
         ctx = _context_inputs(context, B, self.tc_latent_dim, self.vq_bins, tc.device)
@@ -970,6 +1034,53 @@ class Megatts(nn.Module):
             return out
         return (out["wav"], out["wav_lens"]) if return_lengths else out["wav"]
 
+    @torch.no_grad()
+    def edit(self, phone_tokens: torch.Tensor, mels: torch.Tensor, orig_phone, orig_durations, orig_codes, span,
+             span_frames=None, duration_scale=None, sampling: S.Sampling = None, keys=None, plm_context=None,
+             check_range: bool = True, return_lengths: bool = False, return_intermediates: bool = False, **rejected):
+        """Speech editing: regenerate the phones [a, b) = ``span[r]`` of an utterance while the durations and prosody
+        codes around them stay as they were.  ``orig_phone`` / ``orig_durations`` (B, Tp_o) and ``orig_codes``
+        (B, >= ceil(N_o / 8)), N_o the original's frame count, describe the original: ``dt`` and ``p_codes`` of an
+        earlier ``synthesize(..., return_intermediates=True)``, or for a recording its aligner durations and the codes of
+        its mel (``generator.vqpe(mel)[3][0]``).  ``phone_tokens`` (B, Tp_e) is the edited sentence: row r is
+        ``orig_phone[r, :a] + n_r new phones + orig_phone[r, b:]``, n_r = Tp_e - Tp_o + (b - a) >= 0.
+
+        The kept phones are pinned to their original durations inside the ADM loop (1..127 each) and the new ones are
+        decoded after them; ``span_frames`` (B,) gives the new phones exactly that many frames in all (``span_frames`` =
+        L_o, the replaced phones' frames, keeps every later frame where it was), and ``duration_scale`` scales the new
+        phones' predictions, both through ``synthesize``'s duration control.  The prosody LM then decodes only the
+        8-frame blocks that overlap the new frames or straddle one of their ends; the other blocks keep the original's
+        codes as pins of ``MegaPLM.infer`` (megatts2_b200/edit.py states the rule), and steps pinned in every row are not
+        run.  ``sampling``, ``keys``, ``plm_context`` and ``check_range`` are ``synthesize``'s.
+
+        Returns what ``synthesize`` returns: the whole edited utterance.  MRTE's latent depends on the whole phone
+        sequence, and the mel decoder and vocoder see +-20 / +-14 frames around each frame, so samples outside the span
+        move slightly; splicing into the original audio is the caller's choice.  ``return_intermediates`` adds
+        ``edit_frames`` (B, 2), [F_a, F_a + L_n): the regenerated frames (sample 256 (5 + f) is frame f), and
+        ``code_pins`` (B, T) the pins used.  Every argument is checked on the host before any device work; the
+        arguments ``synthesize`` takes for what an edit sets itself, or does not support, are rejected by name."""
+        for k in rejected:
+            if k in ED.REJECTED:
+                raise L.MttsError(f"edit does not take {k}: an edit sets the durations and codes around the span "
+                                  "itself, on the reference-faithful decodes without a prosody mix or a prompt re-vocode")
+        if rejected:
+            raise TypeError(f"edit() got unexpected keyword argument(s) {sorted(rejected)}")
+        plan = ED.EditPlan(phone_tokens, orig_phone, orig_durations, orig_codes, span, span_frames, self.plm.vq_bins)
+        dev = phone_tokens.device
+        control = _duration_control(phone_tokens, None, False, duration_scale, plan.total_frames, plan.pinned_durations)
+        args = (phone_tokens, mels, None, False, None, None, sampling, keys, None, None, None, plm_context, control,
+                plan.code_pins)
+        out = self._synthesize(*args)
+        if check_range and _fp16_operands() and ops.tc_overflow(dev):
+            _warn_fp16_range("re-running this batch on the bf16x3 engine")
+            with pack.engine_scope(pack.ENGINE_BF16X3):
+                out = self._synthesize(*args)
+        if return_intermediates:
+            out["edit_frames"] = plan.edit_frames(out["totals"])
+            out["code_pins"] = plan.code_pins(out["totals"], out["p_codes"].shape[1])
+            return out
+        return (out["wav"], out["wav_lens"]) if return_lengths else out["wav"]
+
     def _revocode_cfg(self):
         """(V, frac, start) of the overlapped prompt re-vocode: V = SM budget of the side stream (MEGATTS2_REVOCODE_SMS; 0 = run
         the re-vocode after the synthesis on the calling stream), frac = share of the batch's prompts re-vocoded there
@@ -1008,7 +1119,9 @@ class Megatts(nn.Module):
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
                     sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None,
-                    plm_context=None, control=None):
+                    plm_context=None, control=None, code_pins=None):
+        # ``code_pins`` (speech editing): totals, T -> the (B, T) code pins of MegaPLM.infer, built once the frame totals
+        # are on the host.
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -1053,7 +1166,8 @@ class Megatts(nn.Module):
             p_codes = self.plm.infer_mix(src, prosody_weights if step_w is None else step_w, sampling=sampling, keys=keys)
         else:
             tc8 = src
-            p_codes = plm_decode(src, sampling=sampling, keys=keys, context=plm_context)
+            kw = {} if code_pins is None else {"pinned": code_pins(totals, tc8.shape[1])}
+            p_codes = plm_decode(src, sampling=sampling, keys=keys, context=plm_context, **kw)
         B, Lmax = tc_expand.shape[0], tc_expand.shape[1]
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]

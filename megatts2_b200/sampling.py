@@ -170,6 +170,39 @@ def pinned_durations(pinned, B, Tp):
     return p.to(torch.int32).contiguous()
 
 
+def pinned_codes(pinned, B, T, V):
+    """``pinned`` prosody codes as a validated (B, T) int32 CPU tensor: -1 leaves step j of utterance b free, 0..V-1 fixes
+    its code.  Anything else (BOS = V and pad = V + 1 included) is an error: a pin is a code the model emits."""
+    p = _integers(pinned, "pinned codes", "(B, T)")
+    if tuple(p.shape) != (B, T):
+        raise L.MttsError(f"pinned codes: shape {tuple(p.shape)}, expected ({B}, {T})")
+    bad = (p != -1) & ((p < 0) | (p >= V))
+    if bool(bad.any()):
+        b, j = (int(x) for x in bad.nonzero()[0])
+        raise L.MttsError(f"pinned codes[{b}, {j}] = {int(p[b, j])}: expected -1 (free) or 0..{V - 1}")
+    return p.to(torch.int32).contiguous()
+
+
+def pinned_runs(pins, return_logits=False):
+    """The maximal runs [j0, j1) of steps at which some row of the validated (B, T) ``pins`` is free: the steps a pinned
+    decode enqueues.  A step pinned in every row is never read back (step j reads codes < j only), so it is skipped;
+    ``return_logits`` keeps the single run [0, T) so every step's logits exist."""
+    T = pins.shape[1]
+    if return_logits:
+        return ((0, T),) if T else ()
+    free = (pins < 0).any(0).tolist() if pins.shape[0] else [False] * T
+    runs, j = [], 0
+    while j < T:
+        if not free[j]:
+            j += 1
+            continue
+        j0 = j
+        while j < T and free[j]:
+            j += 1
+        runs.append((j0, j))
+    return tuple(runs)
+
+
 def total_frames(total, B, Tp, pinned=None):
     """``total_frames`` as a validated (B,) int32 CPU tensor, each total feasible for its utterance: with F its free
     phones (all phones without ``pinned``, a validated (B, Tp) tensor) and P the sum of its pins, [|F| + P, 128 |F| + P]."""
