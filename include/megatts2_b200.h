@@ -196,6 +196,26 @@ int mtts_layernorm_f32(const float* x, int32_t ldx, const float* gamma, const fl
                        int64_t rows, int32_t C, float eps, int32_t post_act, int32_t accumulate,
                        void* stream);
 
+/* Timbre interpolation: MRTE's LayerNorm -> ReLU (modules/mrte.py:168-169) applied to a weighted mix of K sources'
+ * pre-norm attention outputs, one per timbre prompt (Megatts.synthesize(timbre_mels=...)).  Rows r = b*T + t,
+ * 0 <= r < rows; row r of source k is the C floats at y + k*y_ks + r*ldy, and its weight row is the K floats at
+ * weights + b*w_sb + t*w_st ((K,) weights: strides (0, 0); (B, K): (K, 0); (B, T, K): (T*K, K)).  For each row:
+ *   1. wsum = the sum of the positive weights of the row in fp32, in k order; w^_k = w_k / wsum;
+ *   2. m = w^_k0 * y_k0 for the first positive weight k0, then m = fmaf(w^_k, y_k, m) for the later positive weights in
+ *      k order, element by element (the rule of mtts_adm_readout_mix_f32).  Sources with a zero, negative or NaN weight
+ *      are skipped and never read, so non-finite values in them cannot reach the result;
+ *   3. out[r] = post(LN(m) * gamma + beta), with mtts_layernorm_f32's arithmetic for this C, operation for operation.
+ * With exactly one positive weight w^ = 1, so m is that source's row bit for bit and out[r] is what mtts_layernorm_f32
+ * writes for it (res NULL, accumulate 0).  A row without a positive weight normalises the zero row (out = post(beta)).
+ * Since MRTE's out-projection is affine, the mix of its outputs is the attention output under the w^-weighted mixture
+ * of the per-prompt attention distributions.  K in 1..8 and C in {384, 512, 768, 1024} (MTTS_ERR_UNSUPPORTED outside);
+ * post_act none, relu or tanh; y, out, gamma, beta 16-byte aligned, ldy, ldo and y_ks multiples of 4, T >= 1, strides
+ * >= 0; out must not overlap the sources.  Every argument is checked before anything is enqueued; rows = 0 does
+ * nothing. */
+int mtts_mix_layernorm_f32(const float* y, int64_t y_ks, int32_t ldy, int32_t K, const float* weights, int64_t w_sb,
+                           int64_t w_st, int32_t T, const float* gamma, const float* beta, float* out, int32_t ldo,
+                           int64_t rows, int32_t C, float eps, int32_t post_act, void* stream);
+
 /* softmax(Q K^T * scale + mask) V  (F.scaled_dot_product_attention at
  * modules/transformer.py:52-53).  q/k/v/o are (B, T, H, dh) views given by strides;
  * mask is additive fp32 with element strides (mask_sb, mask_sh, mask_sq, 1) or NULL.

@@ -152,6 +152,7 @@ SIGNATURES = {
     "mtts_vq_ste_commit_f32": (C.c_int, [vp, vp, i64, vp, vp, vp, vp]),
     "mtts_vq_ste_commit_bwd_f32": (C.c_int, [vp, vp, vp, vp, f32, i64, vp, vp]),
     "mtts_layernorm_f32": (C.c_int, [vp, i32, vp, vp, vp, i32, vp, i32, i64, i32, f32, i32, i32, vp]),
+    "mtts_mix_layernorm_f32": (C.c_int, [vp, i64, i32, i32, vp, i64, i64, i32, vp, vp, vp, i32, i64, i32, f32, i32, vp]),
     "mtts_attention_f32": (C.c_int, [C.POINTER(AttnParams), vp]),
     "mtts_attention_tc_f32": (C.c_int, [C.POINTER(AttnParams), vp]),
     "mtts_vq_argmin_f32": (C.c_int, [vp, i32, vp, i64, i32, i32, vp, vp]),

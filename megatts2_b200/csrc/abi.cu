@@ -108,6 +108,13 @@ int mtts_layernorm_f32(const float* x, int32_t ldx, const float* gamma, const fl
   return layernorm(x, ldx, gamma, beta, res, ldr, y, ldy, rows, C, eps, post_act, accumulate, (cudaStream_t)stream);
 }
 
+int mtts_mix_layernorm_f32(const float* y, int64_t y_ks, int32_t ldy, int32_t K, const float* weights, int64_t w_sb,
+                           int64_t w_st, int32_t T, const float* gamma, const float* beta, float* out, int32_t ldo,
+                           int64_t rows, int32_t C, float eps, int32_t post_act, void* stream) {
+  return mix_layernorm(y, y_ks, ldy, K, weights, w_sb, w_st, T, gamma, beta, out, ldo, rows, C, eps, post_act,
+                       (cudaStream_t)stream);
+}
+
 int mtts_attention_f32(const mtts_attn_params* p, void* stream) {
   MTTS_REQUIRE(p, "null params");
   return attention(*p, false, (cudaStream_t)stream);

@@ -140,6 +140,11 @@ int tc_overflow_bind(int32_t* flag);
 int mask_tail(float* x, int B, int rows, int L, const int32_t* keep, cudaStream_t st);
 int layernorm(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr, float* y,
               int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, cudaStream_t st);
+// timbre mix: rows r = b T + t of K sources y + k y_ks mixed by the weight rows w + b w_sb + t w_st, then LayerNorm +
+// post_act into out (mtts_mix_layernorm_f32)
+int mix_layernorm(const float* y, int64_t y_ks, int ldy, int K, const float* w, int64_t w_sb, int64_t w_st, int T,
+                  const float* gamma, const float* beta, float* out, int ldo, int64_t rows, int C, float eps, int post_act,
+                  cudaStream_t st);
 // allow_f16_operands: the caller's engine accepts fp16-range operands, so long sequences may use attn_tc.cu (f16x2 planes)
 int attention(const mtts_attn_params& p, bool allow_f16_operands, cudaStream_t st);
 // attention()'s routing as a pure host function: attn_check holds the argument checks, attn_plan picks the kernel

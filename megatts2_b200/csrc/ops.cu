@@ -83,22 +83,14 @@ layernorm_kernel(const float* x, int ldx, const float* __restrict__ gamma, const
   }
 }
 
-// Register-resident variant for the row widths of the path (C = 128*NV, NV float4 per lane): one global read
-// of the row (NV independent 128-bit loads in flight), two shuffle reductions, one write.
+// LayerNorm of one register-resident row v (C = 128*NV, lane l holds elements i*128 + 4l .. +3) and what follows it:
+// post-activation, + res, + y_old, the y store and the operand planes.  Every register-resident LayerNorm calls this one
+// function, so a row that reaches it by another path (mix_layernorm_kernel) is normalised with the same arithmetic.
 template <int NV>
-__global__ void __launch_bounds__(256)
-layernorm_reg_kernel(const float* x, int ldx, const float* __restrict__ gamma, const float* __restrict__ beta,
-                     const float* res, int ldr, float* y, int ldy, int64_t rows, float eps, int post_act,
-                     int accumulate, const PlanesOut po) {
-  pdl_entry();
+__device__ __forceinline__ void layernorm_row(const float4 (&v)[NV], int lane, int64_t row, const float* __restrict__ gamma,
+                                              const float* __restrict__ beta, const float* res, int ldr, float* y, int ldy,
+                                              float eps, int post_act, int accumulate, const PlanesOut& po) {
   constexpr int C = 128 * NV;
-  const int lane = threadIdx.x & 31;
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= rows) return;
-  const float* xr = x + row * ldx;
-  float4 v[NV];
-#pragma unroll
-  for (int i = 0; i < NV; ++i) v[i] = *reinterpret_cast<const float4*>(xr + i * 128 + lane * 4);
   float s = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
@@ -138,6 +130,70 @@ layernorm_reg_kernel(const float* x, int ldx, const float* __restrict__ gamma, c
   }
 }
 
+// Register-resident variant for the row widths of the path (C = 128*NV, NV float4 per lane): one global read
+// of the row (NV independent 128-bit loads in flight), two shuffle reductions, one write.
+template <int NV>
+__global__ void __launch_bounds__(256)
+layernorm_reg_kernel(const float* x, int ldx, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     const float* res, int ldr, float* y, int ldy, int64_t rows, float eps, int post_act,
+                     int accumulate, const PlanesOut po) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const float* xr = x + row * ldx;
+  float4 v[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) v[i] = *reinterpret_cast<const float4*>(xr + i * 128 + lane * 4);
+  layernorm_row<NV>(v, lane, row, gamma, beta, res, ldr, y, ldy, eps, post_act, accumulate, po);
+}
+
+// Timbre mix (the contract is stated with mtts_mix_layernorm_f32 in include/megatts2_b200.h): one warp per row r = b T + t
+// of K sources y + k y_ks, whose weight row is W + b w_sb + t w_st.  The row is mixed by adm_readout_mix_kernel's rule,
+// element by element (the first positive term w^ y, the later ones fmaf(w^, y, acc) in k order; sources without a
+// positive weight are never read), then normalised by layernorm_row: a one-hot row is layernorm_reg_kernel's bit for bit.
+constexpr int LN_MIX_MAX_K = 8;
+template <int NV>
+__global__ void __launch_bounds__(256)
+mix_layernorm_kernel(const float* __restrict__ y, int64_t y_ks, int ldy, int K, const float* __restrict__ W,
+                     int64_t w_sb, int64_t w_st, int T, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     float* out, int ldo, int64_t rows, float eps, int post_act) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int64_t b = row / T, t = row - b * T;
+  const float* wr = W + b * w_sb + t * w_st;
+  float wk[LN_MIX_MAX_K];
+  float wsum = 0.f;
+#pragma unroll
+  for (int k = 0; k < LN_MIX_MAX_K; ++k) {
+    wk[k] = k < K ? __ldg(wr + k) : 0.f;
+    if (wk[k] > 0.f) wsum += wk[k];             // zero weights add nothing; NaN or negative ones are skipped throughout
+  }
+  float4 v[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  bool first = true;
+#pragma unroll
+  for (int k = 0; k < LN_MIX_MAX_K; ++k) {
+    if (k >= K) break;
+    if (!(wk[k] > 0.f)) continue;
+    const float wn = wk[k] / wsum;
+    const float* yr = y + k * y_ks + row * ldy;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const float4 a = *reinterpret_cast<const float4*>(yr + i * 128 + lane * 4);
+      v[i] = first ? make_float4(wn * a.x, wn * a.y, wn * a.z, wn * a.w)
+                   : make_float4(fmaf(wn, a.x, v[i].x), fmaf(wn, a.y, v[i].y), fmaf(wn, a.z, v[i].z),
+                                 fmaf(wn, a.w, v[i].w));
+    }
+    first = false;
+  }
+  const PlanesOut no_planes{nullptr, 0, 0, 0, 0.f, 0, nullptr};
+  layernorm_row<NV>(v, lane, row, gamma, beta, nullptr, 0, out, ldo, eps, post_act, 0, no_planes);
+}
+
 static inline bool al16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
 int layernorm_ex(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr,
@@ -174,6 +230,37 @@ int layernorm(const float* x, int ldx, const float* gamma, const float* beta, co
   MTTS_REQUIRE(y, "null pointer");
   PlanesOut po{nullptr, 0, 0, 0, 0.f, 0, nullptr};
   return layernorm_ex(x, ldx, gamma, beta, res, ldr, y, ldy, rows, C, eps, post_act, accumulate, po, st);
+}
+
+int mix_layernorm(const float* y, int64_t y_ks, int ldy, int K, const float* w, int64_t w_sb, int64_t w_st, int T,
+                  const float* gamma, const float* beta, float* out, int ldo, int64_t rows, int C, float eps, int post_act,
+                  cudaStream_t st) {
+  MTTS_REQUIRE(K >= 1, "K must be >= 1");
+  if (K > LN_MIX_MAX_K)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: K = %lld sources is above the bound of %lld", "mix_layernorm", (long long)K,
+                (long long)LN_MIX_MAX_K);
+  if (C != 384 && C != 512 && C != 768 && C != 1024)
+    return fail(MTTS_ERR_UNSUPPORTED, "%s: C = %lld, expected 384, 512, 768 or 1024", "mix_layernorm", (long long)C);
+  MTTS_REQUIRE(rows >= 0, "rows must be >= 0");
+  MTTS_REQUIRE(y && w && gamma && beta && out, "null pointer");
+  MTTS_REQUIRE(T >= 1 && y_ks >= 0 && w_sb >= 0 && w_st >= 0 && ldy >= C && ldo >= C, "bad T, strides or row strides");
+  MTTS_REQUIRE(post_act == MTTS_ACT_NONE || post_act == MTTS_ACT_RELU || post_act == MTTS_ACT_TANH,
+               "post_act must be none, relu or tanh");
+  MTTS_REQUIRE(al16(y) && al16(out) && al16(gamma) && al16(beta) && ldy % 4 == 0 && ldo % 4 == 0 && y_ks % 4 == 0,
+               "y, out, gamma and beta must be 16-byte aligned, with ldy, ldo and y_ks multiples of 4");
+  if (rows == 0) return 0;
+  const int wpb = 8;
+  const unsigned grid = (unsigned)cdiv64(rows, wpb);
+#define MTTS_LN_MIX(NV) \
+  launch_k(mix_layernorm_kernel<NV>, grid, wpb * 32, 0, st, y, y_ks, ldy, K, w, w_sb, w_st, T, gamma, beta, out, ldo, rows, \
+           eps, post_act)
+  if (C == 1024) MTTS_LN_MIX(8);
+  else if (C == 768) MTTS_LN_MIX(6);
+  else if (C == 512) MTTS_LN_MIX(4);
+  else MTTS_LN_MIX(3);
+#undef MTTS_LN_MIX
+  MTTS_CHECK_LAUNCH();
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------

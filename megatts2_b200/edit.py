@@ -22,7 +22,7 @@ from . import sampling as S
 FRAMES_PER_CODE = 8
 # arguments of ``synthesize`` that an edit sets itself or does not support
 REJECTED = ("forced_durations", "causal_decode", "pinned_durations", "total_frames", "prompt_mels", "prosody_mels",
-            "prosody_weights", "duration_weights")
+            "prosody_weights", "duration_weights", "timbre_mels", "timbre_weights")
 
 
 def _ints(v, what, dims):

@@ -22,7 +22,7 @@ from .. import edit as ED
 from .. import sampling as S
 from ..modules.convnet import ConvNet
 from ..modules.embedding import SinePositionalEmbedding
-from ..modules.mrte import MRTE, LengthRegulator
+from ..modules.mrte import MRTE, LengthRegulator, check_prompts
 from ..modules.tokenizer import HIFIGAN_HOP_LENGTH, HIFIGAN_SR, extract_mel_spec
 from ..modules.transformer import TransformerEncoder, TransformerEncoderLayer, encoder_plan, run_encoder
 from ..modules.vqpe import VQProsodyEncoder
@@ -919,13 +919,6 @@ def _warn_fp16_range(then):
     warnings.warn("megatts2_b200: an activation left the fp16 range of the fp16 operand split; " + then, stacklevel=2)
 
 
-def _synth_mix_weights(weights, K, B, Tp, what):
-    """The validated (B, K) CPU weights of a synthesis mix, or (B, Tp, K) when ``weights`` has one row per phone."""
-    if S.per_step(weights):
-        return S.mix_step_weights(weights, K, B, Tp, what)
-    return S.mix_weights(weights, K, B, what)
-
-
 def _duration_control(phone_tokens, forced_durations, causal_decode, duration_scale, total_frames, pinned_durations):
     """The validated (scale, total, pins) CPU tensors of a synthesis call's duration control, or None without any."""
     if duration_scale is None and total_frames is None and pinned_durations is None:
@@ -966,7 +959,7 @@ class Megatts(nn.Module):
                    return_lengths: bool = False, check_range: bool = True, overlap_prompt: bool = None,
                    sampling: S.Sampling = None, keys=None, prosody_mels=None, prosody_weights=None,
                    duration_weights=None, plm_context=None, duration_scale=None, total_frames=None,
-                   pinned_durations=None):
+                   pinned_durations=None, timbre_mels=None, timbre_weights=None):
         """phone_tokens (B,Tp) int64, mels (B,Tm,80) prompt mel (frames-major) -> wav (B,1,256*(max sum d + 10)).
         Steps = models/megatts2.py:354-373; every utterance's result equals the reference's batch-1 run on it
         (utterances are independent; the only cross-utterance coupling would be the zero rows the LengthRegulator
@@ -1000,7 +993,8 @@ class Megatts(nn.Module):
         steps; ``return_intermediates`` then adds ``prosody_step_weights`` (B, T, K).  Each prompt gives a source latent
         ``mrte.tc_latent(phone_tokens, prompt)``, length-regulated and max-pooled with the target's durations, and the
         codes come from ``MegaPLM.infer_mix`` over the K sources.  The durations (unless ``duration_weights`` is given),
-        the mel decoder and the vocoder keep the target's (``mels``) latent, so the timbre stays the target's.  Not with
+        the mel decoder and the vocoder keep the target's (``mels``) latent, so the timbre stays the target's (``timbre_mels``
+        blends it).  Not with
         ``causal_decode``.
         ``duration_weights`` (opt-in duration interpolation, with ``prosody_mels``): (K,) or (B, K), or (B, Tp, K) with one
         row per phone (the ADM's step t is phone t), the same K; weight 0 belongs to ``mels``.  The durations then come from ``MegaADM.infer_mix`` over [the target's latent, *the prompts'
@@ -1018,18 +1012,29 @@ class Megatts(nn.Module):
         or 1..127: those phones get exactly that many frames, fed back inside the ADM loop so the rest of the utterance
         follows from them (not with ``causal_decode``).  They combine with each other and with ``duration_weights``;
         ``return_intermediates["dt"]`` holds the durations used (``ops.fit_durations`` of the ADM's raw values when a
-        scale or a total is given).  All arguments are checked on the host before any device work."""
+        scale or a total is given).
+        ``timbre_mels`` (opt-in timbre interpolation): a list of (B, Tm_k, 80) timbre prompts, with ``timbre_weights``
+        (K,), (B, K) or (B, Tp, K) with one row per phone, K = 1 + len(timbre_mels) <= 8; weight 0 belongs to ``mels``.
+        The mel decoder then reads ``MRTE.tc_latent_mix(phone_tokens, [mels, *timbre_mels], timbre_weights)``,
+        length-regulated with the durations used, instead of the target's latent, so the voice moves toward the prompts
+        (per phone, with a schedule).  The ADM and the prosody LM keep the target's latent (``duration_weights`` and
+        ``prosody_weights`` are their controls), so ``tc_latent``, ``dt`` and ``p_codes`` do not change; a full voice blend
+        passes the same prompts and weights to all three.  A prompt passed as the same tensor in ``prosody_mels`` and
+        ``timbre_mels`` is encoded once, and MRTE's phone encoder runs once per call.  ``return_intermediates`` adds
+        ``timbre_latent`` (B, Tp, H).
+        All arguments are checked on the host before any device work."""
         dev = phone_tokens.device
         self._check_prosody(phone_tokens, prosody_mels, prosody_weights, causal_decode, duration_weights, plm_context)
         control = _duration_control(phone_tokens, forced_durations, causal_decode, duration_scale, total_frames,
                                     pinned_durations)
+        timbre = self._check_timbre(phone_tokens, timbre_mels, timbre_weights)
         args = (phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt, sampling, keys,
                 prosody_mels, prosody_weights, duration_weights, plm_context, control)
-        out = self._synthesize(*args)
+        out = self._synthesize(*args, timbre=timbre)
         if check_range and _fp16_operands() and ops.tc_overflow(dev):
             _warn_fp16_range("re-running this batch on the bf16x3 engine")
             with pack.engine_scope(pack.ENGINE_BF16X3):
-                out = self._synthesize(*args)
+                out = self._synthesize(*args, timbre=timbre)
         if return_intermediates:
             return out
         return (out["wav"], out["wav_lens"]) if return_lengths else out["wav"]
@@ -1062,7 +1067,8 @@ class Megatts(nn.Module):
         for k in rejected:
             if k in ED.REJECTED:
                 raise L.MttsError(f"edit does not take {k}: an edit sets the durations and codes around the span "
-                                  "itself, on the reference-faithful decodes without a prosody mix or a prompt re-vocode")
+                                  "itself, on the reference-faithful decodes without a prosody mix or a prompt re-vocode, "
+                                  "and keeps the original voice")
         if rejected:
             raise TypeError(f"edit() got unexpected keyword argument(s) {sorted(rejected)}")
         plan = ED.EditPlan(phone_tokens, orig_phone, orig_durations, orig_codes, span, span_frames, self.plm.vq_bins)
@@ -1113,13 +1119,59 @@ class Megatts(nn.Module):
             ops._dev(m, name=f"prosody_mels[{k}]")
             if m.dim() != 3 or m.shape[0] != B or m.shape[2] != nb or m.shape[1] < 1:
                 raise L.MttsError(f"prosody_mels[{k}]: expected ({B}, Tm, {nb}), got {tuple(m.shape)}")
-        _synth_mix_weights(prosody_weights, 1 + len(prosody_mels), B, phone_tokens.shape[1], "prosody mix")
+        S.synth_mix_weights(prosody_weights, 1 + len(prosody_mels), B, phone_tokens.shape[1], "prosody mix")
         if duration_weights is not None:
-            _synth_mix_weights(duration_weights, 1 + len(prosody_mels), B, phone_tokens.shape[1], "duration mix")
+            S.synth_mix_weights(duration_weights, 1 + len(prosody_mels), B, phone_tokens.shape[1], "duration mix")
+
+    def _check_timbre(self, phone_tokens, timbre_mels, timbre_weights):
+        """-> (timbre_mels, their validated (B, K) or (B, Tp, K) CPU weights), or None without a timbre mix."""
+        if timbre_mels is None and timbre_weights is None:
+            return None
+        if timbre_mels is None:
+            raise L.MttsError("timbre_weights without timbre_mels")
+        if isinstance(timbre_mels, torch.Tensor) or not len(timbre_mels):
+            raise L.MttsError("timbre_mels must be a non-empty list of (B, Tm, mel_bins) tensors")
+        if timbre_weights is None:
+            raise L.MttsError("timbre_mels needs timbre_weights: (K,), (B, K) or (B, Tp, K), K = 1 + len(timbre_mels)")
+        K = 1 + len(timbre_mels)
+        if K > S.MIX_MAX_SOURCES:
+            raise L.MttsError(f"timbre_mels: {K - 1} prompts, at most {S.MIX_MAX_SOURCES - 1} (K = 1 + len(timbre_mels) "
+                              f"<= {S.MIX_MAX_SOURCES})")
+        B, Tp = phone_tokens.shape
+        check_prompts(timbre_mels, B, self.generator.mrte.mel_bins, "timbre_mels", phone_tokens.device)
+        return list(timbre_mels), S.synth_mix_weights(timbre_weights, K, B, Tp, "timbre_weights")
+
+    def _mrte(self, phone_tokens, mels, prosody_mels=None, timbre=None):
+        """The call's one MRTE pass -> (tc_latent of ``mels``, the latent of each prosody prompt or None, the timbre blend
+        or None).  Without prompts it is ``mrte.tc_latent(phone_tokens, mels)``.  With them the phone encoder runs once
+        (``MRTE.attend`` over [mels, *timbre_mels, the other prosody prompts]): a prosody prompt that is ``mels`` or one of
+        ``timbre_mels`` (the same tensor object) is not encoded again.  Every latent is ``tc_latent(phone_tokens, its mel)``
+        bit for bit, and the blend is ``MRTE.tc_latent_mix`` over [mels, *timbre_mels]."""
+        mrte = self.generator.mrte
+        if prosody_mels is None and timbre is None:
+            return mrte.tc_latent(phone_tokens, mels), None, None
+        srcs = [mels] + (timbre[0] if timbre is not None else [])
+        slot = {}
+        for k, m in enumerate(srcs):
+            slot.setdefault(id(m), k)
+        for m in prosody_mels or ():
+            if id(m) not in slot:
+                slot[id(m)] = len(srcs)
+                srcs.append(m)
+        ys = mrte.attend(phone_tokens, srcs)
+        lat = {}
+
+        def latent(k):
+            if k not in lat:
+                lat[k] = mrte.norm_relu(ys[k])
+            return lat[k]
+        prosody = None if prosody_mels is None else [latent(slot[id(m)]) for m in prosody_mels]
+        blend = None if timbre is None else mrte.norm_relu_mix(ys[:1 + len(timbre[0])], timbre[1])
+        return latent(0), prosody, blend
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
                     sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None,
-                    plm_context=None, control=None, code_pins=None):
+                    plm_context=None, control=None, code_pins=None, timbre=None):
         # ``code_pins`` (speech editing): totals, T -> the (B, T) code pins of MegaPLM.infer, built once the frame totals
         # are on the host.
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
@@ -1145,22 +1197,22 @@ class Megatts(nn.Module):
                 self._side_stream = torch.cuda.Stream(device=dev)
             side = self._side_stream
             if start == "adm":
-                tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
+                tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
             side.wait_stream(main)
             prompt_mels.record_stream(side)
             with torch.cuda.stream(side), ops.launch_policy(V, pairs=True, pdl=False):
                 pw_side = self.hifi_gan.decode_batch_cl(prompt_mels[:n_side])
             with ops.launch_policy(nsm - V, pairs=False, pdl=True):
                 if start != "adm":
-                    tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
-                dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights, control)
+                    tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
+                dt = self._durations(adm_decode, tc_latent, lats, duration_weights, control)
             main.wait_stream(side)
             pw_side.record_stream(main)
         else:
-            tc_latent = self.generator.mrte.tc_latent(phone_tokens, mels)
-            dt, lats = self._durations(adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights, control)
-        tc_expand, totals, src, step_w = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels, lats,
-                                                          prosody_weights)
+            tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
+            dt = self._durations(adm_decode, tc_latent, lats, duration_weights, control)
+        tc_expand, totals, src, step_w, dec_expand = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, lats,
+                                                                      prosody_weights, timbre_lat)
         if prosody_mels is not None:
             tc8 = src[0]
             p_codes = self.plm.infer_mix(src, prosody_weights if step_w is None else step_w, sampling=sampling, keys=keys)
@@ -1172,7 +1224,7 @@ class Megatts(nn.Module):
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]
         if all(t == Lmax for t in totals):
-            mel = self.generator.decode_mel_cl(tc_expand, p_codes)    # (B, L, 80) channels-last
+            mel = self.generator.decode_mel_cl(dec_expand, p_codes)   # (B, L, 80) channels-last
             wav = self.hifi_gan.decode_batch_cl(mel)
         else:
             # ragged totals: decoder + vocoder per group of equal length (exactly the reference's batch-1 results)
@@ -1182,7 +1234,7 @@ class Megatts(nn.Module):
                 idx = torch.tensor([i for i, t in enumerate(totals) if t == Lg], device=tc_expand.device)
                 if Lg == 0:
                     continue
-                mg = self.generator.decode_mel_cl(tc_expand[idx, :Lg].contiguous(), p_codes[idx, :(Lg + 7) // 8].contiguous())
+                mg = self.generator.decode_mel_cl(dec_expand[idx, :Lg].contiguous(), p_codes[idx, :(Lg + 7) // 8].contiguous())
                 wg = self.hifi_gan.decode_batch_cl(mg)
                 mel[idx, :Lg] = mg
                 wav[idx, :, :wg.shape[-1]] = wg
@@ -1200,12 +1252,13 @@ class Megatts(nn.Module):
                    mel=mel, wav=wav, totals=totals, wav_lens=wav_lens)
         if step_w is not None:
             out["prosody_step_weights"] = step_w
+        if timbre_lat is not None:
+            out["timbre_latent"] = timbre_lat
         return out
 
-    def _durations(self, adm_decode, tc_latent, phone_tokens, prosody_mels, duration_weights, control=None):
-        """-> (dt (B, Tp) int32, the prompts' MRTE latents or None).  Without ``duration_weights``: ``adm_decode`` on
-        ``tc_latent``, and the prompts' latents are left to ``_plm_source``.  With them: MRTE on (phone_tokens, prompt) for
-        each prosody prompt, then ``MegaADM.infer_mix`` over [tc_latent, *those latents].  ``control``, the validated
+    def _durations(self, adm_decode, tc_latent, prosody_latents, duration_weights, control=None):
+        """-> dt (B, Tp) int32.  Without ``duration_weights``: ``adm_decode`` on ``tc_latent``.  With them:
+        ``MegaADM.infer_mix`` over [tc_latent, *prosody_latents] (the prosody prompts' latents of ``_mrte``).  ``control``, the validated
         (scale, total, pins) of ``_duration_control``: the pins go into the ADM loop, and with a scale or a total the
         durations are ``ops.fit_durations`` of the decode's raw values."""
         scale, total, pins = control if control is not None else (None, None, None)
@@ -1213,45 +1266,44 @@ class Megatts(nn.Module):
         kw = {} if pins is None else {"pinned": pins}
         if fit:
             kw["return_raw"] = True
-        lats = None
         if duration_weights is None:
             out = adm_decode(tc_latent, **kw)
         else:
-            lats = [self.generator.mrte.tc_latent(phone_tokens, m) for m in prosody_mels]
-            out = self.adm.infer_mix([tc_latent] + lats, duration_weights, **kw)
+            out = self.adm.infer_mix([tc_latent] + prosody_latents, duration_weights, **kw)
         if fit:
-            return ops.fit_durations(out[1], scale, total, pins), lats
-        return out[..., 0], lats
+            return ops.fit_durations(out[1], scale, total, pins)
+        return out[..., 0]
 
-    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_mels, prosody_latents=None,
-                    prosody_weights=None):
+    def _plm_source(self, tc_latent, dt, forced_durations, phone_tokens, prosody_latents=None, prosody_weights=None,
+                    timbre_latent=None):
         """The synthesis front end between the ADM and the PLM: the durations (``forced_durations`` if given, else
         ``dt``) expand ``tc_latent`` to frames -> (tc_expand (B, Lmax, tc_dim), the per-utterance frame totals on the host
-        (one host sync), the PLM's source, the PLM's step weights).  The source is tc8, tc_expand max-pooled by 8, or with
-        ``prosody_mels`` the list [tc8, *one latent per prosody prompt]: MRTE on (phone_tokens, prompt) (or its
-        ``prosody_latents`` entry when the duration mix already computed it), length-regulated with the same durations to
-        Lmax frames, max-pooled by 8.  The step weights are None unless ``prosody_weights`` has one row per phone; then
-        they are its (B, ceil(Lmax / 8), K) expansion by the same durations (``ops.mix_step_weights``)."""
+        (one host sync), the PLM's source, the PLM's step weights, the mel decoder's latent frames).  The source is tc8,
+        tc_expand max-pooled by 8, or with ``prosody_latents`` (the prosody prompts' latents of ``_mrte``) the list
+        [tc8, *each latent length-regulated with the same durations to Lmax frames and max-pooled by 8].  The step weights
+        are None unless ``prosody_weights`` has one row per phone; then they are its (B, ceil(Lmax / 8), K) expansion by
+        the same durations (``ops.mix_step_weights``).  The decoder's frames are tc_expand, or ``timbre_latent``
+        length-regulated with the same durations to Lmax frames."""
         d_used = dt if forced_durations is None else forced_durations.to(dt.device, torch.int32)
         tc_expand, totals = ops.length_regulate(tc_latent, d_used, return_host_totals=True)   # one host sync
         tc8 = ops.maxpool_time(tc_expand, 8)
-        if prosody_mels is None:
-            return tc_expand, totals, tc8, None
-        mrte, Lmax = self.generator.mrte, tc_expand.shape[1]
-        lats = prosody_latents if prosody_latents is not None else (mrte.tc_latent(phone_tokens, m) for m in prosody_mels)
-        src = [tc8] + [ops.maxpool_time(ops.length_regulate(lat, d_used, l_out=Lmax)[0], 8) for lat in lats]
+        Lmax = tc_expand.shape[1]
+        dec_expand = tc_expand if timbre_latent is None else ops.length_regulate(timbre_latent, d_used, l_out=Lmax)[0]
+        if prosody_latents is None:
+            return tc_expand, totals, tc8, None, dec_expand
+        src = [tc8] + [ops.maxpool_time(ops.length_regulate(lat, d_used, l_out=Lmax)[0], 8) for lat in prosody_latents]
         step_w = None
         if S.per_step(prosody_weights):
             B, Tp = phone_tokens.shape
             pw = S.mix_step_weights(prosody_weights, len(src), B, Tp).to(tc8.device)
             step_w = ops.mix_step_weights(pw, d_used, tc8.shape[1])
-        return tc_expand, totals, src, step_w
+        return tc_expand, totals, src, step_w, dec_expand
 
     def synthesize_stream(self, phone_tokens: torch.Tensor, mels: torch.Tensor, forced_durations: torch.Tensor = None,
                           prompt_mels: torch.Tensor = None, sampling: S.Sampling = None, keys=None, check_range: bool = True,
                           chunk_frames: int = 64, prosody_mels=None, prosody_weights=None, duration_weights=None,
                           plm_context=None, duration_scale=None, total_frames=None, pinned_durations=None,
-                          **unsupported):
+                          timbre_mels=None, timbre_weights=None, **unsupported):
         """``synthesize`` as a generator of waveform chunks, each yielded as soon as the prosody LM has decoded the codes
         its samples depend on.  Arguments as in ``synthesize``; ``chunk_frames`` mel frames (hop = 256 samples each) per
         chunk.  Each chunk is a dict: ``wav`` (B, 1, n) device tensor, ``offset`` (its first sample's index in the waveform
@@ -1278,23 +1330,24 @@ class Megatts(nn.Module):
         self._check_prosody(phone_tokens, prosody_mels, prosody_weights, False, duration_weights, plm_context)
         control = _duration_control(phone_tokens, forced_durations, False, duration_scale, total_frames,
                                     pinned_durations)
+        timbre = self._check_timbre(phone_tokens, timbre_mels, timbre_weights)
         guard = check_range and _fp16_operands()
         return self._stream_outer(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard,
                                   int(chunk_frames), (prosody_mels, prosody_weights, duration_weights, plm_context),
-                                  control)
+                                  control, timbre)
 
     def _stream_outer(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
-                      prosody, control):
+                      prosody, control, timbre):
         try:
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames,
-                                    prosody, control)
+                                    prosody, control, timbre)
         except _RangeRestart:
             _warn_fp16_range("restarting this stream on the bf16x3 engine")
             yield from self._stream(phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, False, chunk_frames,
-                                    prosody, control, engine=pack.ENGINE_BF16X3)
+                                    prosody, control, timbre, engine=pack.ENGINE_BF16X3)
 
     def _stream(self, phone_tokens, mels, forced_durations, prompt_mels, sampling, keys, guard, chunk_frames, prosody,
-                control, engine=None):
+                control, timbre, engine=None):
         # The engine scope is entered around each computing step only, never across a yield: the caller's own work between
         # chunks keeps its engine.
         from .. import stream as SCH
@@ -1308,11 +1361,11 @@ class Megatts(nn.Module):
         hop, pad = HIFIGAN_HOP_LENGTH, voc.cfg["inference_padding"]
         hd, hv = gen.decoder.receptive_field(), voc.receptive_field()
         with torch.no_grad(), scope():
-            tc_latent = gen.mrte.tc_latent(phone_tokens, mels)
             prosody_mels, prosody_weights, duration_weights, plm_context = prosody
-            dt, lats = self._durations(self.adm.infer, tc_latent, phone_tokens, prosody_mels, duration_weights, control)
-            tc_expand, totals, src, step_w = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, prosody_mels,
-                                                              lats, prosody_weights)
+            tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
+            dt = self._durations(self.adm.infer, tc_latent, lats, duration_weights, control)
+            tc_expand, totals, src, step_w, dec_expand = self._plm_source(tc_latent, dt, forced_durations, phone_tokens,
+                                                                          lats, prosody_weights, timbre_lat)
             dec = self.plm.begin_decode(src, sampling=sampling, keys=keys,
                                         weights=prosody_weights if step_w is None else step_w, context=plm_context)
             pw = self.hifi_gan.decode_batch_cl(prompt_mels) if prompt_mels is not None else None
@@ -1350,7 +1403,7 @@ class Megatts(nn.Module):
             wav = torch.zeros(B, 1, n, dtype=torch.float32, device=dev)
             for (rows, win), idx in groups(k, lambda c: (c.rows, c.dec) if c.dec is not None else None):
                 (r0, r1), (da, db) = rows, win
-                m = gen.decode_mel_cl(tc_expand[idx, da:db].contiguous(), dec.target[idx, da // 8:-(-db // 8)])
+                m = gen.decode_mel_cl(dec_expand[idx, da:db].contiguous(), dec.target[idx, da // 8:-(-db // 8)])
                 mel[idx, r0:r1] = m[:, r0 - da:r1 - da]
             for (p0, p1, va, vb), idx in groups(k, lambda c: (c.p0, c.p1) + c.voc):
                 w = self.hifi_gan.decode_batch_cl(mel[idx, va:vb])
@@ -1392,6 +1445,9 @@ class Megatts(nn.Module):
         ``duration_scale`` is: the buckets regroup the utterances, so per-utterance values would not line up."""
         if "prosody_mels" in kw or "prosody_weights" in kw or "plm_context" in kw:
             raise L.MttsError("synthesize_many does not take prosody prompts or a PLM context; call synthesize per batch")
+        if "timbre_mels" in kw or "timbre_weights" in kw:
+            raise L.MttsError("synthesize_many does not take timbre_mels or timbre_weights (timbre prompts); call "
+                              "synthesize per batch")
         if "total_frames" in kw or "pinned_durations" in kw:
             raise L.MttsError("synthesize_many does not take total_frames or pinned_durations (per-utterance values); "
                               "call synthesize per batch")

@@ -8,6 +8,7 @@ import torch.nn as nn
 
 from .. import _lib as L
 from .. import ops
+from .. import sampling as S
 from .convnet import ConvNetDouble
 from .embedding import SinePositionalEmbedding, TokenEmbedding
 from .tokenizer import HIFIGAN_HOP_LENGTH, HIFIGAN_MEL_CHANNELS, HIFIGAN_SR
@@ -33,6 +34,16 @@ class LengthRegulator(nn.Module):
                 z[:, :y.size(1)] = y
                 y = z
         return y
+
+
+def check_prompts(mels, B, mel_bins, name, device):
+    """Every prompt of the list ``mels`` is a CUDA fp32 (B, Tm >= 1, mel_bins) tensor on ``device``."""
+    for k, m in enumerate(mels):
+        ops._dev(m, name=f"{name}[{k}]")
+        if m.dim() != 3 or m.shape[0] != B or m.shape[2] != mel_bins or m.shape[1] < 1:
+            raise L.MttsError(f"{name}[{k}]: expected ({B}, Tm, {mel_bins}), got {tuple(m.shape)}")
+        if m.device != device:
+            raise L.MttsError(f"{name}[{k}]: on {m.device}, expected {device}")
 
 
 class MRTE(nn.Module):
@@ -80,6 +91,48 @@ class MRTE(nn.Module):
         # LayerNorm -> ReLU fused (mrte.py:168-169)
         return ops.layernorm(y, self.norm.weight.detach(), self.norm.bias.detach(), eps=self.norm.eps,
                              post_act=L.ACT_RELU, out=y)
+
+    def attend(self, phone: torch.Tensor, mels) -> torch.Tensor:
+        """The pre-norm attention outputs of K mels: phone (B,Tp) int64, ``mels`` K tensors (B, Tm_k, mel_bins) ->
+        ys (K, B, Tp, hidden), ys[k] = MHA(phone_x, kv=mel_encoder(mels[k])), the y of ``tc_latent(phone, mels[k])`` bit
+        for bit.  The phone encoder runs once; each mel runs its mel encoder and the MHA."""
+        if self.training:
+            raise L.MttsError("training-mode dropout is outside the synthesis path (call .eval())")
+        pe = self.phone_pos_embedding
+        pe.extend_pe(phone)
+        x = ops.embed_pe(phone, self.phone_embedding.word_embeddings.weight.detach(), pe.pe, pe.alpha_host())
+        phone_x = self.phone_encoder(x)
+        ys = torch.empty(len(mels), *phone_x.shape, dtype=torch.float32, device=phone_x.device)
+        for k, mel in enumerate(mels):
+            self.mha(phone_x, kv=self.mel_encoder.forward_cl(mel), out=ys[k])
+        return ys
+
+    def norm_relu(self, y: torch.Tensor) -> torch.Tensor:
+        """ReLU(LayerNorm(y)) into a new tensor: ``tc_latent``'s last step (mrte.py:168-169)."""
+        return ops.layernorm(y, self.norm.weight.detach(), self.norm.bias.detach(), eps=self.norm.eps,
+                             post_act=L.ACT_RELU)
+
+    def norm_relu_mix(self, ys: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
+        """ReLU(LayerNorm(sum_k w^_k ys[k])) (ops.mix_layernorm) for the validated CPU ``weights`` (B, K) or (B, Tp, K)."""
+        return ops.mix_layernorm(ys, weights.to(ys.device), self.norm.weight.detach(), self.norm.bias.detach(),
+                                 eps=self.norm.eps, post_act=L.ACT_RELU)
+
+    def tc_latent_mix(self, phone: torch.Tensor, mels, weights) -> torch.Tensor:
+        """Timbre interpolation: the MRTE latent of a weighted mix of K prompts.  ``mels``: K tensors (B, Tm_k, mel_bins)
+        (the Tm_k may differ); ``weights``: (K,), (B, K) or (B, Tp, K) with one row per phone, >= 0, each row with a
+        positive sum (normalised to w^).  -> (B, Tp, hidden) = ReLU(LayerNorm(sum_k w^_k y_k)), y_k the pre-norm attention
+        output of ``tc_latent(phone, mels[k])``: since the out-projection is affine, that is attention under the
+        w^-weighted mixture of the per-prompt attention distributions, normalised back onto the latent's scale.  A row
+        with one positive weight, on source k, is ``tc_latent(phone, mels[k])``'s row bit for bit.  The phone encoder
+        runs once (``attend``); include/megatts2_b200.h (mtts_mix_layernorm_f32) states the mix."""
+        if isinstance(mels, torch.Tensor) or not len(mels):
+            raise L.MttsError("tc_latent_mix: mels must be a non-empty list of (B, Tm, mel_bins) tensors")
+        if phone.dim() != 2:
+            raise L.MttsError(f"tc_latent_mix: phone must be (B, Tp), got {tuple(phone.shape)}")
+        B, Tp = phone.shape
+        w = S.synth_mix_weights(weights, len(mels), B, Tp, "tc_latent_mix weights")
+        check_prompts(mels, B, self.mel_bins, "mels", phone.device)
+        return self.norm_relu_mix(self.attend(phone, mels), w)
 
     def forward(self, duration_tokens: torch.Tensor, phone: torch.Tensor, phone_lens: torch.Tensor,
                 mel: torch.Tensor):

@@ -57,9 +57,11 @@ class MultiHeadAttention(pack.PlanMixin, nn.Module):
             self._plan = pl
         return self._plan
 
-    def forward(self, q, kv=None, mask=None):
-        """q (B,Tq,D), kv (B,Tk,D) or None (self-attention), additive mask broadcastable to (B,H,Tq,Tk)."""
+    def forward(self, q, kv=None, mask=None, out=None):
+        """q (B,Tq,D), kv (B,Tk,D) or None (self-attention), additive mask broadcastable to (B,H,Tq,Tk).  ``out``: an
+        optional contiguous (B,Tq,D) fp32 tensor the out-projection writes into (inference only)."""
         if self.training:
+            assert out is None, "training-mode attention allocates its own output"
             return self.forward_train(q, kv, mask)
         pl = self._packed()
         D = self.qkv_dim
@@ -71,7 +73,7 @@ class MultiHeadAttention(pack.PlanMixin, nn.Module):
             kvp = ops.linear(kv, pl.wkv, pl.bkv)
             kk, vv = kvp[..., :D], kvp[..., D:]
         att = ops.attention(qq, kk, vv, self.n_heads, mask)
-        return ops.linear(att, pl.wo, self.out_proj[0].bias.detach())
+        return ops.linear(att, pl.wo, self.out_proj[0].bias.detach(), out=out)
 
 
 def _mha_forward_train(self, q, kv=None, mask=None):

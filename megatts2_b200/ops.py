@@ -145,6 +145,31 @@ def layernorm(x, gamma, beta, *, res=None, out=None, eps=1e-5, post_act=L.ACT_NO
     return out
 
 
+def mix_layernorm(ys, weights, gamma, beta, *, eps=1e-5, post_act=L.ACT_NONE, out=None):
+    """Timbre mix (include/megatts2_b200.h, mtts_mix_layernorm_f32): ys (K, B, T, C) fp32, the K sources' rows; weights
+    (K,), (B, K) or (B, T, K) fp32 on ys's device, used as given (validate them with ``sampling.mix_weights`` /
+    ``mix_step_weights``) -> (B, T, C) = post(LayerNorm(sum_k w^_k ys[k])), w^ each row normalised to sum 1.  A row with
+    one positive weight gives ``layernorm`` of that source's row bit for bit."""
+    ys = _dev(ys, name="ys")
+    if ys.dim() != 4:
+        raise L.MttsError(f"mix_layernorm: ys must be (K, B, T, C), got {tuple(ys.shape)}")
+    K, B, T, Cc = ys.shape
+    if not (ys.stride(3) == 1 and ys.stride(1) == T * ys.stride(2)):
+        ys = ys.contiguous()
+    w = _dev(weights, name="weights").contiguous()
+    strides = {(K,): (0, 0), (B, K): (K, 0), (B, T, K): (T * K, K)}.get(tuple(w.shape))
+    if strides is None:
+        raise L.MttsError(f"mix_layernorm: weights of shape {tuple(w.shape)}, expected ({K},), ({B}, {K}) or "
+                          f"({B}, {T}, {K})")
+    if out is None:
+        out = torch.empty(B, T, Cc, dtype=_F32, device=ys.device)
+    o2 = out.reshape(-1, Cc)
+    L.check(L.lib().mtts_mix_layernorm_f32(_ptr(ys), ys.stride(0), ys.stride(2), K, _ptr(w), *strides, max(T, 1),
+                                           _ptr(_dev(gamma)), _ptr(_dev(beta)), _ptr(o2), o2.stride(0), B * T, Cc,
+                                           eps, post_act, _stream()))
+    return out
+
+
 def attention(q, k, v, n_heads, mask=None):
     """q (B,Tq,D), k/v (B,Tk,D) (any row strides, unit channel stride) -> (B,Tq,D).
     mask: additive fp32 broadcastable to (B,H,Tq,Tk).  Under an fp16-range default engine (f16x2, f16) long sequences

@@ -83,13 +83,18 @@ def _real_weights(weights, what, shapes):
 
 def _checked_rows(w64, what):
     """fp64 weights whose last dim is one weight row -> the rows as a contiguous fp32 tensor, every weight finite and
-    >= 0 and every row with a positive fp32 sum."""
-    if not bool(torch.isfinite(w64).all()) or bool((w64 < 0).any()):
-        raise L.MttsError(f"{what}: every weight must be finite and >= 0")
+    >= 0 and every row with a positive fp32 sum.  An error names the first bad weight or row by its index."""
+    bad = ~torch.isfinite(w64) | (w64 < 0)
+    if bool(bad.any()):
+        i = tuple(int(x) for x in bad.nonzero()[0])
+        raise L.MttsError(f"{what}: weight {list(i)} = {float(w64[i])}: every weight must be finite and >= 0")
     w32 = w64.to(torch.float32).contiguous()
     s = w32.sum(-1)
-    if not bool(torch.isfinite(s).all()) or bool((s <= 0).any()):
-        raise L.MttsError(f"{what}: every weight row needs a positive, finite sum")
+    bad = ~torch.isfinite(s) | (s <= 0)
+    if bool(bad.any()):
+        r = tuple(int(x) for x in bad.nonzero()[0])
+        raise L.MttsError(f"{what}: weight row {list(r)} sums to {float(s[r])}: every weight row needs a positive, finite "
+                          "sum")
     return w32
 
 
@@ -125,6 +130,14 @@ def mix_step_weights(weights, K, B, T, what="prosody mix"):
     if tuple(w.shape) != (B, T, K):
         raise L.MttsError(f"{what}: weights of shape {tuple(w.shape)}, expected ({B}, {T}, {K}) (one row per step)")
     return _checked_rows(w.to(device="cpu", dtype=torch.float64), what)
+
+
+def synth_mix_weights(weights, K, B, Tp, what):
+    """The validated (B, K) CPU weights of a synthesis mix over Tp phones, or (B, Tp, K) when ``weights`` has one row
+    per phone."""
+    if per_step(weights):
+        return mix_step_weights(weights, K, B, Tp, what)
+    return mix_weights(weights, K, B, what)
 
 
 DURATION_MAX = 128          # the ADM's durations are 1..128 frames
