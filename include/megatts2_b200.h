@@ -391,6 +391,24 @@ int mtts_vq_ste_commit_bwd_f32(const float* x, const float* out, const float* g_
  * decode_batch(mel, mel_lens, hop_len) (reference call site models/megatts2.py:370). */
 int mtts_mask_tail_f32(float* x, int32_t B, int32_t rows, int32_t L, const int32_t* keep, void* stream);
 
+/* Ragged row copy, one launch for B batch rows (long-form synthesis joins sentences with it: the prosody LM's context
+ * history, its window, and the passage mel).  A buffer holds B batch rows of `*_rows` logical rows of row_bytes bytes;
+ * logical row r of batch row b starts at byte b*sb + r*st.  For b < B and 0 <= r < min(n[b], n_max):
+ *   dst[b, dst_off[b] + r] = src ? src[b, src_off[b] + r] : row_bytes / 4 copies of fill_word,
+ * and only for the r with 0 <= dst_off[b] + r < dst_rows and (with src) 0 <= src_off[b] + r < src_rows: entries of the
+ * tables that would run past either buffer, or below row 0, copy only the rows inside it, so no table value can reach
+ * memory outside the two buffers.  Nothing else of dst is written.  The tables src_off, dst_off and n are (B,) int32 in
+ * device memory; src_off may be NULL when src is (fill mode).  row_bytes is a positive multiple of 4 (so one entry serves
+ * fp32 rows and int64 codes); strides are byte counts, multiples of 4, row strides >= row_bytes, batch strides >= 0
+ * (src_sb = 0 broadcasts one src batch row), and dst's batch rows must not overlap.  16-byte accesses are used when
+ * both bases, every stride and row_bytes are multiples of 16, 4-byte words otherwise.  src and dst must differ and must
+ * not overlap.  B <= 65535.  Every argument is checked before anything is enqueued; B, n_max or dst_rows = 0 does
+ * nothing. */
+int mtts_copy_row_segments(const void* src, int64_t src_sb, int64_t src_st, int64_t src_rows, void* dst, int64_t dst_sb,
+                           int64_t dst_st, int64_t dst_rows, int32_t row_bytes, const int32_t* src_off,
+                           const int32_t* dst_off, const int32_t* n, int32_t B, int32_t n_max, uint32_t fill_word,
+                           void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Composite drivers: whole sub-networks enqueued by one call (C++ launch loop, no Python
  * per-kernel overhead).  Weight pointers refer to PRE-PACKED device buffers owned by the

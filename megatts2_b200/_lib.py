@@ -132,6 +132,8 @@ SIGNATURES = {
     "mtts_set_attention_pair_min": (C.c_int, [i32]),
     "mtts_attention_plan_query": (C.c_int, [C.POINTER(AttnParams), i32, i32, C.POINTER(i32)]),
     "mtts_mask_tail_f32": (C.c_int, [vp, i32, i32, i32, vp, vp]),
+    "mtts_copy_row_segments": (C.c_int, [vp, i64, i64, i64, vp, i64, i64, i64, i32, vp, vp, vp, i32, i32, C.c_uint32,
+                                         vp]),
     "mtts_resample_f32": (C.c_int, [vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, vp, i64, i32, vp, vp]),
     "mtts_peak_normalize_f32": (C.c_int, [vp, i64, i32, i32, vp, vp, vp]),
     "mtts_pcm16_f32": (C.c_int, [vp, i64, vp, vp]),

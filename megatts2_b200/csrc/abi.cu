@@ -209,6 +209,14 @@ int mtts_mask_tail_f32(float* x, int32_t B, int32_t rows, int32_t L, const int32
   return mask_tail(x, B, rows, L, keep, (cudaStream_t)stream);
 }
 
+int mtts_copy_row_segments(const void* src, int64_t src_sb, int64_t src_st, int64_t src_rows, void* dst, int64_t dst_sb,
+                           int64_t dst_st, int64_t dst_rows, int32_t row_bytes, const int32_t* src_off,
+                           const int32_t* dst_off, const int32_t* n, int32_t B, int32_t n_max, uint32_t fill_word,
+                           void* stream) {
+  return copy_row_segments(src, src_sb, src_st, src_rows, dst, dst_sb, dst_st, dst_rows, row_bytes, src_off, dst_off, n,
+                           B, n_max, fill_word, (cudaStream_t)stream);
+}
+
 int mtts_copy_strided_f32(const float* x, int64_t x_sb, int64_t x_st, int64_t x_sc, float* y, int64_t y_sb, int64_t y_st,
                           int64_t y_sc, int32_t B, int32_t T, int32_t C, int32_t pad_rep, void* stream) {
   return copy_strided(x, x_sb, x_st, x_sc, y, y_sb, y_st, y_sc, B, T, C, pad_rep, (cudaStream_t)stream);

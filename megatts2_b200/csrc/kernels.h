@@ -138,6 +138,10 @@ int split_pad(const float* x, int64_t x_sb, int ldx, int B, int T, int C, int hl
               void* planes_base, int fmt, cudaStream_t st);
 int tc_overflow_bind(int32_t* flag);
 int mask_tail(float* x, int B, int rows, int L, const int32_t* keep, cudaStream_t st);
+// ragged row copy / fill, one launch for B batch rows (mtts_copy_row_segments)
+int copy_row_segments(const void* src, int64_t src_sb, int64_t src_st, int64_t src_rows, void* dst, int64_t dst_sb,
+                      int64_t dst_st, int64_t dst_rows, int row_bytes, const int32_t* src_off, const int32_t* dst_off,
+                      const int32_t* n, int B, int n_max, uint32_t fill_word, cudaStream_t st);
 int layernorm(const float* x, int ldx, const float* gamma, const float* beta, const float* res, int ldr, float* y,
               int ldy, int64_t rows, int C, float eps, int post_act, int accumulate, cudaStream_t st);
 // timbre mix: rows r = b T + t of K sources y + k y_ks mixed by the weight rows w + b w_sb + t w_st, then LayerNorm +

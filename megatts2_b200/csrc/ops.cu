@@ -868,6 +868,70 @@ int mask_tail(float* x, int B, int rows, int L, const int32_t* keep, cudaStream_
   return 0;
 }
 
+// Ragged row copy (the contract is stated with mtts_copy_row_segments in include/megatts2_b200.h): CTA row y = batch row
+// b, the x CTAs stride over the (row, word) pairs of b's segment.  The segment is clipped on the device to the rows that
+// lie inside both buffers, so no table value can move an access outside them.  W is uint4 when every address is 16-byte
+// aligned, else uint32_t.
+template <typename W>
+__global__ void copy_row_segments_kernel(const char* __restrict__ src, int64_t src_sb, int64_t src_st, int64_t src_rows,
+                                         char* __restrict__ dst, int64_t dst_sb, int64_t dst_st, int64_t dst_rows,
+                                         int words, const int32_t* __restrict__ src_off,
+                                         const int32_t* __restrict__ dst_off, const int32_t* __restrict__ n, int n_max,
+                                         uint32_t fill_word) {
+  pdl_entry();
+  const int b = blockIdx.y;
+  const int64_t d0 = dst_off[b];
+  const int64_t s0 = src ? (int64_t)src_off[b] : 0;
+  int64_t r0 = d0 < 0 ? -d0 : 0;
+  int64_t r1 = min(min((int64_t)n[b], (int64_t)n_max), dst_rows - d0);
+  if (src) {
+    r0 = max(r0, -s0);
+    r1 = min(r1, src_rows - s0);
+  }
+  if (r1 <= r0) return;
+  W fill;
+  const uint32_t* fw = &fill_word;
+  if constexpr (sizeof(W) == 16) fill = make_uint4(*fw, *fw, *fw, *fw);
+  else fill = *fw;
+  const int64_t total = (r1 - r0) * words;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = r0 + i / words;
+    const int w = (int)(i % words);
+    W* dp = reinterpret_cast<W*>(dst + b * dst_sb + (d0 + r) * dst_st) + w;
+    *dp = src ? reinterpret_cast<const W*>(src + b * src_sb + (s0 + r) * src_st)[w] : fill;
+  }
+}
+
+int copy_row_segments(const void* src, int64_t src_sb, int64_t src_st, int64_t src_rows, void* dst, int64_t dst_sb,
+                      int64_t dst_st, int64_t dst_rows, int row_bytes, const int32_t* src_off, const int32_t* dst_off,
+                      const int32_t* n, int B, int n_max, uint32_t fill_word, cudaStream_t st) {
+  MTTS_REQUIRE(dst && dst_off && n && (!src || src_off), "null pointer (dst, dst_off and n always; src_off with src)");
+  MTTS_REQUIRE(src != dst, "src and dst must differ");
+  MTTS_REQUIRE(row_bytes > 0 && row_bytes % 4 == 0, "row_bytes must be a positive multiple of 4");
+  MTTS_REQUIRE(B >= 0 && B <= 65535, "B must be in 0..65535");
+  MTTS_REQUIRE(n_max >= 0, "n_max must be >= 0");
+  MTTS_REQUIRE(src_rows >= 0 && dst_rows >= 0, "src_rows and dst_rows must be >= 0");
+  MTTS_REQUIRE(src_sb >= 0 && src_st >= row_bytes && dst_sb >= 0 && dst_st >= row_bytes &&
+                   (src_sb | src_st | dst_sb | dst_st) % 4 == 0,
+               "strides must be multiples of 4 bytes, row strides >= row_bytes and batch strides >= 0");
+  MTTS_REQUIRE(B <= 1 || dst_rows == 0 || dst_sb >= dst_rows * dst_st, "dst's batch rows must not overlap");
+  MTTS_REQUIRE((((uintptr_t)src) & 3) == 0 && (((uintptr_t)dst) & 3) == 0, "src and dst must be 4-byte aligned");
+  if (B == 0 || n_max == 0 || dst_rows == 0) return 0;
+  const bool v16 = (((uintptr_t)src | (uintptr_t)dst) & 15) == 0 && row_bytes % 16 == 0 &&
+                   (src_sb | src_st | dst_sb | dst_st) % 16 == 0;
+  const int words = row_bytes / (v16 ? 16 : 4);
+  const int64_t per_b = (int64_t)n_max * words;
+  const dim3 grid((unsigned)(cdiv64(per_b, 256) < 128 ? cdiv64(per_b, 256) : 128), (unsigned)B);
+  if (v16)
+    launch_k(copy_row_segments_kernel<uint4>, grid, 256, 0, st, (const char*)src, src_sb, src_st, src_rows, (char*)dst,
+             dst_sb, dst_st, dst_rows, words, src_off, dst_off, n, n_max, fill_word);
+  else
+    launch_k(copy_row_segments_kernel<uint32_t>, grid, 256, 0, st, (const char*)src, src_sb, src_st, src_rows,
+             (char*)dst, dst_sb, dst_st, dst_rows, words, src_off, dst_off, n, n_max, fill_word);
+  MTTS_CHECK_LAUNCH();
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 // Autoregressive-loop helpers (device-resident state: no host sync inside the loops).
 

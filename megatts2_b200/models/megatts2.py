@@ -19,6 +19,7 @@ from .. import _lib as L
 from .. import autograd as A
 from .. import ops, pack
 from .. import edit as ED
+from .. import passage as PS
 from .. import sampling as S
 from ..modules.convnet import ConvNet
 from ..modules.embedding import SinePositionalEmbedding
@@ -93,6 +94,14 @@ class PLMContext:
     @property
     def P(self):
         return self.tc8.shape[1]
+
+    @staticmethod
+    def from_rows(tc8, codes, max_code) -> "PLMContext":
+        """A context from device rows whose codes are known to be in [0, max_code] (the prosody LM's own codes, or a
+        checked context's), without the host read of ``__init__``."""
+        out = PLMContext.__new__(PLMContext)
+        out.tc8, out.codes, out.max_code = tc8.contiguous(), codes.contiguous(), max_code
+        return out
 
     @staticmethod
     def cat(contexts) -> "PLMContext":
@@ -1141,14 +1150,18 @@ class Megatts(nn.Module):
         check_prompts(timbre_mels, B, self.generator.mrte.mel_bins, "timbre_mels", phone_tokens.device)
         return list(timbre_mels), S.synth_mix_weights(timbre_weights, K, B, Tp, "timbre_weights")
 
-    def _mrte(self, phone_tokens, mels, prosody_mels=None, timbre=None):
+    def _mrte(self, phone_tokens, mels, prosody_mels=None, timbre=None, mel_context=None):
         """The call's one MRTE pass -> (tc_latent of ``mels``, the latent of each prosody prompt or None, the timbre blend
         or None).  Without prompts it is ``mrte.tc_latent(phone_tokens, mels)``.  With them the phone encoder runs once
         (``MRTE.attend`` over [mels, *timbre_mels, the other prosody prompts]): a prosody prompt that is ``mels`` or one of
         ``timbre_mels`` (the same tensor object) is not encoded again.  Every latent is ``tc_latent(phone_tokens, its mel)``
-        bit for bit, and the blend is ``MRTE.tc_latent_mix`` over [mels, *timbre_mels]."""
+        bit for bit, and the blend is ``MRTE.tc_latent_mix`` over [mels, *timbre_mels].  ``mel_context``:
+        ``MRTE.encode_prompt(mels)``, computed once for several calls (a passage's sentences), so ``mels`` is not encoded
+        here."""
         mrte = self.generator.mrte
         if prosody_mels is None and timbre is None:
+            if mel_context is not None:
+                return mrte.tc_latent(phone_tokens, mel_context=mel_context), None, None
             return mrte.tc_latent(phone_tokens, mels), None, None
         srcs = [mels] + (timbre[0] if timbre is not None else [])
         slot = {}
@@ -1158,7 +1171,7 @@ class Megatts(nn.Module):
             if id(m) not in slot:
                 slot[id(m)] = len(srcs)
                 srcs.append(m)
-        ys = mrte.attend(phone_tokens, srcs)
+        ys = mrte.attend(phone_tokens, srcs, None if mel_context is None else [mel_context] + [None] * (len(srcs) - 1))
         lat = {}
 
         def latent(k):
@@ -1171,9 +1184,10 @@ class Megatts(nn.Module):
 
     def _synthesize(self, phone_tokens, mels, forced_durations, causal_decode, prompt_mels, overlap_prompt=None,
                     sampling=None, keys=None, prosody_mels=None, prosody_weights=None, duration_weights=None,
-                    plm_context=None, control=None, code_pins=None, timbre=None):
+                    plm_context=None, control=None, code_pins=None, timbre=None, mel_context=None, mel_only=False):
         # ``code_pins`` (speech editing): totals, T -> the (B, T) code pins of MegaPLM.infer, built once the frame totals
-        # are on the host.
+        # are on the host.  ``mel_context`` (long-form synthesis): ``MRTE.encode_prompt(mels)``, encoded once per passage.
+        # ``mel_only`` stops after the mel decoder: the result has no ``wav`` or ``wav_lens``.
         # The prompt re-vocode (:371-372) depends on nothing the synthesis computes, and the ADM loop (latency-bound: ~4 k short
         # dependent launches that fill a fraction of the SMs) leaves most of the device idle: the re-vocode is enqueued first,
         # on a side stream with an SM budget of V, and MRTE + ADM run beside it on the other SMs.  ops.launch_policy carries
@@ -1197,19 +1211,19 @@ class Megatts(nn.Module):
                 self._side_stream = torch.cuda.Stream(device=dev)
             side = self._side_stream
             if start == "adm":
-                tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
+                tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre, mel_context)
             side.wait_stream(main)
             prompt_mels.record_stream(side)
             with torch.cuda.stream(side), ops.launch_policy(V, pairs=True, pdl=False):
                 pw_side = self.hifi_gan.decode_batch_cl(prompt_mels[:n_side])
             with ops.launch_policy(nsm - V, pairs=False, pdl=True):
                 if start != "adm":
-                    tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
+                    tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre, mel_context)
                 dt = self._durations(adm_decode, tc_latent, lats, duration_weights, control)
             main.wait_stream(side)
             pw_side.record_stream(main)
         else:
-            tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre)
+            tc_latent, lats, timbre_lat = self._mrte(phone_tokens, mels, prosody_mels, timbre, mel_context)
             dt = self._durations(adm_decode, tc_latent, lats, duration_weights, control)
         tc_expand, totals, src, step_w, dec_expand = self._plm_source(tc_latent, dt, forced_durations, phone_tokens, lats,
                                                                       prosody_weights, timbre_lat)
@@ -1223,6 +1237,9 @@ class Megatts(nn.Module):
         B, Lmax = tc_expand.shape[0], tc_expand.shape[1]
         hop = HIFIGAN_HOP_LENGTH
         pad = self.hifi_gan.generator.cfg["inference_padding"]
+        if mel_only:
+            return dict(tc_latent=tc_latent, dt=dt, tc_latent_expand=tc_expand, tc8=tc8, p_codes=p_codes,
+                        mel=self._decode_mel(dec_expand, p_codes, totals), totals=totals)
         if all(t == Lmax for t in totals):
             mel = self.generator.decode_mel_cl(dec_expand, p_codes)   # (B, L, 80) channels-last
             wav = self.hifi_gan.decode_batch_cl(mel)
@@ -1255,6 +1272,19 @@ class Megatts(nn.Module):
         if timbre_lat is not None:
             out["timbre_latent"] = timbre_lat
         return out
+
+    def _decode_mel(self, dec_expand, p_codes, totals):
+        """The mel decoder of ``_synthesize`` without the vocoder: one launch sequence when every total is Lmax, else one
+        per group of equal totals (zero rows past a total)."""
+        B, Lmax = dec_expand.shape[0], dec_expand.shape[1]
+        if all(t == Lmax for t in totals):
+            return self.generator.decode_mel_cl(dec_expand, p_codes)
+        mel = torch.zeros(B, Lmax, self.generator.mrte.mel_bins, dtype=torch.float32, device=dec_expand.device)
+        for Lg in sorted(set(totals) - {0}):
+            idx = torch.tensor([i for i, t in enumerate(totals) if t == Lg], device=dec_expand.device)
+            mel[idx, :Lg] = self.generator.decode_mel_cl(dec_expand[idx, :Lg].contiguous(),
+                                                         p_codes[idx, :(Lg + 7) // 8].contiguous())
+        return mel
 
     def _durations(self, adm_decode, tc_latent, prosody_latents, duration_weights, control=None):
         """-> dt (B, Tp) int32.  Without ``duration_weights``: ``adm_decode`` on ``tc_latent``.  With them:
@@ -1433,6 +1463,137 @@ class Megatts(nn.Module):
                 chunk.update(p_codes=dec.target.clone(), dt=dt, mel=mel,
                              wav_lens=[hop * (t + 2 * pad) + off0 for t in totals])
             yield chunk
+
+    @torch.no_grad()
+    def synthesize_passage(self, sentences, mels, pause_frames=0, context_rows: int = 128, plm_context=None,
+                           forced_durations=None, duration_scale=None, sampling: S.Sampling = None, keys=None,
+                           check_range: bool = True, return_lengths: bool = False, return_intermediates: bool = False,
+                           **rejected):
+        """Long-form synthesis: a passage of S sentences, each decoded with the sentences before it as the prosody LM's
+        context, vocoded as one waveform.  ``sentences``: S phone tensors (B, Tp_i) int64 on one device; row b of each
+        belongs to passage b (B voices or takes of one text).  ``mels`` (B, Tm, 80): the voice prompt, encoded once.
+
+        Sentence i runs what ``synthesize(sentences[i], mels, plm_context=W_i)`` runs up to the mel decoder: MRTE and
+        the ADM see the sentence alone, the regime they were trained on.  W_i is the last P_i = min(context_rows, min_b
+        H_b) rows of each row's history: the rows of ``plm_context`` (Bc = 1 or B), then each earlier sentence's
+        ceil(L / 8) valid max-pooled latents and codes (megatts2_b200/passage.py states the rule).  The window is
+        bounded, so the cost is linear in S.  The default of 128 rows (1024 mel frames, about 16 s at 16 kHz: several
+        sentences) costs about 1.1x the plain PLM decode at B = 1 and 4.4x at B = 64 (DESIGN.md section 7);
+        ``context_rows=0`` makes the sentences independent.  Sampled sentence i of row b draws with the key
+        ``keys[b] + i * 2^32``, so sentence 0 is ``synthesize``'s take and no two sentences share noise.
+
+        Row b's passage mel is its sentences' frames with ``pause_frames`` (an int, or (B, S - 1) ints >= 0) frames of
+        silence (log 1e-5, the front end's floor) after each but the last; the vocoder runs once over it, per group of
+        equal passage length, so sentence edges are ordinary frames to it.  ``forced_durations``: None or one (B, Tp_i)
+        tensor per sentence; ``duration_scale``: a number or (B,); they do not combine.  ``check_range``: the range flag
+        is read after the prompt's encoding, each sentence and the vocoder, and a raised flag redoes that piece alone on
+        bf16x3.  The AR decodes run eagerly: the callers' CUDA-graph caches are left as they were.
+
+        -> wav (B, 1, 256 (max F + 10)) [, wav_lens with ``return_lengths``: 256 (F_b + 10)]; ``return_intermediates``
+        gives a dict with ``wav``, ``wav_lens``, ``mel`` (B, max F, 80), ``frame_offsets`` (B, S) (sentence i of row b
+        starts at frame f, sample 256 (5 + f)), ``context_rows_used`` (S,) and ``sentences`` (per sentence ``dt``,
+        ``p_codes``, ``tc8``, ``totals``).  Every argument is checked on the host before any device work;
+        ``synthesize``'s arguments a passage does not take are rejected by name."""
+        plan = self._passage_plan(sentences, mels, pause_frames, context_rows, plm_context, forced_durations,
+                                  duration_scale, sampling, keys, rejected)
+        guard = check_range and _fp16_operands()
+        B, hop, pad = plan.B, HIFIGAN_HOP_LENGTH, self.hifi_gan.generator.cfg["inference_padding"]
+        pm = PS.PassageMel(B, self.generator.mrte.mel_bins, plan.device)
+        sents, used = [], []
+        for i, (out, P) in enumerate(PS.run_sentences(self, plan, guard)):
+            pm.place(out["mel"], out["totals"], [p[i] for p in plan.pauses] if i < plan.S - 1 else None)
+            sents.append({k: out[k] for k in ("dt", "p_codes", "tc8", "totals")})
+            used.append(P)
+        offsets, F = PS.frame_offsets([s["totals"] for s in sents], plan.pauses)
+        Fmax = max(F)
+        mel = pm.buf[:, :Fmax]
+        wav = torch.zeros(B, 1, hop * (Fmax + 2 * pad), dtype=torch.float32, device=plan.device)
+        live = [b for b in range(B) if F[b] > 0]
+        for n, (ids, w) in PS.vocode(self, mel, live, [F[b] for b in live], guard).items():
+            if len(ids) == B:
+                wav = w
+            else:
+                wav[torch.tensor(ids, device=plan.device), :, :w.shape[-1]] = w
+        wav_lens = [hop * (f + 2 * pad) for f in F]
+        if return_intermediates:
+            return dict(wav=wav, wav_lens=wav_lens, mel=mel, frame_offsets=torch.tensor(offsets, dtype=torch.int64),
+                        context_rows_used=torch.tensor(used, dtype=torch.int64), sentences=sents)
+        return (wav, wav_lens) if return_lengths else wav
+
+    def synthesize_passage_stream(self, sentences, mels, pause_frames=0, context_rows: int = 128, plm_context=None,
+                                  forced_durations=None, duration_scale=None, sampling: S.Sampling = None, keys=None,
+                                  check_range: bool = True, **rejected):
+        """``synthesize_passage`` as a generator of chunks, one per sentence; every argument is checked before the first
+        ``next``.  Chunk i holds each row's samples of the pause before sentence i and of sentence i (the first chunk
+        also the vocoder's leading padding, the last its trailing padding), from a vocoder window with a halo of
+        ``hifi_gan.generator.receptive_field()`` frames on each side.  It is yielded as soon as the passage mel covers
+        its window in every row: right after sentence i when the pause after it is at least the halo in every row,
+        else after sentence i + 1.  Each chunk is a dict: ``wav`` (B, 1, n), ``offset`` and ``valid`` (per row: where
+        its samples start in ``synthesize_passage``'s waveform, and how many of the chunk's first samples are that
+        row's; the rest are zeros), ``sentence`` (i) and ``last``; the last chunk also has ``wav_lens``, ``mel`` and
+        ``frame_offsets``.  Rows whose windows are equal share one vocoder batch.  Put together, the chunks are
+        ``synthesize_passage``'s waveform within rounding (a window can take another tensor-core plan than the whole
+        passage); codes, durations and mel are the same bit for bit.  ``check_range`` redoes a sentence or a chunk's
+        vocoder launches on bf16x3, as ``synthesize_passage`` does."""
+        plan = self._passage_plan(sentences, mels, pause_frames, context_rows, plm_context, forced_durations,
+                                  duration_scale, sampling, keys, rejected)
+        return self._passage_stream(plan, check_range and _fp16_operands())
+
+    def _passage_plan(self, sentences, mels, pause_frames, context_rows, plm_context, forced_durations, duration_scale,
+                      sampling, keys, rejected):
+        return PS.PassagePlan(sentences, mels, pause_frames, context_rows, plm_context, forced_durations,
+                              duration_scale, sampling, keys, self.plm.vq_bins, self.plm.tc_latent_dim,
+                              self.generator.mrte.mel_bins, rejected)
+
+    def _passage_stream(self, plan, guard):
+        import contextlib
+        B, S_, dev = plan.B, plan.S, plan.device
+        hop, pad = HIFIGAN_HOP_LENGTH, self.hifi_gan.generator.cfg["inference_padding"]
+        hv = self.hifi_gan.generator.receptive_field()
+        pm = PS.PassageMel(B, self.generator.mrte.mel_bins, dev)
+        totals, nxt = [], 0
+
+        def chunk(i, final):
+            """chunk i, or None while its window is not covered in every row"""
+            offsets, F = PS.frame_offsets(totals + [[0] * B] * (S_ - len(totals)), plan.pauses)
+            bounds = PS.chunk_bounds(offsets, totals + [[0] * B] * (S_ - len(totals)), F, i, pad)
+            wins = [PS.vocoder_window(p0, p1, pad, hv, pm.f[b], final) for b, (p0, p1) in enumerate(bounds)]
+            if any(w is None for b, w in enumerate(wins) if bounds[b][1] > bounds[b][0]):
+                return None
+            valid = [hop * max(p1 - p0, 0) for p0, p1 in bounds]
+            wav = torch.zeros(B, 1, max(valid), dtype=torch.float32, device=dev)
+            groups = {}
+            for b, ((p0, p1), w) in enumerate(zip(bounds, wins)):
+                if p1 > p0 and w[1] > w[0]:
+                    groups.setdefault((p0, p1) + w, []).append(b)
+            redo = False
+            while True:
+                with pack.engine_scope(pack.ENGINE_BF16X3) if redo else contextlib.nullcontext():
+                    for (p0, p1, va, vb), ids in groups.items():
+                        idx = slice(None) if len(ids) == B else torch.tensor(ids, device=dev)
+                        w = self.hifi_gan.decode_batch_cl(pm.buf[idx, va:vb])
+                        wav[idx, :, :hop * (p1 - p0)] = w[:, :, hop * (p0 - va):hop * (p1 - va)]
+                if redo or not (guard and ops.tc_overflow(dev)):
+                    break
+                _warn_fp16_range(f"re-running the vocoder of chunk {i} of this passage on the bf16x3 engine")
+                redo = True
+            out = dict(wav=wav, offset=[hop * p0 for p0, _ in bounds], valid=valid, sentence=i, last=i == S_ - 1)
+            if i == S_ - 1:
+                out.update(wav_lens=[hop * (f + 2 * pad) for f in F], mel=pm.buf[:, :max(F)],
+                           frame_offsets=torch.tensor(offsets, dtype=torch.int64))
+            return out
+
+        for i, (out, _) in enumerate(PS.run_sentences(self, plan, guard)):
+            with torch.no_grad():
+                pm.place(out["mel"], out["totals"], [p[i] for p in plan.pauses] if i < S_ - 1 else None)
+            totals.append(out["totals"])
+            while nxt <= i:
+                with torch.no_grad():
+                    c = chunk(nxt, i == S_ - 1)
+                if c is None:
+                    break
+                yield c
+                nxt += 1
 
     @torch.no_grad()
     def synthesize_many(self, items, max_batch: int = 64, sampling: S.Sampling = None, **kw):

@@ -74,28 +74,39 @@ class MRTE(nn.Module):
         self.activation = nn.ReLU()
         self.length_regulator = LengthRegulator(mel_frames, sample_rate, duration_token_ms)
 
-    def tc_latent(self, phone: torch.Tensor, *args):
+    def encode_prompt(self, mel: torch.Tensor) -> torch.Tensor:
+        """The mel encoder's output for a prompt mel (B, Tm, mel_bins) -> (B, ceil(Tm / 16), hidden) channels-last: what
+        ``tc_latent`` attends to.  Passing it back as ``mel_context=`` gives the same latent bit for bit without encoding
+        the prompt again (long-form synthesis encodes its prompt once per passage)."""
+        if self.training:
+            raise L.MttsError("training-mode dropout is outside the synthesis path (call .eval())")
+        return self.mel_encoder.forward_cl(mel)
+
+    def tc_latent(self, phone: torch.Tensor, *args, mel_context: torch.Tensor = None):
         """tc_latent(phone (B,Tp) int64, mel (B,Tm,mel_bins)) -> (B,Tp,hidden), >= 0  (mrte.py:154-171).
         Also accepts tc_latent(phone, phone_lens, mel): phone_lens is ignored, exactly like the
-        unmasked reference computation."""
-        mel = args[-1]
+        unmasked reference computation.  ``mel_context``: ``encode_prompt(mel)``, computed earlier; the mel argument
+        is then not read."""
+        mel = args[-1] if args else None
         if self.training:
             raise L.MttsError("training-mode dropout is outside the synthesis path (call .eval())")
         pe = self.phone_pos_embedding
         pe.extend_pe(phone)
         # embedding gather + alpha * sine PE in one kernel (mrte.py:159-160)
         x = ops.embed_pe(phone, self.phone_embedding.word_embeddings.weight.detach(), pe.pe, pe.alpha_host())
-        mel_context = self.mel_encoder.forward_cl(mel)             # (B, Tm/16, H), already channels-last
+        if mel_context is None:
+            mel_context = self.mel_encoder.forward_cl(mel)         # (B, Tm/16, H), already channels-last
         phone_x = self.phone_encoder(x)
         y = self.mha(phone_x, kv=mel_context)
         # LayerNorm -> ReLU fused (mrte.py:168-169)
         return ops.layernorm(y, self.norm.weight.detach(), self.norm.bias.detach(), eps=self.norm.eps,
                              post_act=L.ACT_RELU, out=y)
 
-    def attend(self, phone: torch.Tensor, mels) -> torch.Tensor:
+    def attend(self, phone: torch.Tensor, mels, mel_context=None) -> torch.Tensor:
         """The pre-norm attention outputs of K mels: phone (B,Tp) int64, ``mels`` K tensors (B, Tm_k, mel_bins) ->
         ys (K, B, Tp, hidden), ys[k] = MHA(phone_x, kv=mel_encoder(mels[k])), the y of ``tc_latent(phone, mels[k])`` bit
-        for bit.  The phone encoder runs once; each mel runs its mel encoder and the MHA."""
+        for bit.  The phone encoder runs once; each mel runs its mel encoder and the MHA.  ``mel_context``: a list of K
+        entries, each ``encode_prompt(mels[k])`` or None; a given entry replaces that mel's encoder pass."""
         if self.training:
             raise L.MttsError("training-mode dropout is outside the synthesis path (call .eval())")
         pe = self.phone_pos_embedding
@@ -104,7 +115,8 @@ class MRTE(nn.Module):
         phone_x = self.phone_encoder(x)
         ys = torch.empty(len(mels), *phone_x.shape, dtype=torch.float32, device=phone_x.device)
         for k, mel in enumerate(mels):
-            self.mha(phone_x, kv=self.mel_encoder.forward_cl(mel), out=ys[k])
+            ctx = None if mel_context is None else mel_context[k]
+            self.mha(phone_x, kv=self.mel_encoder.forward_cl(mel) if ctx is None else ctx, out=ys[k])
         return ys
 
     def norm_relu(self, y: torch.Tensor) -> torch.Tensor:

@@ -411,6 +411,54 @@ def mask_tail(x, keep):
     return x
 
 
+def copy_row_segments(dst, dst_off, n, src=None, src_off=None, fill=None):
+    """Ragged row copy in one launch (include/megatts2_b200.h, mtts_copy_row_segments): for each batch row b,
+    ``dst[b, dst_off[b] + r] = src[b, src_off[b] + r]`` for r < n[b], or ``fill`` (a float for fp32 rows) in every element
+    without ``src``.  dst and src are (B, rows, ...) device tensors of one dtype whose rows are contiguous (src may be
+    (1, rows, ...), broadcast to every b); the tables are host ints, uploaded with the copy (no host sync).  Rows that
+    would fall outside either tensor are not copied.  -> dst."""
+    if (src is None) == (fill is None) or (src is None) != (src_off is None):
+        raise L.MttsError("copy_row_segments: give src and src_off, or fill")
+    if not isinstance(dst, torch.Tensor) or dst.dim() < 2:
+        raise L.MttsError("copy_row_segments: dst must be a (B, rows, ...) CUDA tensor")
+    _dev(dst, dst.dtype, "dst")
+    B, row_elems = dst.shape[0], math.prod(dst.shape[2:])
+    row_bytes = row_elems * dst.element_size()
+
+    def rows_of(t, name):
+        if t.dim() < 2 or tuple(t.shape[2:]) != tuple(dst.shape[2:]) or t.dtype != dst.dtype or t.device != dst.device:
+            raise L.MttsError(f"copy_row_segments: {name} {tuple(t.shape)} {t.dtype} does not match dst "
+                              f"{tuple(dst.shape)} {dst.dtype}")
+        if math.prod(t.shape[2:]) > 1 and not t[0, 0].is_contiguous():
+            raise L.MttsError(f"copy_row_segments: {name}'s rows must be contiguous")
+        es = t.element_size()
+        st = t.stride(1) * es if t.shape[1] > 1 else row_bytes
+        return (0 if t.shape[0] == 1 else t.stride(0) * es), st, t.shape[1]
+
+    d_sb, d_st, d_rows = rows_of(dst, "dst")
+    tables = [list(dst_off), list(n)] + ([] if src is None else [list(src_off)])
+    if any(len(t) != B for t in tables):
+        raise L.MttsError(f"copy_row_segments: every table needs B = {B} entries")
+    n_max = max(tables[1], default=0)
+    if src is not None:
+        if src.shape[0] not in (1, B):
+            raise L.MttsError(f"copy_row_segments: src has {src.shape[0]} batch rows, expected 1 or {B}")
+        s_sb, s_st, s_rows = rows_of(src, "src")
+        fill_word = 0
+    else:
+        if dst.element_size() != 4:
+            raise L.MttsError("copy_row_segments: fill needs a 4-byte dtype")
+        s_sb, s_st, s_rows = 0, row_bytes, 0
+        fill_word = int(torch.tensor([fill], dtype=dst.dtype).view(torch.int32)[0]) & 0xFFFFFFFF
+    if B == 0 or n_max <= 0:
+        return dst
+    tab = torch.tensor(tables, dtype=torch.int32).to(dst.device, non_blocking=True)    # one upload, no host sync
+    L.check(L.lib().mtts_copy_row_segments(_ptr(src), s_sb, s_st, s_rows, _ptr(dst), d_sb, d_st, d_rows, row_bytes,
+                                           _ptr(tab[2]) if src is not None else None, _ptr(tab[0]), _ptr(tab[1]), B,
+                                           n_max, fill_word, _stream()))
+    return dst
+
+
 def to_channels_last(x_bct, pad_rep=0):
     """(B, C, T) any strides -> contiguous (B, T + 2*pad_rep, C)."""
     x = _dev(x_bct, name="x")
